@@ -1,6 +1,6 @@
-# Builds libctr_b200.so (sm_100a only) in-tree; `python -c "import __graft_entry__ as g; g.build()"` calls this.
+# Builds libctr_b200.so (sm_90a, H100) in-tree; `python -c "import __graft_entry__ as g; g.build()"` calls this.
 NVCC      ?= nvcc
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVCCFLAGS := -O3 -std=c++17 -lineinfo $(ARCH) -Xcompiler -fPIC,-Wall,-Wno-unused-function -Xptxas -v
 SRC_DIR   := tf_repos_b200/csrc
 SRCS      := $(wildcard $(SRC_DIR)/*.cu)

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Drop-in for deep_ctr/Model_pipeline/DCN.py on the B200 engine (flags: DCN.py:29-58, incl. --cross_layers)."""
+"""Drop-in for deep_ctr/Model_pipeline/DCN.py on the H100 engine (flags: DCN.py:29-58, incl. --cross_layers)."""
 import os
 import sys
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Drop-in for deep_ctr/Model_pipeline/DIN.py on the B200 engine: same flags (DIN.py:26-54), TFRecord input
+"""Drop-in for deep_ctr/Model_pipeline/DIN.py on the H100 engine: same flags (DIN.py:26-54), TFRecord input
 (`data_dir/tr/*tfrecord`, `data_dir/te/*tfrecord`), task types {train, eval, infer, export}, e.g.
   python Model_pipeline/DIN.py --task_type=train --field_size=11 --feature_size=1000000 --embedding_size=32 \
       --batch_size=1024 --num_epochs=1 --model_dir=./model_ckpt/aliccp/DIN/ --data_dir=./data/aliccp/"""

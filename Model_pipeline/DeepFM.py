@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Drop-in for deep_ctr/Model_pipeline/DeepFM.py on the B200 engine: same flags (DeepFM.py:34-60), same
+"""Drop-in for deep_ctr/Model_pipeline/DeepFM.py on the H100 engine: same flags (DeepFM.py:34-60), same
 libsvm input, same task types.  e.g.
   python Model_pipeline/DeepFM.py --task_type=train --learning_rate=0.0005 --optimizer=Adam --num_epochs=1 \
       --batch_size=256 --field_size=39 --feature_size=117581 --deep_layers=400,400,400 --dropout=0.5,0.5,0.5 \

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Drop-in for deep_ctr/Model_pipeline/PNN.py on the B200 engine (same flags and per-model defaults)."""
+"""Drop-in for deep_ctr/Model_pipeline/PNN.py on the H100 engine (same flags and per-model defaults)."""
 import os
 import sys
 

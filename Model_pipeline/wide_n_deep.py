@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Drop-in for deep_ctr/Model_pipeline/wide_n_deep.py on the B200 engine: same flags (wide_n_deep.py:21-47), same
+"""Drop-in for deep_ctr/Model_pipeline/wide_n_deep.py on the H100 engine: same flags (wide_n_deep.py:21-47), same
 CSV input (tr*csv / va*csv / te*csv, 40 columns), same task types {train, predict, export_model}, e.g.
   python Model_pipeline/wide_n_deep.py --model_type=wide_n_deep --num_epochs=1 --batch_size=128 \
       --model_dir=./model_ckpt/criteo/wide_n_deep/ --data_dir=./data/criteo/"""

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- DeepFM training samples/sec on Criteo-39-field synthetic data (BASELINE.json metric).
 
-  python bench.py --gpus N --steps K --warmup W            our arm (B200, libctr_b200.so)
+  python bench.py --gpus N --steps K --warmup W            our arm (H100, libctr_b200.so)
   python bench.py --impl reference --gpus N --steps K ...  the reference's CPU path (oracle port:
                                                             TensorFlow is not installable here)
 
@@ -16,6 +16,9 @@ lazily, one pass over HBM per 16 steps.  `exact_every_step` reports the plain HB
 `e2e`     : same steps fed from pinned HOST buffers through the public API, loss read back per step.
 `lazy`    : the same step when only gathered rows are updated (NOT the reference's result; reported
             for context, never as the headline).
+--dump-outputs DIR writes what the last timed step computed (loss terms, then every variable after the flush;
+a fixed seeded sample of the rows of each embedding table) as DIR/<name>.npy, so that two builds can be
+compared output for output on identical inputs.
 """
 from __future__ import annotations
 
@@ -52,6 +55,8 @@ def parse():
     ap.add_argument("--tables", default="auto", choices=["auto", "replicated", "sharded"],
                     help="N>1: 'sharded' = rows owned by id %% N, NCCL all-to-all exchange (default); "
                          "'replicated' = data parallel with all-gathered sparse gradients")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's outputs as DIR/<name>.npy (rank 0)")
     return ap.parse_args()
 
 
@@ -60,7 +65,7 @@ def peaks():
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s, not measured)"
 
 
 class ClockSampler(threading.Thread):
@@ -227,6 +232,46 @@ EPOCH = int(os.environ.get("CTR_BENCH_EPOCH", "16"))  # steps per epoch of the e
 # reported configuration, the override exists for the epoch-length trade-off measurement in DESIGN.md §6
 
 
+DUMP_TABLE_ROWS = 65536  # rows of each embedding table written by --dump-outputs (fixed seeded sample)
+
+
+def dump_outputs(dirname, model, parts):
+    """The arrays a caller of the timed path receives after its last step: the loss terms train_step returned and the
+    variables (flushed).  Embedding tables contribute the same seeded sample of rows in every run; <= ~10 MB in all."""
+    import numpy as np
+    import torch
+    os.makedirs(dirname, exist_ok=True)
+    out = {"loss_parts": parts}
+    if hasattr(model, "variables"):
+        for name, t in model.variables().items():
+            if t.dim() == 2 and t.shape[0] > DUMP_TABLE_ROWS:
+                g = torch.Generator().manual_seed(0)
+                rows = torch.randint(t.shape[0], (DUMP_TABLE_ROWS,), generator=g).sort().values
+                t = t[rows.to(t.device)]
+            elif t.dim() == 1 and t.shape[0] > DUMP_TABLE_ROWS:
+                g = torch.Generator().manual_seed(1)
+                rows = torch.randint(t.shape[0], (DUMP_TABLE_ROWS,), generator=g).sort().values
+                t = t[rows.to(t.device)]
+            out[name.replace("/", "__")] = t
+    for name, t in out.items():
+        a = t.detach().cpu()
+        a = a.numpy() if a.dtype in (torch.float32, torch.float64) else a.float().numpy()
+        np.save(os.path.join(dirname, name + ".npy"), a)
+
+
+def device_info(torch, dev):
+    """The card a number was measured on: its name and the power limit it ran under (NVML; None if unavailable)."""
+    info = {"name": torch.cuda.get_device_name(dev), "power_limit_w": None}
+    try:
+        import pynvml
+        pynvml.nvmlInit()
+        h = pynvml.nvmlDeviceGetHandleByIndex(dev.index)
+        info["power_limit_w"] = pynvml.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0
+    except Exception:
+        pass
+    return info
+
+
 def main_b200(args):
     import torch
     import torch.distributed as dist
@@ -279,9 +324,11 @@ def main_b200(args):
             return model.train_step_graphed(ids, vals, labels)
         return model.train_step(ids, vals, labels)
 
+    last_parts = [None]
+
     def step_dev(i):
         ids, vals, labels = devb[i % N_BATCHES]
-        train(ids, vals, labels)
+        last_parts[0] = train(ids, vals, labels)
 
     counts = {}
     step_exact_marker = object()
@@ -326,6 +373,8 @@ def main_b200(args):
     sampler.start()
     ms_total = timed(step_dev, args.steps, args.warmup, finish=model.flush)
     sampler.stop_flag = True
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, model, last_parts[0])
     launches = counts["launches"]
     sweep_ms = [a.elapsed_time(b) for a, b in model.updater.sweep_events]
     sweep_steps = list(model.updater.sweep_steps)
@@ -524,7 +573,7 @@ def main_b200(args):
                     "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 12 + 8, "last_loss": last_loss,
                     "sweep_avg_ms": (sum(e2e_sweep_ms) / len(e2e_sweep_ms) if e2e_sweep_ms else None),
                     "clocks": sampler2.summary()},
-            "gpu_launches": launches, "clocks": sampler.summary(),
+            "gpu_launches": launches, "clocks": sampler.summary(), "device": device_info(torch, dev),
             "roofline": {"kernel": f"epoch_sweep_adam_kernel on fm_v ({EPOCH} Adam steps per element per pass; CUDA events around the pass incl. the ~1 ms second pass over the rows gathered during the epoch)",
                          "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
                          "frac": (achieved / peak if achieved else None), "traffic": traffic,
@@ -541,9 +590,7 @@ def main_b200(args):
                          "fma_pipe_active_pct_ncu": (json.load(open(os.path.join(ROOT, "profiles", "sweep_traffic.json"))).get("epoch_fma_pipe_active_pct") if os.path.exists(os.path.join(ROOT, "profiles", "sweep_traffic.json")) else None),
                          "note": "by design NOT HBM-bound: the pass replays 16 optimizer steps per element in registers (IEEE "
                                  "div+sqrt recurrence: 21 fp32 operations + 2 MUFU per element-step, bit-identical to the every-step "
-                                 "formulation) to cut HBM traffic 16x; its limiter is instruction issue on the packed fp32 pipe "
-                                 "(FFMA2-class instructions hold the port 2 cycles: profiles/r02_ubench_f32x2.txt, "
-                                 "profiles/r02_ncu_sweep_adam_packed.txt).  `frac` is computed from full 16-step passes only; the "
+                                 "formulation) to cut HBM traffic 16x; its limiter is instruction issue.  `frac` is computed from full 16-step passes only; the "
                                  "flush that ends the timed region is listed under partial_passes.  The HBM-bound formulation of the "
                                  "same update is reported under exact_every_step; the same steps from the long-run (parked) table "
                                  "state under steady_state."}}
@@ -609,7 +656,7 @@ def side_models(torch, dev, synth, vocab):
         m = DCN(F, vocab, K, B, cross_layers=L, update_mode="exact_deferred", epoch_steps=EPOCH, device=dev)
         ms = timeit(lambda i: m.train_step_graphed(*bt[i % 8]), m, 2 * EPOCH, graphed=True)
         out["configs[2]_dcn"] = {"value": B / ms * 1e3, "unit": "samples/s", "ms_per_step": ms,
-                                 "config": f"DCN 1xB200, B={B} F={F} vocab={vocab} k={K} cross_layers={L}, Adam, l2 1e-4, "
+                                 "config": f"DCN 1xH100, B={B} F={F} vocab={vocab} k={K} cross_layers={L}, Adam, l2 1e-4, "
                                            "dropout 0.5, exact TF update semantics (exact-deferred)"}
         del m, bt
         torch.cuda.empty_cache()
@@ -625,7 +672,7 @@ def side_models(torch, dev, synth, vocab):
         m = DIN(Fp, N, K, B, P, max_a_int=8, update_mode="exact_deferred", epoch_steps=EPOCH, device=dev)
         ms = timeit(lambda i: m.train_step(*bt[i % 4]), m, EPOCH)
         out["configs[3]_din"] = {"value": B / ms * 1e3, "unit": "samples/s", "ms_per_step": ms,
-                                 "config": f"DIN 1xB200, B={B} F'={Fp} seq_len={P} (lengths ~U[1,100]) items={N} k={K}, "
+                                 "config": f"DIN 1xH100, B={B} F'={Fp} seq_len={P} (lengths ~U[1,100]) items={N} k={K}, "
                                            "attention hidden 256, Adam, l2 1e-4, dropout 0.5, exact-deferred update"}
         del m, bt
         torch.cuda.empty_cache()

@@ -1,5 +1,5 @@
 /*
- * ctr_b200.h -- C ABI of libctr_b200.so, the B200 (sm_100a) CTR feature-interaction engine.
+ * ctr_b200.h -- C ABI of libctr_b200.so, the H100 (sm_90a) CTR feature-interaction engine.
  *
  * This is the drop-in boundary for the hot path of lambdaji/tf_repos'
  * deep_ctr/Model_pipeline/*.py `model_fn`s.  The reference has no FFI of its own (it is
@@ -54,7 +54,7 @@ int ctr_abi_version(void);
 const char* ctr_last_error(void);
 /* number of kernels this library has launched in this process (bench.py's gpu_launches) */
 int64_t ctr_launch_count(void);
-/* number of SMs the library sized its persistent grids for (148 on B200); <0 on error */
+/* number of SMs the library sized its persistent grids for (132 on H100 SXM); <0 on error */
 int ctr_device_sm_count(void);
 
 /* ---- K1: gather + scale + FM first/second order + emit x ------------------------------------

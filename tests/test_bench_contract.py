@@ -57,8 +57,8 @@ def test_reference_arm_maps_no_product_code():
 def test_committed_bench_line_roofline_reproduces_from_its_own_numbers():
     """`frac` must follow from algorithmic bytes / avg launch duration / peak, computed from full 16-step passes only."""
     import glob
-    paths = sorted(glob.glob(os.path.join(ROOT, "profiles", "r02_bench_n1_final*.json")))
-    assert paths, "no committed round-2 bench line"
+    paths = sorted(glob.glob(os.path.join(ROOT, "profiles", "bench_n1_h100*.json")))
+    assert paths, "no committed bench line"
     for p in paths:
         d = json.loads([l for l in open(p) if l.startswith("{")][-1])
         r = d["roofline"]

@@ -120,7 +120,7 @@ dist.destroy_process_group()
 '''
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 @pytest.mark.parametrize("mode", ["exact", "exact_deferred", "lazy"])
 def test_sharded_two_ranks_equal_single_engine(tmp_path, mode):
     script = tmp_path / "w.py"

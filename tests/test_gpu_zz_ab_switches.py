@@ -68,7 +68,7 @@ def test_switch_leaves_every_bit_unchanged(default_run, env):
     assert d["hash"] == default_run["hash"] and d["losses"] == default_run["losses"]
 
 
-@pytest.mark.parametrize("env", [{"CTR_GEMM_WS": "0"}, {"CTR_GEMM": "simt"}],
+@pytest.mark.parametrize("env", [{"CTR_GEMM": "simt"}],
                          ids=lambda e: ",".join(f"{k}={v}" for k, v in e.items()))
 def test_gemm_switch_within_fp32_tolerance(default_run, env):
     d = _run(env)

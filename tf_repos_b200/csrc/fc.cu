@@ -1,9 +1,6 @@
 // fc.cu -- the dense 'Deep-part': fully_connected layers (DeepFM.py:152-167), forward and backward,
-// fp32 SIMT with fused epilogues (bias + relu + dropout; dZ + bias-gradient).
-//
-// Why fp32 SIMT and not tcgen05: the parity target is 1e-5 relative on the logits; TF32/BF16
-// tensor-core inputs lose 1e-3.  (A 3xTF32 split on tcgen05 is the planned upgrade; these GEMMs are
-// ~3 % of an exact-semantics step.)
+// with fused epilogues (bias + relu + dropout; dZ + bias-gradient).  The products run on the tensor cores
+// (tc_gemm.cu, 3xTF32); the fp32 SIMT tiles below are the CTR_GEMM=simt alternative.
 //
 // One templated tile kernel serves the three products of a layer:
 //   forward   out[M,N]  = act(in[M,K] @ W[K,N] + b)          (A reduce-contiguous, B row-contiguous)
@@ -249,7 +246,7 @@ __global__ void dropout_mask_kernel(float* __restrict__ mask, int64_t n, float k
   }
 }
 
-// tc_gemm.cu: the same products on tcgen05 tensor cores (3xTF32).  CTR_GEMM=simt selects the SIMT tiles.
+// tc_gemm.cu: the same products on wgmma tensor cores (3xTF32).  CTR_GEMM=simt selects the SIMT tiles.
 int tc_gemm_dispatch(int kind, int epi, const float* A, int lda, const float* B, int ldb, float* C, int ldc, int M, int N,
                      int R, int S, const float* bias, int act, const float* mask, float keep, const float* gbias, int gP,
                      cudaStream_t st);

@@ -400,8 +400,7 @@ static int launch_fwd(const void* ids, const float* vals, const float* V, const 
                       int32_t* oob, cudaStream_t st) {
   const int wpb = 4;
   dim3 grid((B + wpb - 1) / wpb), block(wpb * 32);
-  // measured on B200 (profiles/r02_k1_tma_vs_ldg.txt): bulk copies lose at 64 B rows (1.59x), tie at 128-256 B
-  // (1.04-1.09x) and win at 512 B rows (0.92x) => default: TMA staging for K == 128 only; CTR_FM_EMBED_TMA=0/1 forces
+  // bulk copies pay off only for long rows => default: TMA staging for K == 128 (512 B rows) only; CTR_FM_EMBED_TMA=0/1 forces
   static int use_tma = -2;
   if (use_tma == -2) { const char* e = getenv("CTR_FM_EMBED_TMA"); use_tma = e ? atoi(e) : -1; }
   const bool tma = use_tma == 1 || (use_tma == -1 && K == 128);

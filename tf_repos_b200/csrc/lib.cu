@@ -20,9 +20,9 @@ int sm_count() {
   static int cached = 0;
   if (cached > 0) return cached;
   int dev = 0, n = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-    return 148;
+    return 132;
   cached = n;
   return n;
 }

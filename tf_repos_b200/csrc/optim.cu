@@ -100,7 +100,7 @@ opt_patch_rows_kernel(float* __restrict__ var, float* __restrict__ slot0, float*
 constexpr int SWEEP_THREADS = 256;
 
 // UNROLL float4 triples in flight per thread; MINB = resident CTAs per SM the register budget is
-// squeezed for (tuned on B200, see profiles/): the kernel is a pure stream, so what matters is bytes
+// squeezed for: the kernel is a pure stream, so what matters is bytes
 // in flight per SM = MINB * 256 threads * UNROLL * 48 B.
 template <int OPT, int SWEEP_UNROLL, int MINB>
 __global__ void __launch_bounds__(SWEEP_THREADS, MINB)

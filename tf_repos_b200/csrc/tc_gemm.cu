@@ -1,21 +1,21 @@
-// tc_gemm.cu -- the dense GEMMs of the MLP / attention layers on the 5th-generation tensor cores
-// (tcgen05.mma, accumulators in TMEM), at fp32-class accuracy through a 3xTF32 split.
+// tc_gemm.cu -- the dense GEMMs of the MLP / attention layers on the Hopper tensor cores (wgmma, fp32
+// accumulators in registers), at fp32-class accuracy through a 3xTF32 split.
 //
 // Why 3xTF32: the parity target is 1e-5 relative on the logits; a plain TF32 (10-bit mantissa) or
 // BF16 product loses 1e-3.  Each fp32 operand is split on the fly into hi = rn_tf32(a) and
 // lo = a - hi (exact); D += A_lo*B_hi + A_hi*B_lo + A_hi*B_hi on the tensor cores recovers ~2^-21
-// relative accuracy with fp32 accumulation in TMEM, at 1/3 of the TF32 rate (still ~5x the fp32
+// relative accuracy with fp32 accumulation, at 1/3 of the TF32 rate (still several times the fp32
 // SIMT pipe).
 //
-// Structure of one CTA (128 threads, one 128 x BN output tile, BN <= 128):
-//   loop over 32-wide reduction slices, 2-stage ring (1 stage when the reduction is a single slice):
-//     all threads : registers (loaded one slice ahead, coalesced for either operand orientation)
-//                   -> hi/lo split -> st.shared in the canonical K-major SWIZZLE_128B UMMA layout
-//                   fence.proxy.async ; __syncthreads ; issue the NEXT slice's global loads
-//     thread 0    : 4 k-steps x 3 tcgen05.mma.cta_group::1.kind::tf32 (M=128, N=BN, K=8) ;
-//                   tcgen05.commit -> mbarrier of the stage (frees it for the refill two slices later)
-//   epilogue      : tcgen05.ld 32x32b (thread t owns accumulator row t) -> staging tile in shared memory ->
-//                   whole rows per warp: bias / group bias / relu / dropout / accumulate -> 512 B coalesced stores
+// Structure of one CTA (256 threads = two warpgroups, one 128 x BN output tile, BN in {32, 64, 128}):
+//   loop over 32-wide reduction slices, 2-stage shared-memory ring (1 stage when the reduction is one slice):
+//     all threads  : registers (loaded one slice ahead, coalesced for either operand orientation)
+//                    -> hi/lo split -> st.shared in the canonical K-major SWIZZLE_128B layout
+//                    fence.proxy.async ; __syncthreads ; issue the NEXT slice's global loads
+//     warpgroup w  : rows 64w..64w+63: 4 k-steps x 3 wgmma.m64nBNk8.tf32 ; commit ; wait
+//                    (the stage is refilled two slices later, after every warpgroup has waited on it)
+//   epilogue       : accumulator fragments -> staging tile in shared memory ->
+//                    whole rows per warp: bias / group bias / relu / dropout / accumulate -> 512 B coalesced stores
 // Operands are staged by plain loads rather than TMA because the three products of a layer need
 // three different operand orientations of fp32 data that must be split anyway.
 #include <stdlib.h>
@@ -24,58 +24,73 @@
 
 namespace ctr {
 
-constexpr int TC_BM = 128, TC_BK = 32;
+constexpr int TC_BM = 128, TC_BK = 32, TC_THREADS = 256;
 constexpr int TC_TILE_BYTES = TC_BM * TC_BK * 4;            // 16 KB: one 128 x 32 fp32 operand tile
 constexpr int TC_STAGE_BYTES = 4 * TC_TILE_BYTES;           // A_hi, A_lo, B_hi, B_lo
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "WAIT_LOOP:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra DONE;\n\t"
-      "bra WAIT_LOOP;\n\t"
-      "DONE:\n\t"
-      "}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor):
+// K-major, SWIZZLE_128B shared-memory matrix descriptor (sm_90 wgmma):
 //   start_address[0,14) = addr>>4 ; LBO[16,30) = 1 (unused for swizzled K-major) ; SBO[32,46) = 1024 B >> 4
-//   version[46,48) = 1 (sm_100) ; layout_type[61,64) = 2 (SWIZZLE_128B)
+//   layout_type[62,64) = 1 (SWIZZLE_128B)
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
 
-// instruction descriptor (cute::UMMA::InstrDescriptor): D fp32, A/B tf32, both K-major
-__device__ __forceinline__ uint32_t make_idesc(int M, int N) {
-  uint32_t d = 0;
-  d |= 1u << 4;                      // c_format  = F32
-  d |= 2u << 7;                      // a_format  = TF32
-  d |= 2u << 10;                     // b_format  = TF32
-  d |= (uint32_t)(N >> 3) << 17;     // n_dim
-  d |= (uint32_t)(M >> 4) << 24;     // m_dim
-  return d;
-}
+// D[64 x N] += A[64 x 8] * B[8 x N], both operands K-major in shared memory, fp32 accumulators in registers:
+// thread t of the warpgroup holds rows 16*(t/32) + (t%32)/4 (+8) and columns 8j + 2*(t%4) (+1), j < N/8
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc);
 
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+template <>
+__device__ __forceinline__ void wgmma_tf32<32>(float (&d)[16], uint64_t adesc, uint64_t bdesc) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+      "setp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(1));
+}
+
+template <>
+__device__ __forceinline__ void wgmma_tf32<64>(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(1));
+}
+
+template <>
+__device__ __forceinline__ void wgmma_tf32<128>(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(1));
+}
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving accesses of the accumulators across the asynchronous wgmma window
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
 __device__ __forceinline__ float tf32_hi(float x) {
@@ -89,18 +104,19 @@ __device__ __forceinline__ uint32_t sw128_off(int row, int chunk) {
   return (uint32_t)((row >> 3) * 1024 + (row & 7) * 128 + ((chunk ^ (row & 7)) << 4));
 }
 
+
 // ---- operand staging -----------------------------------------------------------------------------------------
-// One 128 x 32 fp32 operand tile = 8 float4 per thread.  RC (the reduction index is the contiguous one in
+// One 128 x 32 fp32 operand tile = 4 float4 per thread of the 256.  RC (the reduction index is the contiguous one in
 // global memory): a warp reads 4 rows x 128 B per instruction (8 lanes per row) -- coalesced -- and the same
 // (row, 16-byte chunk) assignment makes the swizzled shared-memory stores conflict-free.  !RC (the tile row
-// index is the contiguous one): thread t owns tile row t, consecutive threads read consecutive addresses.
+// index is the contiguous one): thread t owns tile row t%128 and half t/128 of the slice.
 template <bool RC>
-__device__ __forceinline__ void load_tile(float4 (&r)[8], const float* __restrict__ P, int ld, int row0, int n_rows,
-                                          int r0, int r_end, int tid) {
+__device__ __forceinline__ void load_tile(float4 (&r)[4], const float* __restrict__ P, int ld, int row0, int n_rows,
+                                             int r0, int r_end, int tid) {
   if (RC) {
-    const int sub = (tid & 31) >> 3, ch = tid & 7, wrow = (tid >> 5) * 32;
+    const int sub = (tid & 31) >> 3, ch = tid & 7, wrow = (tid >> 5) * 16;
 #pragma unroll
-    for (int it = 0; it < 8; ++it) {
+    for (int it = 0; it < 4; ++it) {
       const int g = row0 + wrow + it * 4 + sub, k0 = r0 + ch * 4;
       const float* p = P + (int64_t)g * ld + k0;
       if (g < n_rows && k0 + 4 <= r_end && ((((uintptr_t)p) & 15) == 0)) {
@@ -114,33 +130,51 @@ __device__ __forceinline__ void load_tile(float4 (&r)[8], const float* __restric
       }
     }
   } else {
-    const int g = row0 + tid;
+    const int g = row0 + (tid & 127), half = tid >> 7;
     const bool in = g < n_rows;
     const float* p = P + (int64_t)r0 * ld + g;
 #pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      r[c].x = (in && r0 + 4 * c < r_end) ? p[(int64_t)(4 * c) * ld] : 0.f;
-      r[c].y = (in && r0 + 4 * c + 1 < r_end) ? p[(int64_t)(4 * c + 1) * ld] : 0.f;
-      r[c].z = (in && r0 + 4 * c + 2 < r_end) ? p[(int64_t)(4 * c + 2) * ld] : 0.f;
-      r[c].w = (in && r0 + 4 * c + 3 < r_end) ? p[(int64_t)(4 * c + 3) * ld] : 0.f;
+    for (int c = 0; c < 4; ++c) {
+      const int cc = half * 4 + c;
+      r[c].x = (in && r0 + 4 * cc < r_end) ? p[(int64_t)(4 * cc) * ld] : 0.f;
+      r[c].y = (in && r0 + 4 * cc + 1 < r_end) ? p[(int64_t)(4 * cc + 1) * ld] : 0.f;
+      r[c].z = (in && r0 + 4 * cc + 2 < r_end) ? p[(int64_t)(4 * cc + 2) * ld] : 0.f;
+      r[c].w = (in && r0 + 4 * cc + 3 < r_end) ? p[(int64_t)(4 * cc + 3) * ld] : 0.f;
     }
   }
 }
 
-// hi/lo split + store into the K-major SWIZZLE_128B tiles
+// Interior tiles and full 32-wide slices (all of a layer but its edges): no bounds logic, pointers advanced by the
+// caller.  `base` already points at this thread's first element of slice 0 (RC: row (wrow+sub), 16 B chunk ch;
+// !RC: tile row tid&127, reduction index (tid>>7)*16); r0 is the slice's offset along the reduction.
 template <bool RC>
-__device__ __forceinline__ void store_tile(const float4 (&r)[8], uint8_t* hi_tile, uint8_t* lo_tile, int tid) {
-  const int sub = (tid & 31) >> 3, ch = tid & 7, wrow = (tid >> 5) * 32;
+__device__ __forceinline__ void load_tile_fast(float4 (&r)[4], const float* __restrict__ base, int ld, int r0) {
+  if (RC) {
+    const float* p = base + r0;
 #pragma unroll
-  for (int it = 0; it < 8; ++it) {
-    const int row = RC ? (wrow + it * 4 + sub) : tid;
-    const int chunk = RC ? ch : it;
+    for (int it = 0; it < 4; ++it) r[it] = __ldg(reinterpret_cast<const float4*>(p + (int64_t)(it * 4) * ld));
+  } else {
+    const float* p = base + (int64_t)r0 * ld;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      r[c].x = __ldg(p + (int64_t)(4 * c) * ld);
+      r[c].y = __ldg(p + (int64_t)(4 * c + 1) * ld);
+      r[c].z = __ldg(p + (int64_t)(4 * c + 2) * ld);
+      r[c].w = __ldg(p + (int64_t)(4 * c + 3) * ld);
+    }
+  }
+}
+
+// hi/lo split + store with the swizzled offsets precomputed once per thread (they do not depend on the slice)
+__device__ __forceinline__ void store_tile_fast(const float4 (&r)[4], uint8_t* hi_tile, uint8_t* lo_tile,
+                                                   const uint32_t (&off)[4]) {
+#pragma unroll
+  for (int it = 0; it < 4; ++it) {
     float4 hi, lo;
     hi.x = tf32_hi(r[it].x); hi.y = tf32_hi(r[it].y); hi.z = tf32_hi(r[it].z); hi.w = tf32_hi(r[it].w);
     lo.x = r[it].x - hi.x; lo.y = r[it].y - hi.y; lo.z = r[it].z - hi.z; lo.w = r[it].w - hi.w;
-    const uint32_t off = sw128_off(row, chunk);
-    *reinterpret_cast<float4*>(hi_tile + off) = hi;
-    *reinterpret_cast<float4*>(lo_tile + off) = lo;
+    *reinterpret_cast<float4*>(hi_tile + off[it]) = hi;
+    *reinterpret_cast<float4*>(lo_tile + off[it]) = lo;
   }
 }
 
@@ -148,7 +182,7 @@ constexpr int TC_STG_PITCH = TC_BM + 4;                          // epilogue sta
 constexpr int TC_STG_BYTES = TC_BM * TC_STG_PITCH * 4;
 constexpr int tc_smem_bytes(int stages) { return (stages * TC_STAGE_BYTES > TC_STG_BYTES ? stages * TC_STAGE_BYTES : TC_STG_BYTES) + 1024; }
 
-// ---- epilogue 2 (both kernels): NW warps write whole rows of the staged tile (lane l <-> columns 4l..4l+3, 512 B
+// ---- epilogue: NW warps write whole rows of the staged tile (lane l <-> columns 4l..4l+3, 512 B
 // coalesced): bias / group bias / relu / dropout (EPI 1), accumulate (EPI 2).  When a row needs a global read first
 // (dropout mask, old C) the reads of 4 rows are issued together: one dependent load per row made the masked forward of
 // DIN's attention layer latency-bound at 1.1 TB/s.
@@ -234,400 +268,110 @@ __device__ __forceinline__ void tc_epilogue_rows(const float* __restrict__ stg, 
 // C[i][j] = sum_r A(i,r) * B(r,j)
 //   A_RC: A(i,r) = A[i*lda + r] else A[r*lda + i];  B_RC: B(r,j) = B[j*ldb + r] else B[r*ldb + j]
 // EPI 0: store (split-R chunk z to C + z*M*ldc)  1: act(acc + bias + gbias[i/gP]) (/keep*mask)  2: C += acc
-// STAGES: depth of the operand ring (1 when the reduction fits one 32-wide slice: two CTAs per SM then)
-template <bool A_RC, bool B_RC, int EPI, int STAGES>
-__global__ void __launch_bounds__(128)
+// BN: tile width (32 / 64 only when the whole of N fits: narrow products do not pay for a 128-wide MMA)
+template <bool A_RC, bool B_RC, int EPI, int BN>
+__global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const float* __restrict__ A, int lda, const float* __restrict__ B, int ldb, float* __restrict__ C,
                int ldc, int M, int N, int R, const float* __restrict__ bias, int act, const float* __restrict__ mask,
                float keep, const float* __restrict__ gbias, int gP) {
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint64_t bar_stage[STAGES];
-  __shared__ uint32_t tmem_base_s;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // SWIZZLE_128B wants 1024 B alignment
-  const int i0 = blockIdx.y * TC_BM, j0 = blockIdx.x * TC_BM;
-  const int n_here = min(N - j0, TC_BM);
-  const int n_pad = (n_here + 15) & ~15;                       // UMMA_N: multiple of 16 for M = 128
-  const int r_chunk = (R + gridDim.z - 1) / gridDim.z;
-  const int r_begin = blockIdx.z * r_chunk, r_end = min(R, r_begin + r_chunk);
-  const int KT = (r_end - r_begin + TC_BK - 1) / TC_BK;
-
-  if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) mbar_init(&bar_stage[s], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {   // TMEM: 2 x 128 columns x 128 lanes of fp32 accumulators (main | small terms)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "r"(256));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  // the first slice's global loads fly while the TMEM allocation settles
-  float4 ra[8], rb[8];
-  if (KT > 0) {
-    load_tile<A_RC>(ra, A, lda, i0, M, r_begin, r_end, tid);
-    load_tile<B_RC>(rb, B, ldb, j0, N, r_begin, r_end, tid);
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_d = tmem_base_s;
-  const uint32_t idesc = make_idesc(TC_BM, n_pad);
-
-  for (int kt = 0; kt < KT; ++kt) {
-    const int s = kt % STAGES;
-    if (kt >= STAGES) {   // the MMAs that read this stage STAGES slices ago must be done
-      mbar_wait(&bar_stage[s], (uint32_t)(((kt / STAGES) - 1) & 1));
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    }
-    uint8_t* st = smem + s * TC_STAGE_BYTES;
-    store_tile<A_RC>(ra, st, st + TC_TILE_BYTES, tid);
-    store_tile<B_RC>(rb, st + 2 * TC_TILE_BYTES, st + 3 * TC_TILE_BYTES, tid);
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to the tensor core
-    __syncthreads();
-    if (kt + 1 < KT) {   // next slice: global -> registers while the tensor core works on this one
-      const int r0 = r_begin + (kt + 1) * TC_BK;
-      load_tile<A_RC>(ra, A, lda, i0, M, r0, r_end, tid);
-      load_tile<B_RC>(rb, B, ldb, j0, N, r0, r_end, tid);
-    }
-    if (tid == 0) {
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t a_hi = smem_u32(st), a_lo = a_hi + TC_TILE_BYTES, b_hi = a_hi + 2 * TC_TILE_BYTES, b_lo = a_hi + 3 * TC_TILE_BYTES;
-#pragma unroll
-      for (int k = 0; k < TC_BK / 8; ++k) {                        // UMMA_K = 8 tf32 = 32 bytes inside the 128 B swizzle atom
-        const uint32_t ko = k * 32;
-        // The tensor core accumulates in fp32 with truncation, so every accumulation costs ~2^-24 of the
-        // accumulator, with a bias.  The two cross terms (2^-11 of the result) go to their own accumulator:
-        // the main one then sees one accumulation per k-step instead of three.
-        const uint32_t first = (kt > 0 || k > 0) ? 1u : 0u;
-        umma_tf32(tmem_d + 128, make_desc(a_lo + ko), make_desc(b_hi + ko), idesc, first);
-        umma_tf32(tmem_d + 128, make_desc(a_hi + ko), make_desc(b_lo + ko), idesc, 1u);
-        umma_tf32(tmem_d, make_desc(a_hi + ko), make_desc(b_hi + ko), idesc, first);
-      }
-      asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&bar_stage[s])) : "memory");
-    }
-  }
-  if (KT > 0) {   // the last commit tracks every MMA issued before it
-    mbar_wait(&bar_stage[(KT - 1) % STAGES], (uint32_t)(((KT - 1) / STAGES) & 1));
-  }
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-
-  // ---- epilogue 1: TMEM -> registers (thread t <-> accumulator row t) -> staging tile in shared memory
-  // (the operand stages are free: every MMA that read them has completed)
-  float* stg = reinterpret_cast<float*>(smem);
-  for (int c0 = 0; c0 < n_pad; c0 += 16) {
-    uint32_t r[16], r2[16];
-    if (KT > 0) {
-      const uint32_t taddr = tmem_d + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0;
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-          : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-            "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-          : "r"(taddr));
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-          : "=r"(r2[0]), "=r"(r2[1]), "=r"(r2[2]), "=r"(r2[3]), "=r"(r2[4]), "=r"(r2[5]), "=r"(r2[6]), "=r"(r2[7]), "=r"(r2[8]),
-            "=r"(r2[9]), "=r"(r2[10]), "=r"(r2[11]), "=r"(r2[12]), "=r"(r2[13]), "=r"(r2[14]), "=r"(r2[15])
-          : "r"(taddr + 128));
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-      for (int q = 0; q < 16; ++q) r[q] = __float_as_uint(__uint_as_float(r[q]) + __uint_as_float(r2[q]));
-    } else {
-#pragma unroll
-      for (int q = 0; q < 16; ++q) r[q] = 0u;
-    }
-#pragma unroll
-    for (int q = 0; q < 16; q += 4)
-      *reinterpret_cast<uint4*>(stg + tid * TC_STG_PITCH + c0 + q) = make_uint4(r[q], r[q + 1], r[q + 2], r[q + 3]);
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"(256));
-
-  // ---- epilogue 2: a warp writes whole rows (lane l <-> columns 4l..4l+3): 512 B coalesced stores
-  float* Cz = C + (EPI == 0 ? (int64_t)blockIdx.z * M * ldc : 0);
-  tc_epilogue_rows<EPI, 4>(stg, Cz, ldc, M, N, i0, j0, n_here, warp, lane, bias, act, mask, keep, gbias, gP);
-}
-
-
-// ================================================================================================================
-// Warp-specialised variant (reductions of >= 3 slices): 8 producer warps, 1 MMA warp, 3-stage mbarrier ring.
-//   producers (warps 0-7, 256 threads): global -> registers (two slices ahead) -> hi/lo split -> swizzled st.shared
-//       -> fence.proxy.async -> arrive on full[s]; before refilling a stage they wait on empty[s]
-//   MMA warp (warp 8, one elected lane): wait full[s] -> 12 x tcgen05.mma (3xTF32, two accumulators) ->
-//       tcgen05.commit -> empty[s]; after the last slice a commit on accum_done
-//   epilogue: warps 0-3 drain TMEM (lane quarter = warp) into the staging tile, then all 8 producer warps write rows.
-// No __syncthreads inside the main loop: staging of slice k+1.. overlaps the tensor core working on slice k.
-// ================================================================================================================
-constexpr int WS_PROD = 256, WS_THREADS = WS_PROD + 32, WS_STAGES = 3, WS_PF = 2;   // WS_PF = 3 spills at the 168-register cap of a 9-warp CTA and is slower (33.3 vs 28.5 us)
-
-template <bool RC>
-__device__ __forceinline__ void ws_load_tile(float4 (&r)[4], const float* __restrict__ P, int ld, int row0, int n_rows,
-                                             int r0, int r_end, int tid) {
-  if (RC) {
-    const int sub = (tid & 31) >> 3, ch = tid & 7, wrow = (tid >> 5) * 16;
-#pragma unroll
-    for (int it = 0; it < 4; ++it) {
-      const int g = row0 + wrow + it * 4 + sub, k0 = r0 + ch * 4;
-      const float* p = P + (int64_t)g * ld + k0;
-      if (g < n_rows && k0 + 4 <= r_end && ((((uintptr_t)p) & 15) == 0)) {
-        r[it] = __ldg(reinterpret_cast<const float4*>(p));
-      } else {
-        const bool in = g < n_rows;
-        r[it].x = (in && k0 < r_end) ? p[0] : 0.f;
-        r[it].y = (in && k0 + 1 < r_end) ? p[1] : 0.f;
-        r[it].z = (in && k0 + 2 < r_end) ? p[2] : 0.f;
-        r[it].w = (in && k0 + 3 < r_end) ? p[3] : 0.f;
-      }
-    }
-  } else {
-    const int g = row0 + (tid & 127), half = tid >> 7;
-    const bool in = g < n_rows;
-    const float* p = P + (int64_t)r0 * ld + g;
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      const int cc = half * 4 + c;
-      r[c].x = (in && r0 + 4 * cc < r_end) ? p[(int64_t)(4 * cc) * ld] : 0.f;
-      r[c].y = (in && r0 + 4 * cc + 1 < r_end) ? p[(int64_t)(4 * cc + 1) * ld] : 0.f;
-      r[c].z = (in && r0 + 4 * cc + 2 < r_end) ? p[(int64_t)(4 * cc + 2) * ld] : 0.f;
-      r[c].w = (in && r0 + 4 * cc + 3 < r_end) ? p[(int64_t)(4 * cc + 3) * ld] : 0.f;
-    }
-  }
-}
-
-// Interior tiles and full 32-wide slices (all of a layer but its edges): no bounds logic, pointers advanced by the
-// caller.  `base` already points at this thread's first element of slice 0 (RC: row (wrow+sub), 16 B chunk ch;
-// !RC: tile row tid&127, reduction index (tid>>7)*16); r0 is the slice's offset along the reduction.
-template <bool RC>
-__device__ __forceinline__ void ws_load_tile_fast(float4 (&r)[4], const float* __restrict__ base, int ld, int r0) {
-  if (RC) {
-    const float* p = base + r0;
-#pragma unroll
-    for (int it = 0; it < 4; ++it) r[it] = __ldg(reinterpret_cast<const float4*>(p + (int64_t)(it * 4) * ld));
-  } else {
-    const float* p = base + (int64_t)r0 * ld;
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      r[c].x = __ldg(p + (int64_t)(4 * c) * ld);
-      r[c].y = __ldg(p + (int64_t)(4 * c + 1) * ld);
-      r[c].z = __ldg(p + (int64_t)(4 * c + 2) * ld);
-      r[c].w = __ldg(p + (int64_t)(4 * c + 3) * ld);
-    }
-  }
-}
-
-// hi/lo split + store with the swizzled offsets precomputed once per thread (they do not depend on the slice)
-__device__ __forceinline__ void ws_store_tile_fast(const float4 (&r)[4], uint8_t* hi_tile, uint8_t* lo_tile,
-                                                   const uint32_t (&off)[4]) {
-#pragma unroll
-  for (int it = 0; it < 4; ++it) {
-    float4 hi, lo;
-    hi.x = tf32_hi(r[it].x); hi.y = tf32_hi(r[it].y); hi.z = tf32_hi(r[it].z); hi.w = tf32_hi(r[it].w);
-    lo.x = r[it].x - hi.x; lo.y = r[it].y - hi.y; lo.z = r[it].z - hi.z; lo.w = r[it].w - hi.w;
-    *reinterpret_cast<float4*>(hi_tile + off[it]) = hi;
-    *reinterpret_cast<float4*>(lo_tile + off[it]) = lo;
-  }
-}
-
-template <bool RC>
-__device__ __forceinline__ void ws_store_tile(const float4 (&r)[4], uint8_t* hi_tile, uint8_t* lo_tile, int tid) {
-  const int sub = (tid & 31) >> 3, ch = tid & 7, wrow = (tid >> 5) * 16;
-#pragma unroll
-  for (int it = 0; it < 4; ++it) {
-    const int row = RC ? (wrow + it * 4 + sub) : (tid & 127);
-    const int chunk = RC ? ch : ((tid >> 7) * 4 + it);
-    float4 hi, lo;
-    hi.x = tf32_hi(r[it].x); hi.y = tf32_hi(r[it].y); hi.z = tf32_hi(r[it].z); hi.w = tf32_hi(r[it].w);
-    lo.x = r[it].x - hi.x; lo.y = r[it].y - hi.y; lo.z = r[it].z - hi.z; lo.w = r[it].w - hi.w;
-    const uint32_t off = sw128_off(row, chunk);
-    *reinterpret_cast<float4*>(hi_tile + off) = hi;
-    *reinterpret_cast<float4*>(lo_tile + off) = lo;
-  }
-}
-
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_ws(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "WS_WAIT_LOOP:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra WS_DONE;\n\t"
-      "bra WS_WAIT_LOOP;\n\t"
-      "WS_DONE:\n\t"
-      "}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void prod_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
-
-template <bool A_RC, bool B_RC, int EPI>
-__global__ void __launch_bounds__(WS_THREADS, 1)
-tc_gemm_ws_kernel(const float* __restrict__ A, int lda, const float* __restrict__ B, int ldb, float* __restrict__ C,
-                  int ldc, int M, int N, int R, const float* __restrict__ bias, int act, const float* __restrict__ mask,
-                  float keep, const float* __restrict__ gbias, int gP) {
-  extern __shared__ uint8_t smem_raw[];
-  __shared__ uint64_t bar_full[WS_STAGES], bar_empty[WS_STAGES], bar_done;
-  __shared__ uint32_t tmem_base_s;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  const int i0 = blockIdx.y * TC_BM, j0 = blockIdx.x * TC_BM;
-  const int n_here = min(N - j0, TC_BM);
-  const int n_pad = (n_here + 15) & ~15;
+  const int i0 = blockIdx.y * TC_BM, j0 = blockIdx.x * BN;
+  const int n_here = min(N - j0, BN);
   const int r_chunk = (R + gridDim.z - 1) / gridDim.z;
   const int r_begin = blockIdx.z * r_chunk, r_end = min(R, r_begin + r_chunk);
   const int KT = max((r_end - r_begin + TC_BK - 1) / TC_BK, 0);
+  const int stages = KT > 1 ? 2 : 1;
 
-  if (tid == 0) {
-    for (int s = 0; s < WS_STAGES; ++s) { mbar_init(&bar_full[s], WS_PROD); mbar_init(&bar_empty[s], 1); }
-    mbar_init(&bar_done, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "r"(256));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_d = tmem_base_s;
-
-  if (warp == 8) {
-    // ---------------- MMA issuer ----------------
-    if (lane == 0 && KT > 0) {
-      const uint32_t idesc = make_idesc(TC_BM, n_pad);
-      for (int kt = 0; kt < KT; ++kt) {
-        const int s = kt % WS_STAGES;
-        mbar_wait_ws(&bar_full[s], (uint32_t)((kt / WS_STAGES) & 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t a_hi = smem_u32(smem + s * TC_STAGE_BYTES), a_lo = a_hi + TC_TILE_BYTES, b_hi = a_hi + 2 * TC_TILE_BYTES,
-                       b_lo = a_hi + 3 * TC_TILE_BYTES;
+  // per-thread constants of the operand staging
+  const int sub = (tid & 31) >> 3, ch = tid & 7, wrow = (tid >> 5) * 16;
+  uint32_t offA[4], offB[4];
 #pragma unroll
-        for (int k = 0; k < TC_BK / 8; ++k) {
-          const uint32_t ko = k * 32;
-          const uint32_t first = (kt > 0 || k > 0) ? 1u : 0u;
-          umma_tf32(tmem_d + 128, make_desc(a_lo + ko), make_desc(b_hi + ko), idesc, first);
-          umma_tf32(tmem_d + 128, make_desc(a_hi + ko), make_desc(b_lo + ko), idesc, 1u);
-          umma_tf32(tmem_d, make_desc(a_hi + ko), make_desc(b_hi + ko), idesc, first);
-        }
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&bar_empty[s])) : "memory");
-      }
-      asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&bar_done)) : "memory");
+  for (int it = 0; it < 4; ++it) {
+    offA[it] = A_RC ? sw128_off(wrow + it * 4 + sub, ch) : sw128_off(tid & 127, (tid >> 7) * 4 + it);
+    offB[it] = B_RC ? sw128_off(wrow + it * 4 + sub, ch) : sw128_off(tid & 127, (tid >> 7) * 4 + it);
+  }
+  const float* baseA = A_RC ? A + (int64_t)(i0 + wrow + sub) * lda + ch * 4 : A + (int64_t)((tid >> 7) * 16) * lda + i0 + (tid & 127);
+  const float* baseB = B_RC ? B + (int64_t)(j0 + wrow + sub) * ldb + ch * 4 : B + (int64_t)((tid >> 7) * 16) * ldb + j0 + (tid & 127);
+  // interior tile, and 16 B alignment of every float4 the RC path reads
+  const bool fullA = (i0 + TC_BM <= M) && (!A_RC || (((lda & 3) == 0) && ((((uintptr_t)A) & 15) == 0) && ((r_begin & 3) == 0)));
+  const bool fullB = (j0 + TC_BM <= N) && (!B_RC || (((ldb & 3) == 0) && ((((uintptr_t)B) & 15) == 0) && ((r_begin & 3) == 0)));
+  auto load_slice = [&](float4 (&a)[4], float4 (&b)[4], int kt) {
+    const int r0 = r_begin + kt * TC_BK;
+    const bool whole = r0 + TC_BK <= r_end;
+    if (fullA && whole) load_tile_fast<A_RC>(a, baseA, lda, r0); else load_tile<A_RC>(a, A, lda, i0, M, r0, r_end, tid);
+    if (fullB && whole) load_tile_fast<B_RC>(b, baseB, ldb, r0); else load_tile<B_RC>(b, B, ldb, j0, N, r0, r_end, tid);
+  };
+
+  // Two accumulators: the tensor core adds in fp32 with truncation, so every accumulation costs ~2^-24 of the
+  // accumulator, with a bias.  The two cross terms (2^-11 of the result) go to their own accumulator: the main
+  // one then sees one accumulation per k-step instead of three.
+  float acc[BN / 2], acc2[BN / 2];
+#pragma unroll
+  for (int q = 0; q < BN / 2; ++q) { acc[q] = 0.f; acc2[q] = 0.f; }
+  float4 ra[4], rb[4];
+  if (KT > 0) load_slice(ra, rb, 0);
+  for (int kt = 0; kt < KT; ++kt) {
+    // stage kt%2 was last read by the MMAs of slice kt-2, which both warpgroups waited for before the barrier of kt-1
+    uint8_t* st = smem + (kt % stages) * TC_STAGE_BYTES;
+    store_tile_fast(ra, st, st + TC_TILE_BYTES, offA);
+    store_tile_fast(rb, st + 2 * TC_TILE_BYTES, st + 3 * TC_TILE_BYTES, offB);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to the tensor core
+    __syncthreads();
+    if (kt + 1 < KT) load_slice(ra, rb, kt + 1);   // next slice: global -> registers while the tensor core works
+    const uint32_t a_hi = smem_u32(st) + wg * (TC_TILE_BYTES / 2), a_lo = a_hi + TC_TILE_BYTES;
+    const uint32_t b_hi = smem_u32(st) + 2 * TC_TILE_BYTES, b_lo = b_hi + TC_TILE_BYTES;
+    fence_regs(acc); fence_regs(acc2);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < TC_BK / 8; ++k) {                        // K = 8 tf32 = 32 bytes inside the 128 B swizzle atom
+      const uint32_t ko = k * 32;
+      wgmma_tf32<BN>(acc2, make_desc(a_lo + ko), make_desc(b_hi + ko));
+      wgmma_tf32<BN>(acc2, make_desc(a_hi + ko), make_desc(b_lo + ko));
+      wgmma_tf32<BN>(acc, make_desc(a_hi + ko), make_desc(b_hi + ko));
     }
-    return;
+    wgmma_commit();
+    wgmma_wait_all();
+    fence_regs(acc); fence_regs(acc2);
   }
+  __syncthreads();   // every MMA has completed: the operand stages become the staging tile
 
-  // ---------------- producers ----------------
-  {
-    // per-thread constants of the fast path
-    const int sub = (tid & 31) >> 3, ch = tid & 7, wrow = (tid >> 5) * 16;
-    uint32_t offA[4], offB[4];
-#pragma unroll
-    for (int it = 0; it < 4; ++it) {
-      offA[it] = A_RC ? sw128_off(wrow + it * 4 + sub, ch) : sw128_off(tid & 127, (tid >> 7) * 4 + it);
-      offB[it] = B_RC ? sw128_off(wrow + it * 4 + sub, ch) : sw128_off(tid & 127, (tid >> 7) * 4 + it);
-    }
-    const float* baseA = A_RC ? A + (int64_t)(i0 + wrow + sub) * lda + ch * 4 : A + (int64_t)((tid >> 7) * 16) * lda + i0 + (tid & 127);
-    const float* baseB = B_RC ? B + (int64_t)(j0 + wrow + sub) * ldb + ch * 4 : B + (int64_t)((tid >> 7) * 16) * ldb + j0 + (tid & 127);
-    // interior tile, and 16 B alignment of every float4 the RC path reads
-    const bool fullA = (i0 + TC_BM <= M) && (!A_RC || (((lda & 3) == 0) && ((((uintptr_t)A) & 15) == 0) && ((r_begin & 3) == 0)));
-    const bool fullB = (j0 + TC_BM <= N) && (!B_RC || (((ldb & 3) == 0) && ((((uintptr_t)B) & 15) == 0) && ((r_begin & 3) == 0)));
-    auto load_slice = [&](float4 (&a)[4], float4 (&b)[4], int kt) {
-      const int r0 = r_begin + kt * TC_BK;
-      const bool whole = r0 + TC_BK <= r_end;
-      if (fullA && whole) ws_load_tile_fast<A_RC>(a, baseA, lda, r0); else ws_load_tile<A_RC>(a, A, lda, i0, M, r0, r_end, tid);
-      if (fullB && whole) ws_load_tile_fast<B_RC>(b, baseB, ldb, r0); else ws_load_tile<B_RC>(b, B, ldb, j0, N, r0, r_end, tid);
-    };
-    // WS_PF slices of operands in flight in registers (global/L2 latency is what the producers wait on)
-    float4 ra[WS_PF][4], rb[WS_PF][4];
-#pragma unroll
-    for (int u = 0; u < WS_PF; ++u)
-      if (u < KT) load_slice(ra[u], rb[u], u);
-    for (int kt0 = 0; kt0 < KT; kt0 += WS_PF) {
-#pragma unroll
-      for (int u = 0; u < WS_PF; ++u) {
-        const int kt = kt0 + u;
-        if (kt < KT) {
-          const int s = kt % WS_STAGES;
-          if (kt >= WS_STAGES) mbar_wait_ws(&bar_empty[s], (uint32_t)(((kt / WS_STAGES) - 1) & 1));
-          uint8_t* st = smem + s * TC_STAGE_BYTES;
-          ws_store_tile_fast(ra[u], st, st + TC_TILE_BYTES, offA);
-          ws_store_tile_fast(rb[u], st + 2 * TC_TILE_BYTES, st + 3 * TC_TILE_BYTES, offB);
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-          mbar_arrive(&bar_full[s]);
-          if (kt + WS_PF < KT) load_slice(ra[u], rb[u], kt + WS_PF);
-        }
-      }
-    }
-  }
-  if (KT > 0) mbar_wait_ws(&bar_done, 0u);
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-
-  // ---------------- epilogue 1 (warps 0-3): TMEM -> registers -> staging tile ----------------
+  // ---- epilogue 1: fragments -> staging tile (row 64*wg + 16*(warp%4) + lane/4 (+8), columns 8j + 2*(lane%4))
   float* stg = reinterpret_cast<float*>(smem);
-  if (warp < 4) {
-    for (int c0 = 0; c0 < n_pad; c0 += 16) {
-      uint32_t r[16], r2[16];
-      if (KT > 0) {
-        const uint32_t taddr = tmem_d + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0;
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-            : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-              "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-            : "r"(taddr));
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-            : "=r"(r2[0]), "=r"(r2[1]), "=r"(r2[2]), "=r"(r2[3]), "=r"(r2[4]), "=r"(r2[5]), "=r"(r2[6]), "=r"(r2[7]), "=r"(r2[8]),
-              "=r"(r2[9]), "=r"(r2[10]), "=r"(r2[11]), "=r"(r2[12]), "=r"(r2[13]), "=r"(r2[14]), "=r"(r2[15])
-            : "r"(taddr + 128));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+  const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
-        for (int q = 0; q < 16; ++q) r[q] = __float_as_uint(__uint_as_float(r[q]) + __uint_as_float(r2[q]));
-      } else {
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = 8 * j + 2 * (lane & 3);
 #pragma unroll
-        for (int q = 0; q < 16; ++q) r[q] = 0u;
-      }
-#pragma unroll
-      for (int q = 0; q < 16; q += 4)
-        *reinterpret_cast<uint4*>(stg + tid * TC_STG_PITCH + c0 + q) = make_uint4(r[q], r[q + 1], r[q + 2], r[q + 3]);
+    for (int h = 0; h < 2; ++h) {
+      const int q = 4 * j + 2 * h;
+      *reinterpret_cast<float2*>(stg + (row0 + 8 * h) * TC_STG_PITCH + col) =
+          make_float2(acc[q] + acc2[q], acc[q + 1] + acc2[q + 1]);
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  prod_bar_sync();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"(256));
+  __syncthreads();
 
-  // ---------------- epilogue 2 (warps 0-7): whole rows, 512 B coalesced stores ----------------
+  // ---- epilogue 2: a warp writes whole rows (lane l <-> columns 4l..4l+3): 512 B coalesced stores
   float* Cz = C + (EPI == 0 ? (int64_t)blockIdx.z * M * ldc : 0);
-  tc_epilogue_rows<EPI, 8>(stg, Cz, ldc, M, N, i0, j0, n_here, warp, lane, bias, act, mask, keep, gbias, gP);
+  tc_epilogue_rows<EPI, TC_THREADS / 32>(stg, Cz, ldc, M, N, i0, j0, n_here, warp, lane, bias, act, mask, keep, gbias, gP);
 }
 
-template <bool A_RC, bool B_RC, int EPI>
-static int launch_tc_ws(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int M, int N, int R, int S,
+template <bool A_RC, bool B_RC, int EPI, int BN>
+static int launch_tc_bn(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int M, int N, int R, int S,
                         const float* bias, int act, const float* mask, float keep, const float* gbias, int gP,
                         cudaStream_t st) {
   static bool attr = false;
-  constexpr int smem = WS_STAGES * TC_STAGE_BYTES + 1024;
+  constexpr int smem_max = tc_smem_bytes(2);
   if (!attr) {
-    cudaFuncSetAttribute(tc_gemm_ws_kernel<A_RC, B_RC, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaFuncSetAttribute(tc_gemm_kernel<A_RC, B_RC, EPI, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max);
     attr = true;
   }
-  dim3 grid((N + TC_BM - 1) / TC_BM, (M + TC_BM - 1) / TC_BM, S);
-  tc_gemm_ws_kernel<A_RC, B_RC, EPI><<<grid, WS_THREADS, smem, st>>>(A, lda, B, ldb, C, ldc, M, N, R, bias, act, mask, keep,
-                                                                    gbias, gP);
-  return 0;
-}
-
-template <bool A_RC, bool B_RC, int EPI, int STAGES>
-static int launch_tc_s(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int M, int N, int R, int S,
-                       const float* bias, int act, const float* mask, float keep, const float* gbias, int gP,
-                       cudaStream_t st) {
-  static bool attr = false;
-  constexpr int smem = tc_smem_bytes(STAGES);
-  if (!attr) {
-    cudaFuncSetAttribute(tc_gemm_kernel<A_RC, B_RC, EPI, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    attr = true;
-  }
-  dim3 grid((N + TC_BM - 1) / TC_BM, (M + TC_BM - 1) / TC_BM, S);
-  tc_gemm_kernel<A_RC, B_RC, EPI, STAGES><<<grid, 128, smem, st>>>(A, lda, B, ldb, C, ldc, M, N, R, bias, act, mask, keep,
-                                                                    gbias, gP);
+  const int r_chunk = (R + S - 1) / S;
+  const int smem = tc_smem_bytes(r_chunk > TC_BK ? 2 : 1);   // one slice: one stage, so that more CTAs fit an SM
+  dim3 grid((N + BN - 1) / BN, (M + TC_BM - 1) / TC_BM, S);
+  tc_gemm_kernel<A_RC, B_RC, EPI, BN><<<grid, TC_THREADS, smem, st>>>(A, lda, B, ldb, C, ldc, M, N, R, bias, act, mask,
+                                                                      keep, gbias, gP);
   return 0;
 }
 
@@ -635,15 +379,9 @@ template <bool A_RC, bool B_RC, int EPI>
 static int launch_tc(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int M, int N, int R, int S,
                      const float* bias, int act, const float* mask, float keep, const float* gbias, int gP,
                      cudaStream_t st) {
-  const int r_chunk = (R + S - 1) / S;
-  // CTR_GEMM_WS=0 keeps the single-role kernel for every shape (A/B switch, tools/bench_gemm.py)
-  static int ws = -1;
-  if (ws < 0) { const char* e = getenv("CTR_GEMM_WS"); ws = e ? atoi(e) : 1; }
-  if (ws && r_chunk >= 3 * TC_BK)
-    return launch_tc_ws<A_RC, B_RC, EPI>(A, lda, B, ldb, C, ldc, M, N, R, S, bias, act, mask, keep, gbias, gP, st);
-  if (r_chunk <= TC_BK)
-    return launch_tc_s<A_RC, B_RC, EPI, 1>(A, lda, B, ldb, C, ldc, M, N, R, S, bias, act, mask, keep, gbias, gP, st);
-  return launch_tc_s<A_RC, B_RC, EPI, 2>(A, lda, B, ldb, C, ldc, M, N, R, S, bias, act, mask, keep, gbias, gP, st);
+  if (N <= 32) return launch_tc_bn<A_RC, B_RC, EPI, 32>(A, lda, B, ldb, C, ldc, M, N, R, S, bias, act, mask, keep, gbias, gP, st);
+  if (N <= 64) return launch_tc_bn<A_RC, B_RC, EPI, 64>(A, lda, B, ldb, C, ldc, M, N, R, S, bias, act, mask, keep, gbias, gP, st);
+  return launch_tc_bn<A_RC, B_RC, EPI, 128>(A, lda, B, ldb, C, ldc, M, N, R, S, bias, act, mask, keep, gbias, gP, st);
 }
 
 // entry used by fc.cu: kind 0 = forward (A_RC, !B_RC, EPI 1), 1 = dIn (A_RC, B_RC, EPI 0 / 2), 2 = dW (!A_RC, !B_RC, EPI 0)

@@ -1,4 +1,4 @@
-"""Deep & Cross Network on the B200 engine: mirror of `model_fn` in deep_ctr/Model_pipeline/DCN.py:105-230.
+"""Deep & Cross Network on the H100 engine: mirror of `model_fn` in deep_ctr/Model_pipeline/DCN.py:105-230.
 
 Variables (TF names): `emb [N,K]`, `cross_w [L,D]`, `cross_b [L,D]` (all three L2-regularised,
 DCN.py:198-199), `Deep-Network/mlp{i}/...`, `DCN-out/out_layer/...`.  No first-order term, no bias

@@ -1,8 +1,8 @@
-"""DeepFM on the B200 engine: host-side mirror of `model_fn` in deep_ctr/Model_pipeline/DeepFM.py:100-221.
+"""DeepFM on the H100 engine: host-side mirror of `model_fn` in deep_ctr/Model_pipeline/DeepFM.py:100-221.
 
 Same parameters (`field_size, feature_size, embedding_size, l2_reg, learning_rate, deep_layers,
 dropout`, DeepFM.py:329-338), same variable names (`fm_bias, fm_w, fm_v, Deep-part/mlp{i}/...`),
-same modes (TRAIN / EVAL / PREDICT).  Everything numerical runs in hand-written sm_100a kernels
+same modes (TRAIN / EVAL / PREDICT).  Everything numerical runs in hand-written sm_90a kernels
 through the C ABI; see tf_repos_b200/base.py for the update modes and data parallelism.
 """
 from __future__ import annotations

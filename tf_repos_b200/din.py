@@ -1,4 +1,4 @@
-"""Deep Interest Network on the B200 engine: mirror of `model_fn` in deep_ctr/Model_pipeline/DIN.py:101-257.
+"""Deep Interest Network on the H100 engine: mirror of `model_fn` in deep_ctr/Model_pipeline/DIN.py:101-257.
 
 Inputs (the TFRecord features of DIN.py:60-77, already densified the way the reference does with
 sparse_tensor_to_dense, DIN.py:153-154):

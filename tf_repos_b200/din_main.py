@@ -1,4 +1,4 @@
-"""input_fn / main(_) of deep_ctr/Model_pipeline/DIN.py:57-99,300-392 on the B200 engine.
+"""input_fn / main(_) of deep_ctr/Model_pipeline/DIN.py:57-99,300-392 on the H100 engine.
 
 Input: TFRecord files of tf.Example (`data_dir/tr/*tfrecord`, `data_dir/te/*tfrecord`; eval files = test files, quirk
 Q6, DIN.py:342-345) with the features of DIN.py:60-77:

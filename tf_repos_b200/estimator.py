@@ -1,5 +1,5 @@
 """The observable contract of `main()` + tf.estimator in deep_ctr/Model_pipeline/DeepFM.py:284-366, on the
-B200 engine: same task types (train / eval / infer / export), same file globbing (tr*libsvm, va*libsvm,
+H100 engine: same task types (train / eval / infer / export), same file globbing (tr*libsvm, va*libsvm,
 te*libsvm), same `model_dir + dt_dir` quirk (Q2), `pred.txt` with "%f\\n" per row, AUC with
 tf.metrics.auc's 200 thresholds, `global_step/sec` logging every log_steps, resume from the checkpoint
 in model_dir.  The tf.estimator runtime itself (hooks, summaries, TF_CONFIG parameter servers) is out of

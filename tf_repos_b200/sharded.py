@@ -1,5 +1,5 @@
-"""Row-sharded embedding tables for DeepFM (BASELINE.json configs[4]: 1e9-row table over 8 B200s, where
-fm_v + fm_w + Adam slots = 204 GB exceed one GPU's 180 GB).  Not in the reference (SURVEY.md 8e).
+"""Row-sharded embedding tables for DeepFM (BASELINE.json configs[4]: 1e9-row table over 8 H100s, where
+fm_v + fm_w + Adam slots = 204 GB exceed one GPU's 80 GB).  Not in the reference (SURVEY.md 8e).
 
 owner(id) = id % G, local row = id // G.  One process per GPU, data-parallel batches:
 

@@ -1,4 +1,4 @@
-"""main(_) / input_fn of deep_ctr/Model_pipeline/wide_n_deep.py:55-82,181-242 on the B200 engine.
+"""main(_) / input_fn of deep_ctr/Model_pipeline/wide_n_deep.py:55-82,181-242 on the H100 engine.
 
 CSV input (wide_n_deep.py:55-82): tf.decode_csv with record_defaults [[0.0]] + 13*[[0.0]] + 26*[[0]] -> label
 `is_click`, I1..I13 float, C14..C39 int; TextLineDataset -> map -> repeat(num_epochs) -> batch (batches straddle

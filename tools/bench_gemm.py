@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Times ctr_fc_fwd / ctr_fc_bwd for the MLP and DIN-attention shapes; run with CTR_GEMM=simt to compare the
-fp32 SIMT tiles against the default tcgen05 3xTF32 path; prints TFLOP/s (2*M*K*N per product) and max error."""
+fp32 SIMT tiles against the default wgmma 3xTF32 path; prints TFLOP/s (2*M*K*N per product) and max error."""
 import os
 import sys
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Side measurements for BASELINE.json configs[2] (DCN) and configs[3] (DIN): training samples/s on one B200
+"""Side measurements for BASELINE.json configs[2] (DCN) and configs[3] (DIN): training samples/s on one H100
 with the inputs resident in HBM, CUDA-event timed.  (bench.py is the contract benchmark: DeepFM configs[1].)"""
 import json
 import os
@@ -61,5 +61,4 @@ if "din" in which:
         print(f"DIN {mode:15s} {ms:8.3f} ms/step  {B / ms * 1e3 / 1e6:7.3f} M samples/s", flush=True)
         del m
         torch.cuda.empty_cache()
-os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-json.dump(out, open(os.path.join(ROOT, "gpurun_out", "bench_models.json"), "w"), indent=1)
+print(json.dumps(out), flush=True)

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Summarise an `ncu --metrics gpu__time_duration.sum --csv` launch list: per-kernel count, total
-device time and share.  usage: tools/summarize_launches.py gpurun_out/launches.csv [> profiles/x.txt]"""
+device time and share.  usage: tools/summarize_launches.py launches.csv"""
 import collections
 import csv
 import re
