@@ -283,6 +283,18 @@ int ctr_cross_bwd(const float* x0, const float* w, const float* b, const float* 
                   const float* dx_in, int B, int D, int L, float* dx0, float* dw, float* db, void* ws,
                   size_t ws_bytes, ctr_stream_t stream);
 
+/* ---- DeepMVM multi-view product (DeepMVM.py:144-150) ----------------------------------------------
+ * a = x + mvm_b (broadcast over the batch);  x_mvm[b,k] = (((a[b,0,k] * a[b,1,k]) * a[b,2,k]) * ... ) * a[b,F-1,k]
+ * x: [B, F*K] (K1 CTR_FM_PLAIN output), mvm_b: [F,K], x_mvm: [B,K].  Every op is one IEEE-rounded fp32 op in field
+ * order, with gradual underflow (bit-identical to a sequential fp32 restatement).  F <= 64, K <= 256.
+ * bwd (TF autodiff of the chain, no division): with g = d_xmvm and P_i = a_0*...*a_i as the forward rounds it,
+ * for i = F-1..1 { da_i = g*P_{i-1}; g = g*a_i }, da_0 = g;  d_e = da + dX (dX NULL = 0), d_e: [B, F*K];
+ * d_mvm_b[f,k] = sum_b da[b,f,k] (overwritten; per-CTA partials in ws, fixed-order merge: deterministic). */
+int ctr_mvm_fwd(const float* x, const float* mvm_b, int B, int F, int K, float* x_mvm, ctr_stream_t stream);
+size_t ctr_mvm_bwd_workspace_bytes(int B, int F, int K);
+int ctr_mvm_bwd(const float* x, const float* mvm_b, const float* d_xmvm, const float* dX, int B, int F, int K,
+                float* d_e, float* d_mvm_b, void* ws, size_t ws_bytes, ctr_stream_t stream);
+
 /* ---- K6/K9: DIN embedding + field-wise pooling layers (DIN.py:143-183) ---------------------------
  * gather_scale_rows: out[(i/G)*ld_group + (i%G)*K + k] = V[ids[i]][k] * (wgt ? wgt[i] : 1)
  *     (tf.nn.embedding_lookup of feat_ids / a_catids / padded behaviour ids, DIN.py:143-147,155-156;

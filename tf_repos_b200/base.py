@@ -205,14 +205,18 @@ class CTRModel:
         self.dense.apply()
         self.global_step += 1
         parts = [self.loss_ce]
-        if dense_reg is not None:
+        if dense_reg is not None and not self.table_reg_first:
             parts.append(dense_reg)
         if self.W is not None:
             parts.append(upd.reg[1:2])
         parts.append(upd.reg[0:1])
+        if dense_reg is not None and self.table_reg_first:
+            parts.append(dense_reg)
         return torch.cat(parts)
 
     bias_name: Optional[str] = None
+    # loss-term order: False = dense terms before the tables (DCN.py:198-199), True = after them (DeepMVM.py:197-199)
+    table_reg_first = False
 
     # ---- CUDA-graph replay of the step ----------------------------------------------------------------------
     def train_step_graphed(self, ids: torch.Tensor, vals: torch.Tensor, labels: torch.Tensor) -> torch.Tensor:

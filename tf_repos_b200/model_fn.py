@@ -13,7 +13,7 @@ returned spec carries results and a `train_op` callable:
 features: "feat_ids" int32|int64 [B,F] or [B,F,1], "feat_vals" float32 same shape (the input_fn contract, :97-98).
 params: field_size, feature_size, embedding_size, learning_rate, l2_reg, deep_layers, dropout (:329-338) plus, because
 the reference reads them from FLAGS inside model_fn, optional optimizer (:204-211), batch_size, update_mode, model
-('DeepFM' | 'DCN' | 'NFM' | 'PNN' | 'AFM') and that model's extra keys (cross_layers, model_type, attention_layers).
+('DeepFM' | 'DCN' | 'DeepMVM' | 'NFM' | 'PNN' | 'AFM') and that model's extra keys (cross_layers, model_type, attention_layers).
 """
 from __future__ import annotations
 
@@ -48,6 +48,9 @@ def build_model(params: Dict[str, Any], batch_size: int, device="cuda"):
     if name == "DCN":
         from .dcn import DCN
         return DCN(F, N, K, batch_size, deep_layers=params.get("deep_layers", "256,128,64"), cross_layers=int(params.get("cross_layers", 3)), **kw)
+    if name == "DeepMVM":
+        from .deepmvm import DeepMVM
+        return DeepMVM(F, N, K, batch_size, deep_layers=params.get("deep_layers", "256,128,64"), **kw)
     if name == "NFM":
         from .nfm import NFM
         return NFM(F, N, K, batch_size, deep_layers=params.get("deep_layers", "128,64"), **kw)
@@ -57,7 +60,7 @@ def build_model(params: Dict[str, Any], batch_size: int, device="cuda"):
     if name == "AFM":
         from .afm import AFM
         return AFM(F, N, K, batch_size, attention_layers=params.get("attention_layers", "256"), **kw)
-    raise ValueError(f"params['model'] = {name!r} is not one of DeepFM, DCN, NFM, PNN, AFM")
+    raise ValueError(f"params['model'] = {name!r} is not one of DeepFM, DCN, DeepMVM, NFM, PNN, AFM")
 
 
 def model_fn(features: Dict[str, torch.Tensor], labels: Optional[torch.Tensor], mode: str, params: Dict[str, Any],

@@ -273,6 +273,28 @@ def cross_bwd(x0, w, b, s, dxL, dx_in, dx0, dw, db, ws):
           "ctr_cross_bwd")
 
 
+def mvm_fwd(x, mvm_b, x_mvm):
+    """x [B, F*K] (K1 FM_PLAIN output), mvm_b [F,K] -> x_mvm [B,K] (DeepMVM.py:144-150)."""
+    F, K = mvm_b.shape
+    B = x.shape[0]
+    check(_L.ctr_mvm_fwd(_p(x, torch.float32, "x"), _p(mvm_b, torch.float32, "mvm_b"), B, F, K,
+                         _p(x_mvm, torch.float32, "x_mvm"), _stream()), "ctr_mvm_fwd")
+
+
+def mvm_bwd_workspace_bytes(B, F, K) -> int:
+    return int(_L.ctr_mvm_bwd_workspace_bytes(B, F, K))
+
+
+def mvm_bwd(x, mvm_b, d_xmvm, dX, d_e, d_mvm_b, ws):
+    """d_e [B, F*K] = d x through the product (+ dX when given); d_mvm_b [F,K] overwritten."""
+    F, K = mvm_b.shape
+    B = x.shape[0]
+    check(_L.ctr_mvm_bwd(_p(x, torch.float32, "x"), _p(mvm_b, torch.float32, "mvm_b"),
+                         _p(d_xmvm, torch.float32, "d_xmvm"), _p(dX, torch.float32, "dX"), B, F, K,
+                         _p(d_e, torch.float32, "d_e"), _p(d_mvm_b, torch.float32, "d_mvm_b"), _p(ws),
+                         ws.numel() * ws.element_size(), _stream()), "ctr_mvm_bwd")
+
+
 def _dptr(t: torch.Tensor) -> int:
     """device pointer of a (possibly strided / offset) view; only the base address is used"""
     if not t.is_cuda or t.dtype != torch.float32:

@@ -29,6 +29,10 @@ def _build(model_name: str, p: Dict, batch_size: int, device):
     if model_name == "DCN":
         from .dcn import DCN
         return DCN(F, N, K, batch_size, deep_layers=p["deep_layers"], cross_layers=int(p["cross_layers"]), **common)
+    if model_name == "DeepMVM":
+        from .deepmvm import DeepMVM
+        return DeepMVM(F, N, K, batch_size, deep_layers=p["deep_layers"], batch_norm=bool(p.get("batch_norm", False)),
+                       **common)
     if model_name == "NFM":
         from .nfm import NFM
         return NFM(F, N, K, batch_size, deep_layers=p["deep_layers"], **common)
