@@ -295,6 +295,33 @@ size_t ctr_mvm_bwd_workspace_bytes(int B, int F, int K);
 int ctr_mvm_bwd(const float* x, const float* mvm_b, const float* d_xmvm, const float* dX, int B, int F, int K,
                 float* d_e, float* d_mvm_b, void* ws, size_t ws_bytes, ctr_stream_t stream);
 
+/* ---- ESMM shared embedding layer and multi-task head (DeepMTL/Model_pipeline/DeepCvrMTL.py) --------------------
+ * embed_fwd (:153-164): x [B, (F'+8)K] = [common F'K | u_cat | u_shop | u_brand | u_int | a_cat | a_shop | a_brand |
+ *     a_int] from feat_ids [B,F'], a_ids [3,B] (a_cat, a_shop, a_brand) and one CSR over 5B bags: bag j*B+b (j = u_cat,
+ *     u_shop, u_brand, u_int, a_int) is occurrences [bag_off[j*B+b], bag_off[j*B+b+1]) of bag_ids / bag_wgt.
+ *     bag sum = ((0 + e_0*w_0) + e_1*w_1) + ... in occurrence order, each * and + one IEEE-rounded op (no FMA); a_int is
+ *     unweighted (its bag_wgt entries are not read).  Empty bag -> +0 row.  Ids outside [0,N) are counted into
+ *     oob[0] (oob[1] = first) like ctr_gather_scale_rows and contribute zero rows.  K in {4,8,16,32,64,128,256}.
+ * embed_bwd: g_rows [n_rows, K] in the order [common (row b*F'+f) | a_cat B | a_shop B | a_brand B | occurrences
+ *     bag_off[5B] | zero rows up to n_rows]: the dx slice of each lookup, times w (one rounded multiply) for u_* bags.
+ * head (:205-223), one CTA, fixed-order reductions (deterministic); labels y, z NULL => inference:
+ *     pctr = sigmoid(y_ctr), pcvr = sigmoid(y_cvr), pctcvr = pctr*pcvr;
+ *     losses[0] = sum_{i<n} CE(y_ctr_i, y_i) / n;  losses[1] = sum_{i<n} -(z*log(p+eps)) - ((1-z)*log((1-p)+eps)) / n,
+ *     eps = 1e-7 (tf.losses.log_loss, SUM_BY_NONZERO_WEIGHTS);
+ *     with g_ctr = w_ctr/n, g_cvr = w_cvr/n (w_ctr, w_cvr: the fp32 constants w and 1-w):
+ *       dp = ((-g_cvr*z) * rcp(p+eps)) + -((-g_cvr*(1-z)) * rcp((1-p)+eps))
+ *       d_cvr = ((dp*pctr)*pcvr)*(1-pcvr)
+ *       d_ctr = (pctr - y)*g_ctr + ((dp*pcvr)*pctr)*(1-pctr)
+ *     rows n..B-1 get d = +0. */
+int ctr_esmm_embed_fwd(const int32_t* feat_ids, const int32_t* a_ids, const int32_t* bag_ids, const float* bag_wgt,
+                       const int32_t* bag_off, const float* V, int64_t N, int B, int Fp, int K, float* x, int32_t* oob,
+                       ctr_stream_t stream);
+int ctr_esmm_embed_bwd(const float* dx, const float* bag_wgt, const int32_t* bag_off, int B, int Fp, int K,
+                       int64_t n_rows, float* g_rows, ctr_stream_t stream);
+int ctr_esmm_head(const float* y_ctr, const float* y_cvr, const float* y, const float* z, int B, int n, float w_ctr,
+                  float w_cvr, float* pctr, float* pcvr, float* pctcvr, float* losses, float* d_ctr, float* d_cvr,
+                  ctr_stream_t stream);
+
 /* ---- K6/K9: DIN embedding + field-wise pooling layers (DIN.py:143-183) ---------------------------
  * gather_scale_rows: out[(i/G)*ld_group + (i%G)*K + k] = V[ids[i]][k] * (wgt ? wgt[i] : 1)
  *     (tf.nn.embedding_lookup of feat_ids / a_catids / padded behaviour ids, DIN.py:143-147,155-156;

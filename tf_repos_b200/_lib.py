@@ -76,6 +76,9 @@ SIGNATURES = {
     "ctr_mvm_fwd": (c_int, [P, P, c_int, c_int, c_int, P, P]),
     "ctr_mvm_bwd_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "ctr_mvm_bwd": (c_int, [P, P, P, P, c_int, c_int, c_int, P, P, P, c_size_t, P]),
+    "ctr_esmm_embed_fwd": (c_int, [P, P, P, P, P, P, c_int64, c_int, c_int, c_int, P, P, P]),
+    "ctr_esmm_embed_bwd": (c_int, [P, P, P, c_int, c_int, c_int, c_int64, P, P]),
+    "ctr_esmm_head": (c_int, [P, P, P, P, c_int, c_int, c_float, c_float, P, P, P, P, P, P, P]),
     "ctr_gather_scale_rows": (c_int, [P, P, P, c_int64, c_int64, c_int, c_int, c_int64, P, P, P]),
     "ctr_bag_sum_fwd": (c_int, [P, P, P, P, c_int64, c_int, c_int, c_int64, P, P]),
     "ctr_bag_sum_bwd": (c_int, [P, c_int64, P, P, c_int, c_int, P, P]),

@@ -33,21 +33,23 @@ from .tfrecord import parse_example, read_records
 U_FIELDS = ("cat", "shop", "brand", "int")
 
 
-def decode_tfrecord_files(files: Sequence[str], field_size: int) -> Dict[str, list]:
-    """All examples of `files`, feature by feature (tf.parse_single_example with the spec of DIN.py:60-77)."""
+def decode_tfrecord_files(files: Sequence[str], field_size: int, labels: Sequence[str] = ("y",)) -> Dict[str, list]:
+    """All examples of `files`, feature by feature (tf.parse_single_example with the spec of DIN.py:60-77).
+    `labels`: the required float label features (ESMM also requires z, DeepCvrMTL.py:67-68)."""
     print("Parsing", list(files))
-    d: Dict[str, list] = {k: [] for k in ("y", "feat_ids", "a_cat", "a_shop", "a_brand", "a_int")}
+    d: Dict[str, list] = {k: [] for k in tuple(labels) + ("feat_ids", "a_cat", "a_shop", "a_brand", "a_int")}
     for f in U_FIELDS:
         d["u_%sids" % f], d["u_%svals" % f] = [], []
     for path in files:
         for rec in read_records(path):
             ex = parse_example(rec)
-            for key in ("y", "feat_ids", "a_catids", "a_shopids", "a_brandids"):
+            for key in tuple(labels) + ("feat_ids", "a_catids", "a_shopids", "a_brandids"):
                 if key not in ex or len(ex[key]) == 0:
-                    raise ValueError(f"{path}: Feature: {key} (data type: {'float' if key == 'y' else 'int64'}) is required but could not be found.")
+                    raise ValueError(f"{path}: Feature: {key} (data type: {'float' if key in labels else 'int64'}) is required but could not be found.")
             if len(ex["feat_ids"]) != field_size:
                 raise ValueError(f"{path}: feat_ids has {len(ex['feat_ids'])} values, field_size is {field_size}")
-            d["y"].append(float(ex["y"][0]))
+            for key in labels:
+                d[key].append(float(ex[key][0]))
             d["feat_ids"].append(np.asarray(ex["feat_ids"], dtype=np.int64))
             d["a_cat"].append(int(ex["a_catids"][0])); d["a_shop"].append(int(ex["a_shopids"][0]))
             d["a_brand"].append(int(ex["a_brandids"][0]))

@@ -23,14 +23,15 @@ class MLP:
     def __init__(self, in_dim: int, layers: Sequence[int], keep_prob: Sequence[float], B: int, device,
                  scope: str = "Deep-part", out_scope: Optional[str] = "deep_out", out_extra_in: int = 0,
                  seed: int = 0, layer_fmt: str = "mlp{i}", w_name: str = "weights", b_name: str = "biases",
-                 batch_norm: bool = False, bn_decay: float = 0.9):
-        # layer_fmt / w_name / b_name: TF variable naming (contrib fully_connected: mlp{i}/weights|biases;
-        # the canned estimators' Dense layers: hiddenlayer_{i}/kernel|bias)
-        self.layer_fmt, self.w_name, self.b_name = layer_fmt, w_name, b_name
+                 batch_norm: bool = False, bn_decay: float = 0.9, *, bn_fmt: str = "bn_{i}"):
+        # layer_fmt / w_name / b_name / bn_fmt: TF variable naming (contrib fully_connected: mlp{i}/weights|biases;
+        # the canned estimators' Dense layers: hiddenlayer_{i}/kernel|bias; ESMM's towers: cvr_mlp{i}, cvr_bn_{i}).
+        # An empty scope leaves the names unprefixed (DeepCvrMTL.py's tf.name_scope does not prefix get_variable).
+        self.layer_fmt, self.w_name, self.b_name, self.bn_fmt = layer_fmt, w_name, b_name, bn_fmt
         self.in_dim, self.layers, self.keep = in_dim, list(layers), list(keep_prob)
         self.scope, self.out_scope, self.B, self.device = scope, out_scope, B, device
         # TF name of the output layer: "<scope>/<out_scope>", or out_scope itself when it is a full path
-        self.out_name = out_scope if (out_scope and "/" in out_scope) else f"{scope}/{out_scope}"
+        self.out_name = out_scope if (out_scope and "/" in out_scope) else self._scoped(out_scope)
         self.last_dim = self.layers[-1] if self.layers else in_dim
         self.out_extra_in = out_extra_in
         self.out_in = self.last_dim + out_extra_in
@@ -50,22 +51,25 @@ class MLP:
             self.bn_mean = [torch.zeros(w, **f32) for w in self.layers]    # batch moments saved for the backward
             self.bn_var = [torch.ones(w, **f32) for w in self.layers]
             for i, w in enumerate(self.layers):
-                self.bn_state[f"{scope}/bn_{i}/moving_mean"] = torch.zeros(w, **f32)
-                self.bn_state[f"{scope}/bn_{i}/moving_variance"] = torch.ones(w, **f32)
+                self.bn_state[self._bn(i, "moving_mean")] = torch.zeros(w, **f32)
+                self.bn_state[self._bn(i, "moving_variance")] = torch.ones(w, **f32)
         dims = [in_dim] + self.layers
         ws = max([ops.fc_bwd_workspace_bytes(B, dims[i], dims[i + 1]) for i in range(len(self.layers))] +
                  [ops.fc1_bwd_workspace_bytes(B, self.last_dim, out_extra_in), 16])
         self.ws = torch.empty(ws, dtype=torch.uint8, device=device)
         self._active = [None] * len(self.layers)
 
+    def _scoped(self, name: str) -> str:
+        return f"{self.scope}/{name}" if self.scope else name
+
     def _w(self, i: int) -> str:
-        return f"{self.scope}/{self.layer_fmt.format(i=i)}/{self.w_name}"
+        return self._scoped(f"{self.layer_fmt.format(i=i)}/{self.w_name}")
 
     def _b(self, i: int) -> str:
-        return f"{self.scope}/{self.layer_fmt.format(i=i)}/{self.b_name}"
+        return self._scoped(f"{self.layer_fmt.format(i=i)}/{self.b_name}")
 
     def _bn(self, i: int, what: str) -> str:
-        return f"{self.scope}/bn_{i}/{what}"
+        return self._scoped(f"{self.bn_fmt.format(i=i)}/{what}")
 
     def specs(self):
         out, d = [], self.in_dim

@@ -295,6 +295,34 @@ def mvm_bwd(x, mvm_b, d_xmvm, dX, d_e, d_mvm_b, ws):
                          ws.numel() * ws.element_size(), _stream()), "ctr_mvm_bwd")
 
 
+def esmm_embed_fwd(feat_ids, a_ids, bag_ids, bag_wgt, bag_off, V, x, oob=None):
+    """DeepCvrMTL.py:153-164.  feat_ids [B,F'], a_ids [3,B], CSR bags (bag_off [5B+1]) -> x [B,(F'+8)K]."""
+    N, K = V.shape
+    B, Fp = feat_ids.shape
+    check(_L.ctr_esmm_embed_fwd(_p(feat_ids, torch.int32, "feat_ids"), _p(a_ids, torch.int32, "a_ids"),
+                                _p(bag_ids, torch.int32, "bag_ids"), _p(bag_wgt, torch.float32, "bag_wgt"),
+                                _p(bag_off, torch.int32, "bag_off"), _p(V, torch.float32, "V"), N, B, Fp, K,
+                                _p(x, torch.float32, "x"), _p(oob, torch.int32, "oob"), _stream()), "ctr_esmm_embed_fwd")
+
+
+def esmm_embed_bwd(dx, bag_wgt, bag_off, B, Fp, K, g_rows):
+    """g_rows [n_rows, K]: per-occurrence gradient rows in the model's ids order, zero past the batch's occurrences."""
+    check(_L.ctr_esmm_embed_bwd(_p(dx, torch.float32, "dx"), _p(bag_wgt, torch.float32, "bag_wgt"),
+                                _p(bag_off, torch.int32, "bag_off"), B, Fp, K, g_rows.shape[0],
+                                _p(g_rows, torch.float32, "g_rows"), _stream()), "ctr_esmm_embed_bwd")
+
+
+def esmm_head(y_ctr, y_cvr, y, z, n, w_ctr, w_cvr, pctr, pcvr, pctcvr, losses=None, d_ctr=None, d_cvr=None):
+    """DeepCvrMTL.py:205-223.  w_ctr, w_cvr: the task weights w and 1-w (each rounded to fp32 by ctypes)."""
+    B = y_ctr.numel()
+    check(_L.ctr_esmm_head(_p(y_ctr, torch.float32, "y_ctr"), _p(y_cvr, torch.float32, "y_cvr"),
+                           _p(y, torch.float32, "y"), _p(z, torch.float32, "z"), B, int(n), float(w_ctr), float(w_cvr),
+                           _p(pctr, torch.float32, "pctr"), _p(pcvr, torch.float32, "pcvr"),
+                           _p(pctcvr, torch.float32, "pctcvr"), _p(losses, torch.float32, "losses"),
+                           _p(d_ctr, torch.float32, "d_ctr"), _p(d_cvr, torch.float32, "d_cvr"), _stream()),
+          "ctr_esmm_head")
+
+
 def _dptr(t: torch.Tensor) -> int:
     """device pointer of a (possibly strided / offset) view; only the base address is used"""
     if not t.is_cuda or t.dtype != torch.float32:

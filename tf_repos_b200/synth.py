@@ -73,3 +73,25 @@ def din_batch(B: int, N: int, Fp: int = 11, P: int = 100, max_a_int: int = 8, se
     batch = {"feat_ids": feat_ids, "a_ids": a_ids, "a_int_ids": a_int_ids, "a_int_off": a_off,
              "u_ids": u_ids, "u_wgt": u_wgt}
     return {k: v.to(device) for k, v in batch.items()}, labels.to(device)
+
+
+def esmm_batch(B: int, N: int, Fp: int = 11, max_lens=(49, 499, 49, 49, 8), min_len: int = 1, seed: int = 0,
+               device="cpu"):
+    """Synthetic ESMM batch (DeepCvrMTL.py:66-83, Ali-CCP layout) in the CSR form of tf_repos_b200.esmm: ids uniform in
+    [0, N) (id 0 is an ordinary id), bag j of each sample ~ U{min_len..max_lens[j]} ids (j = u_cat, u_shop, u_brand,
+    u_int, a_int), weights ~ U(0,3); y ~ Bernoulli(0.25), z = y * Bernoulli(0.3) (a conversion follows a click).
+    Returns (batch, (y, z))."""
+    g = torch.Generator().manual_seed(seed)
+    ri = lambda *shape: torch.randint(0, N, shape, generator=g, dtype=torch.int64).to(torch.int32)
+    feat_ids = ri(B, Fp)
+    a_ids = ri(3, B)
+    lens = torch.stack([torch.randint(min_len, m + 1, (B,), generator=g) for m in max_lens])     # [5, B]
+    off = torch.zeros(5 * B + 1, dtype=torch.int32)
+    off[1:] = torch.cumsum(lens.reshape(-1), 0).to(torch.int32)
+    nnz = int(off[-1])
+    bag_ids = ri(nnz)
+    bag_wgt = torch.rand(nnz, generator=g) * 3.0
+    y = (torch.rand(B, generator=g) < 0.25).float()
+    z = y * (torch.rand(B, generator=g) < 0.3).float()
+    batch = {"feat_ids": feat_ids, "a_ids": a_ids, "bag_ids": bag_ids, "bag_wgt": bag_wgt, "bag_off": off}
+    return {k: v.to(device) for k, v in batch.items()}, (y.to(device), z.to(device))
