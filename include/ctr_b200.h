@@ -327,7 +327,9 @@ int ctr_esmm_head(const float* y_ctr, const float* y_cvr, const float* y, const 
  *     (tf.nn.embedding_lookup of feat_ids / a_catids / padded behaviour ids, DIN.py:143-147,155-156;
  *      G, ld_group let the rows land directly inside the concatenated MLP input, DIN.py:199)
  * bag_sum: tf.nn.embedding_lookup_sparse(combiner="sum") over CSR bags (a_intids, DIN.py:148; the
- *     non-attention pooling branch :180-183) and its gradient g_rows[i] = d_out[bag(i)] * w_i
+ *     non-attention pooling branch :180-183) and its gradient g_rows[i] = d_out[bag(i)] * w_i.
+ *     An id outside [0,N) adds nothing; bag_sum_fwd_oob also counts it into oob[0] (oob[1] = first) like
+ *     ctr_gather_scale_rows (TF raises InvalidArgumentError).  ctr_bag_sum_fwd is bag_sum_fwd_oob with oob = NULL.
  * din_pool: att = sigmoid(z); u[b] = sum_p (ids[b,p] > 0) * att[b,p] * E[b,p,:]   (DIN.py:169-172)
  *     bwd: dE = mask*att*du (written, not accumulated); dz = mask*att*(1-att)*(E . du)
  * group_sum: dU[b] = sum_p dZ[b*P+p]   (gradient of ctr_fc_fwd_grouped's group bias)
@@ -337,6 +339,8 @@ int ctr_gather_scale_rows(const int32_t* ids, const float* wgt, const float* V, 
                           int G, int64_t ld_group, float* out, int32_t* oob, ctr_stream_t stream);
 int ctr_bag_sum_fwd(const int32_t* ids, const float* wgt, const int32_t* offsets, const float* V, int64_t N,
                     int B, int K, int64_t ld, float* out, ctr_stream_t stream);
+int ctr_bag_sum_fwd_oob(const int32_t* ids, const float* wgt, const int32_t* offsets, const float* V, int64_t N,
+                        int B, int K, int64_t ld, float* out, int32_t* oob, ctr_stream_t stream);
 int ctr_bag_sum_bwd(const float* d_out, int64_t ld, const float* wgt, const int32_t* offsets, int B, int K,
                     float* g_rows, ctr_stream_t stream);
 int ctr_scale_rows(const float* x, const float* add, const float* w, int64_t n, int K, int G, int64_t ld_group,

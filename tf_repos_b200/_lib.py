@@ -81,6 +81,7 @@ SIGNATURES = {
     "ctr_esmm_head": (c_int, [P, P, P, P, c_int, c_int, c_float, c_float, P, P, P, P, P, P, P]),
     "ctr_gather_scale_rows": (c_int, [P, P, P, c_int64, c_int64, c_int, c_int, c_int64, P, P, P]),
     "ctr_bag_sum_fwd": (c_int, [P, P, P, P, c_int64, c_int, c_int, c_int64, P, P]),
+    "ctr_bag_sum_fwd_oob": (c_int, [P, P, P, P, c_int64, c_int, c_int, c_int64, P, P, P]),
     "ctr_bag_sum_bwd": (c_int, [P, c_int64, P, P, c_int, c_int, P, P]),
     "ctr_scale_rows": (c_int, [P, P, P, c_int64, c_int, c_int, c_int64, P, P]),
     "ctr_din_pool_fwd": (c_int, [P, P, P, c_int, c_int, c_int, P, P, c_int64, P]),

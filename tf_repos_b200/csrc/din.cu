@@ -36,11 +36,12 @@ gather_scale_rows_kernel(const int32_t* __restrict__ ids, const float* __restric
 }
 
 // out[b*ld + k] = sum_{i in [off[b], off[b+1])} V[ids[i]][k] * w_i      (one lane group per bag)
+// ids outside [0, N) add nothing and are counted into oob like gather_scale_rows_kernel
 template <int LPR, int VEC>
 __global__ void __launch_bounds__(256)
 bag_sum_fwd_kernel(const int32_t* __restrict__ ids, const float* __restrict__ wgt,
                    const int32_t* __restrict__ offsets, const float* __restrict__ V, int64_t N, int B,
-                   int64_t ld, float* __restrict__ out) {
+                   int64_t ld, float* __restrict__ out, int32_t* __restrict__ oob) {
   constexpr int K = 4 * LPR * VEC;
   const int b = (int)(((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / LPR);
   const int c = threadIdx.x % LPR;
@@ -51,7 +52,10 @@ bag_sum_fwd_kernel(const int32_t* __restrict__ ids, const float* __restrict__ wg
   for (int i = offsets[b]; i < offsets[b + 1]; ++i) {
     int64_t id = ids[i];
     float w = wgt ? wgt[i] : 1.f;
-    if (id < 0 || id >= N) { id = 0; w = 0.f; }
+    if (id < 0 || id >= N) {
+      if (oob && c == 0) { if (atomicAdd(&oob[0], 1) == 0) oob[1] = (int32_t)id; }
+      id = 0; w = 0.f;
+    }
     const float4* row = reinterpret_cast<const float4*>(V + id * K) + c;
 #pragma unroll
     for (int v = 0; v < VEC; ++v) acc[v] = f4_fma(__ldg(row + v * LPR), make_float4(w, w, w, w), acc[v]);
@@ -266,12 +270,18 @@ int ctr_gather_scale_rows(const int32_t* ids, const float* wgt, const float* V, 
 
 int ctr_bag_sum_fwd(const int32_t* ids, const float* wgt, const int32_t* offsets, const float* V, int64_t N,
                     int B, int K, int64_t ld, float* out, ctr_stream_t stream) {
+  return ctr_bag_sum_fwd_oob(ids, wgt, offsets, V, N, B, K, ld, out, nullptr, stream);
+}
+
+int ctr_bag_sum_fwd_oob(const int32_t* ids, const float* wgt, const int32_t* offsets, const float* V, int64_t N,
+                        int B, int K, int64_t ld, float* out, int32_t* oob, ctr_stream_t stream) {
   CTR_REQUIRE(B >= 0 && K > 0 && N > 0, CTR_ERR_INVALID_ARG, "ctr_bag_sum_fwd: bad args");
   if (B == 0) return CTR_OK;
   CTR_REQUIRE(offsets && V && out, CTR_ERR_INVALID_ARG, "ctr_bag_sum_fwd: null buffer");
   cudaStream_t st = as_stream(stream);
-#define BF(LPR, VEC) \
-  bag_sum_fwd_kernel<LPR, VEC><<<(unsigned)ceil_div64((int64_t)B * LPR, 256), 256, 0, st>>>(ids, wgt, offsets, V, N, B, ld, out);
+#define BF(LPR, VEC)                                                                                                   \
+  bag_sum_fwd_kernel<LPR, VEC><<<(unsigned)ceil_div64((int64_t)B * LPR, 256), 256, 0, st>>>(ids, wgt, offsets, V, N, B, \
+                                                                                            ld, out, oob);
   DIN_K_SWITCH(K, BF)
 #undef BF
   CTR_LAUNCHED("ctr_bag_sum_fwd");

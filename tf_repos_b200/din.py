@@ -171,7 +171,7 @@ class DIN:
         ops.gather_scale_rows(batch["feat_ids"].reshape(-1), None, V, x, Fp, Dx, self.oob)                 # :143
         for j in range(3):                                                                                   # :145-147
             ops.gather_scale_rows(batch["a_ids"][j], None, V, x[:, self.off_a + j * K:], 1, Dx, self.oob)
-        ops.bag_sum_fwd(batch["a_int_ids"], None, batch["a_int_off"], V, x[:, self.off_a + 3 * K:], Dx)     # :148
+        ops.bag_sum_fwd(batch["a_int_ids"], None, batch["a_int_off"], V, x[:, self.off_a + 3 * K:], Dx, self.oob)  # :148
         if self.attention_pooling:
             W = self.dense[f"{ATT}/att_fc0/weights"]
             b1 = self.dense[f"{ATT}/att_fc0/biases"]
@@ -197,7 +197,7 @@ class DIN:
         else:
             for f in range(4):   # embedding_lookup_sparse(sp_weights, combiner="sum")  (DIN.py:180-183)
                 ops.bag_sum_fwd(batch["u_ids"][f].reshape(-1), batch["u_wgt"][f].reshape(-1), self._pad_offsets(),
-                                V, x[:, self.off_u + f * K:], Dx)
+                                V, x[:, self.off_u + f * K:], Dx, self.oob)
         mm = masks.get("mlp") if masks else None
         self._a = self.mlp.forward_hidden(x, self.dense, train, mm, step_dev=self.opt.state[3:4])            # :199-208
         return self.mlp.forward_out(self._a, self.dense)                                                    # :211-214

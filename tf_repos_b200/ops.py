@@ -338,12 +338,13 @@ def gather_scale_rows(ids, wgt, V, out_view, G, ld_group, oob=None):
                                    _stream()), "ctr_gather_scale_rows")
 
 
-def bag_sum_fwd(ids, wgt, offsets, V, out_view, ld):
+def bag_sum_fwd(ids, wgt, offsets, V, out_view, ld, oob=None):
+    """oob: int32 [2] counter of ids outside [0, N) (count, first), as in gather_scale_rows"""
     N, K = V.shape
     B = offsets.numel() - 1
-    check(_L.ctr_bag_sum_fwd(_p(ids, torch.int32, "ids"), _p(wgt, torch.float32, "wgt"),
-                             _p(offsets, torch.int32, "offsets"), _p(V, torch.float32, "V"), N, B, K, ld,
-                             _dptr(out_view), _stream()), "ctr_bag_sum_fwd")
+    check(_L.ctr_bag_sum_fwd_oob(_p(ids, torch.int32, "ids"), _p(wgt, torch.float32, "wgt"),
+                                 _p(offsets, torch.int32, "offsets"), _p(V, torch.float32, "V"), N, B, K, ld,
+                                 _dptr(out_view), _p(oob, torch.int32, "oob"), _stream()), "ctr_bag_sum_fwd_oob")
 
 
 def bag_sum_bwd(d_out_view, ld, wgt, offsets, K, g_rows):
