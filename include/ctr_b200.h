@@ -192,14 +192,24 @@ int ctr_epoch_rows2(int opt, int apply, float* var, float* slot0, float* slot1, 
  * rewrites, for every step < upto, one entry per CTA it launches (fewer than *n_partials_host) and ctr_epoch_reg_loss
  * sums whole rows, so the entries no CTA owns must hold 0.
  * list / list_cap / list_count / ss_rows (optional, Adam): scratch for the packed-pipe sweep (csrc/epoch_adam.cu):
- * device int32[list_cap] with list_cap >= min(n_rows, ids gathered since `from`), a device int32 counter, and the
- * row kernels' per-step sum(var^2) accumulator (the `ss` of ctr_epoch_rows).  NULL selects the scalar kernels.
- * *list_count returns the number of gathered rows found; if it exceeds list_cap the precondition was violated and
- * the rows beyond list_cap were NOT caught up (the engine sizes the list so that this cannot happen). */
+ * device int32[list_cap], a device int32 counter, and the row kernels' per-step sum(var^2) accumulator (the `ss` of
+ * ctr_epoch_rows).  NULL selects the scalar kernels.
+ * CAPACITY: the list receives every row whose `last` byte exceeds `from`, i.e. every row a ctr_epoch_rows call
+ * gathered since the previous sweep.  With at most n_ids distinct ids per step that is at most
+ * min(n_rows, n_ids * (upto - from)) <= min(n_rows, n_ids * ctr_epoch_max_steps()) rows; list_cap must be at least
+ * that.  *list_count returns the number of gathered rows found.  If it exceeds list_cap, the rows beyond list_cap
+ * were NOT caught up although their `last` byte is rewritten: the table is wrong.  ctr_epoch_sweep_ovf reports this. */
 int ctr_epoch_sweep(int opt, float* var, float* slot0, float* slot1, uint8_t* last, int64_t n_rows, int K,
                     const float* hyper, const float* lr_table, int from, int upto, int reset, double* ss_partials,
                     int* n_partials_host, int32_t* list, int64_t list_cap, int32_t* list_count, double* ss_rows,
                     ctr_stream_t stream);
+/* ctr_epoch_sweep, plus list_overflow (nullable): device int32 counter to which the packed sweep ADDS the number of
+ * gathered rows it found beyond list_cap (it is not cleared here).  Non-zero after a call means the capacity rule
+ * above was broken and the table no longer holds the every-step state; the models' check_ids() raises on it. */
+int ctr_epoch_sweep_ovf(int opt, float* var, float* slot0, float* slot1, uint8_t* last, int64_t n_rows, int K,
+                        const float* hyper, const float* lr_table, int from, int upto, int reset, double* ss_partials,
+                        int* n_partials_host, int32_t* list, int64_t list_cap, int32_t* list_count, double* ss_rows,
+                        int32_t* list_overflow, ctr_stream_t stream);
 /* reg[s] (+)= scale*(ss_rows[s] + sum_b ss_partials[s][b]) for s < upto; clears ss_rows[s] */
 int ctr_epoch_reg_loss(double* ss_rows, const double* ss_partials, int n_partials, int upto, float scale,
                        float* reg, int accumulate, ctr_stream_t stream);

@@ -135,6 +135,7 @@ class CTRModel:
 
     def check_ids(self):
         """TF raises InvalidArgumentError for ids outside [0, feature_size); we count them on device."""
+        self.updater.check_list_overflow()
         cnt, first = self.oob.tolist()
         if cnt:
             self.oob.zero_()

@@ -26,8 +26,8 @@ constexpr int EPOCH_MAX = 32;  // max steps per epoch (lr table / ss table size)
 // epoch_adam.cu: Adam sweep on the packed fp32 pipe (rows nothing gathered since `from`; the others go to `list`)
 bool launch_epoch_sweep_adam(float* var, float* slot0, float* slot1, const uint8_t* last, int64_t n_rows, int K,
                              const float* hyper, const float* lr_table, int from, int upto, double* ss_partials,
-                             int n_partials, int32_t* list, int32_t* list_count, int64_t list_cap, int grid,
-                             cudaStream_t st);
+                             int n_partials, int32_t* list, int32_t* list_count, int64_t list_cap,
+                             int32_t* list_overflow, int grid, cudaStream_t st);
 
 __device__ __forceinline__ float sq4(const float4& x) {
   return (x.x * x.x + x.y * x.y) + (x.z * x.z + x.w * x.w);
@@ -144,7 +144,8 @@ epoch_rows_kernel(float* __restrict__ var, float* __restrict__ slot0, float* __r
   if (WITH_W && threadIdx.x < EPOCH_MAX && ssw_blk[threadIdx.x] != 0.f) atomicAdd(&w.ss[threadIdx.x], (double)ssw_blk[threadIdx.x]);
 }
 
-// any K (incl. the scalar first-order table, K = 1): one thread per (row, k)
+// any K (incl. the scalar first-order table, K = 1): one thread per (row, k).  A CTA holds 256/K whole rows and is
+// rounded up to whole warps (the body shuffles with the full mask); the surplus threads own no element.
 template <int OPT, bool APPLY>
 __global__ void __launch_bounds__(256)
 epoch_rows_generic_kernel(float* __restrict__ var, float* __restrict__ slot0, float* __restrict__ slot1,
@@ -156,11 +157,11 @@ epoch_rows_generic_kernel(float* __restrict__ var, float* __restrict__ slot0, fl
   __shared__ float ss_blk[EPOCH_MAX];
   if (threadIdx.x < EPOCH_MAX) ss_blk[threadIdx.x] = 0.f;
   __syncthreads();
-  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t u = t / K;
-  const int k = (int)(t % K);
+  const int rows_per_cta = 256 / K;
+  const int64_t u = (int64_t)blockIdx.x * rows_per_cta + threadIdx.x / K;
+  const int k = (int)(threadIdx.x % K);
   const int lane = threadIdx.x & 31;
-  const bool active = u < n_max && u < n_uniq[0];
+  const bool active = (int)threadIdx.x < rows_per_cta * K && u < n_max && u < n_uniq[0];
   Hyper h = load_hyper(hyper);
   const int64_t id = active ? uniq[u] : 0;
   const int l0 = active ? last[id] : j;
@@ -192,8 +193,8 @@ epoch_rows_generic_kernel(float* __restrict__ var, float* __restrict__ slot0, fl
     var[e] = x; slot0[e] = a;
     if (two) slot1[e] = b;
   }
-  // the row's `last` byte is written after every k of the row has read it; the launch uses (256/K)*K threads
-  // per CTA, so a row never straddles two CTAs
+  // the row's `last` byte is written after every k of the row has read it; a CTA holds whole rows, so a row
+  // never straddles two CTAs
   __syncthreads();
   if (active && k == 0) last[id] = (uint8_t)(set_last >= 0 ? set_last : (APPLY ? j + 1 : j));
   if (threadIdx.x < EPOCH_MAX && ss_blk[threadIdx.x] != 0.f) atomicAdd(&ss[threadIdx.x], (double)ss_blk[threadIdx.x]);
@@ -547,8 +548,10 @@ static int launch_epoch_rows(int opt, int apply, float* var, float* slot0, float
                              const int32_t* uniq, const int32_t* n_uniq, const float* g_uniq, int64_t n_max, int K,
                              const float* hyper, const float* lr_table, int j, double* ss, int set_last,
                              cudaStream_t st) {
-  // generic path: a row's K threads sit in one CTA (they synchronise on the row's `last` byte)
-  const int gen_block = K <= 256 ? (256 / K) * K : 0;
+  // generic path: a row's K threads sit in one CTA (they synchronise on the row's `last` byte); 256/K rows per CTA,
+  // the CTA rounded up to whole warps
+  const int gen_rows = K <= 256 ? 256 / K : 0;
+  const int gen_block = (gen_rows * K + 31) / 32 * 32;
 #define ER_K(OPT, AP, KK, LPR, VEC)                                                                  \
   case KK:                                                                                           \
     epoch_rows_kernel<OPT, LPR, VEC, AP><<<(unsigned)ceil_div64(n_max * LPR, 256), 256, 0, st>>>(    \
@@ -559,7 +562,7 @@ static int launch_epoch_rows(int opt, int apply, float* var, float* slot0, float
     ER_K(OPT, AP, 4, 1, 1) ER_K(OPT, AP, 8, 2, 1) ER_K(OPT, AP, 16, 4, 1) ER_K(OPT, AP, 32, 8, 1)    \
     ER_K(OPT, AP, 64, 16, 1) ER_K(OPT, AP, 128, 32, 1) ER_K(OPT, AP, 256, 32, 2)                     \
     default:                                                                                         \
-      epoch_rows_generic_kernel<OPT, AP><<<(unsigned)ceil_div64(n_max * K, gen_block), gen_block, 0, st>>>( \
+      epoch_rows_generic_kernel<OPT, AP><<<(unsigned)ceil_div64(n_max, gen_rows), gen_block, 0, st>>>(   \
           var, slot0, slot1, last, uniq, n_uniq, g_uniq, n_max, K, hyper, lr_table, j, ss, set_last); \
   }
 #define ER_CALL(OPT)                     \
@@ -630,10 +633,10 @@ int ctr_epoch_rows2(int opt, int apply, float* var, float* slot0, float* slot1, 
   return CTR_OK;
 }
 
-int ctr_epoch_sweep(int opt, float* var, float* slot0, float* slot1, uint8_t* last, int64_t n_rows, int K,
-                    const float* hyper, const float* lr_table, int from, int upto, int reset, double* ss_partials,
-                    int* n_partials_host, int32_t* list, int64_t list_cap, int32_t* list_count, double* ss_rows,
-                    ctr_stream_t stream) {
+int ctr_epoch_sweep_ovf(int opt, float* var, float* slot0, float* slot1, uint8_t* last, int64_t n_rows, int K,
+                        const float* hyper, const float* lr_table, int from, int upto, int reset, double* ss_partials,
+                        int* n_partials_host, int32_t* list, int64_t list_cap, int32_t* list_count, double* ss_rows,
+                        int32_t* list_overflow, ctr_stream_t stream) {
   CTR_REQUIRE(n_rows >= 0 && K > 0 && from >= 0 && from <= upto && upto <= EPOCH_MAX, CTR_ERR_INVALID_ARG,
               "ctr_epoch_sweep: bad n_rows/K/from/upto");
   // tuning hook (tools/tune_epoch.py): CTR_EPOCH_CFG selects (unroll, CTAs/SM) of the scalar K%4==0 kernel;
@@ -666,7 +669,8 @@ int ctr_epoch_sweep(int opt, float* var, float* slot0, float* slot1, uint8_t* la
     CTR_REQUIRE(cudaMemsetAsync(list_count, 0, sizeof(int32_t), st) == cudaSuccess, CTR_ERR_CUDA,
                 "ctr_epoch_sweep: memset failed");
     const bool ok = launch_epoch_sweep_adam(var, slot0, slot1, last, n_rows, K, hyper, lr_table, from, upto,
-                                            ss_partials, n_partials, list, list_count, list_cap, grid, st);
+                                            ss_partials, n_partials, list, list_count, list_cap, list_overflow, grid,
+                                            st);
     CTR_REQUIRE(ok, CTR_ERR_UNSUPPORTED, "ctr_epoch_sweep: packed path refused K=%d", K);
     CTR_LAUNCHED("ctr_epoch_sweep(adam)");
     // rows gathered since `from`: catch up from their own `last` to upto; they get their final `last` here
@@ -719,6 +723,14 @@ int ctr_epoch_sweep(int opt, float* var, float* slot0, float* slot1, uint8_t* la
     CTR_LAUNCHED("ctr_epoch_sweep(last)");
   }
   return CTR_OK;
+}
+
+int ctr_epoch_sweep(int opt, float* var, float* slot0, float* slot1, uint8_t* last, int64_t n_rows, int K,
+                    const float* hyper, const float* lr_table, int from, int upto, int reset, double* ss_partials,
+                    int* n_partials_host, int32_t* list, int64_t list_cap, int32_t* list_count, double* ss_rows,
+                    ctr_stream_t stream) {
+  return ctr_epoch_sweep_ovf(opt, var, slot0, slot1, last, n_rows, K, hyper, lr_table, from, upto, reset, ss_partials,
+                             n_partials_host, list, list_cap, list_count, ss_rows, nullptr, stream);
 }
 
 int ctr_epoch_reg_loss(double* ss_rows, const double* ss_partials, int n_partials, int upto, float scale,

@@ -128,14 +128,18 @@ class SparseUpdater:
     def enable_epochs(self, P: int, tables: Sequence[Table]):
         """Allocates the per-row `last` bytes and the per-step sum(var^2) accumulators."""
         pmax = ops.epoch_max_steps()
-        assert 1 <= P <= pmax
+        if not 1 <= P <= pmax:
+            raise ValueError(f"epoch_steps={P}: must be in [1, {pmax}] (the `last` bytes and lr table hold {pmax} steps)")
         dev = tables[0].var.device
         self.P = P
         self.flush_pos = 0   # steps of the current epoch every row's stored state already contains (mid-epoch flush)
         self.n_epart = ops.epoch_partials_count()
         self.ep = {}
+        # rows the packed Adam sweep found but could not list (a list smaller than include/ctr_b200.h's bound)
+        self.list_overflow = torch.zeros(1, dtype=torch.int32, device=dev)
         for t in tables:
-            # rows gathered since the last sweep, collected by the packed Adam sweep for its second pass
+            # rows gathered since the last sweep, collected by the packed Adam sweep for its second pass: at most
+            # n distinct ids per step, P <= pmax steps per epoch
             cap = max(min(self.n * pmax, t.N), 1)
             self.ep[t.name] = dict(
                 list=torch.empty(cap, dtype=torch.int32, device=dev),
@@ -178,7 +182,7 @@ class SparseUpdater:
                 ev[0].record()
             ops.epoch_sweep(o.opt, t.var, t.slot(0), t.slot(1), e["last"], t.N, t.K, o.record(HYPER_TABLE),
                             o.lr_table, self.flush_pos, upto, reset, e["partials"], e["list"], e["list_count"],
-                            e["ss"])
+                            e["ss"], self.list_overflow)
             if ev is not None:
                 ev[1].record()
                 self.sweep_events.append(ev)
@@ -186,6 +190,15 @@ class SparseUpdater:
             # accumulate: a mid-epoch flush and the epoch-end sweep each contribute their share
             ops.epoch_reg_loss(e["ss"], e["partials"], self.n_epart, upto, 0.5 * l2_reg, e["reg"], accumulate=True)
         self.flush_pos = 0 if reset else upto
+
+    def check_list_overflow(self):
+        """Raises if an epoch sweep dropped gathered rows (their state is then not the every-step state)."""
+        ovf = getattr(self, "list_overflow", None)
+        n = int(ovf.item()) if ovf is not None else 0
+        if n:
+            ovf.zero_()
+            raise RuntimeError(f"exact-deferred epoch sweep: {n} gathered rows did not fit in the row list and were "
+                               "not caught up; the table state is invalid")
 
     def epoch_begin(self):
         for e in self.ep.values():

@@ -101,6 +101,7 @@ class ESMM:
             vs[name].copy_(v.to(self.device, torch.float32).reshape(vs[name].shape))
 
     def check_ids(self):
+        self.updater.check_list_overflow()
         cnt, first = self.oob.tolist()
         if cnt:
             self.oob.zero_()

@@ -501,18 +501,20 @@ def epoch_partials_count() -> int:
 
 
 def epoch_sweep(opt, var, slot0, slot1, last, n_rows, K, hyper, lr_table, from_: int, upto: int, reset: bool,
-                ss_partials, list_buf=None, list_count=None, ss_rows=None):
-    """list_buf / list_count / ss_rows: scratch of the packed-pipe Adam sweep (None: scalar kernels)."""
+                ss_partials, list_buf=None, list_count=None, ss_rows=None, list_overflow=None):
+    """list_buf / list_count / ss_rows: scratch of the packed-pipe Adam sweep (None: scalar kernels).
+    list_overflow: int32 [1] counter; gathered rows that did not fit in list_buf are added to it (see check_ids)."""
     n_part = ctypes.c_int(0)
     check(
-        _L.ctr_epoch_sweep(
+        _L.ctr_epoch_sweep_ovf(
             opt, _p(var, torch.float32, "var"), _p(slot0, torch.float32, "slot0"),
             _p(slot1, torch.float32, "slot1"), _p(last, torch.uint8, "last"), n_rows, K,
             _p(hyper, torch.float32, "hyper"), _p(lr_table, torch.float32, "lr_table"), from_, upto, int(reset),
             _p(ss_partials, torch.float64, "ss_partials"), ctypes.byref(n_part),
             _p(list_buf, torch.int32, "list"), (list_buf.numel() if list_buf is not None else 0),
-            _p(list_count, torch.int32, "list_count"), _p(ss_rows, torch.float64, "ss_rows"), _stream()),
-        "ctr_epoch_sweep")
+            _p(list_count, torch.int32, "list_count"), _p(ss_rows, torch.float64, "ss_rows"),
+            _p(list_overflow, torch.int32, "list_overflow"), _stream()),
+        "ctr_epoch_sweep_ovf")
     return n_part.value
 
 

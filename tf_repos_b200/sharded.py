@@ -267,6 +267,7 @@ class ShardedDeepFM:
         return torch.cat([self.loss_ce, upd.reg[1:2], upd.reg[0:1]])   # reg terms: this rank's shard only
 
     def check_ids(self):
+        self.updater.check_list_overflow()
         cnt, first = self.oob.tolist()
         if cnt:
             self.oob.zero_()
