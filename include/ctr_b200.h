@@ -285,7 +285,10 @@ int ctr_bn_bwd(const float* d_out, const float* x, int n, int H, const float* sa
 /* ---- K5: DCN cross network (DCN.py:140-145) ------------------------------------------------------
  * x_{l+1} = x0 * (x_l . w_l) + x_l + b_l,  l = 0..L-1;  w,b: [L,D];  x0: [B,D], D = F*K (D%4==0, <=2048)
  * fwd saves the L scalars s[b,l] = x_l . w_l;  bwd recomputes x_l from x0 and s.
- * bwd: dx0 = dx_in (NULL = 0) + dL/dx0 through the cross network;  dw, db: [L,D] (deterministic). */
+ * bwd: dx0 = dx_in (NULL = 0) + dL/dx0 through the cross network;  dw, db: [L,D] (deterministic).
+ * Limits (CTR_ERR_UNSUPPORTED, checked before anything else, so a call with B = 0 and NULL buffers probes them):
+ *   both: D % 4 == 0, D <= 2048, L <= 32;  fwd: L >= 0 (L = 0 copies x0);  bwd: L >= 1 and the per-warp slab
+ *   2*L*D floats must fit 200 KB (8*L*D <= 204800 bytes: D = 2048 allows L <= 12).  B = 0 launches nothing. */
 int ctr_cross_fwd(const float* x0, const float* w, const float* b, int B, int D, int L, float* xL, float* s,
                   ctr_stream_t stream);
 size_t ctr_cross_bwd_workspace_bytes(int B, int D, int L);
@@ -378,7 +381,10 @@ int ctr_axpby(const float* a, float alpha, const float* b, float beta, int64_t n
  * afm_pool:   att = softmax_p(logit) (AFM.py:151), w = dropout(att) (:152-153), y_emb = sum_p w_p pw_p (:156);
  *   bwd: dpw = w * dy_emb (written), dlogit = softmax backward.
  * dropout_apply: out = x / keep * mask  (NFM's dropout on the bi-interaction vector, NFM.py:136-137;
- *   AFM's on y_emb, AFM.py:157-158) */
+ *   AFM's on y_emb, AFM.py:157-158)
+ * Limits (CTR_ERR_UNSUPPORTED, checked before anything else, so a call with B = 0 and NULL buffers probes them):
+ *   pnn_product_fwd: 16*F*(K+1) <= 204800 bytes of shared memory (F = 39: K <= 327);
+ *   pnn_product_bwd: 32*F*(K+1) <= 204800 (F = 39: K <= 163);  afm_pool_*: P <= 10240 (F <= 143). */
 int ctr_pnn_product_fwd(const float* x, int B, int F, int K, int outer, float* z, ctr_stream_t stream);
 int ctr_pnn_product_bwd(const float* x, const float* dz, int B, int F, int K, int outer, float* dX,
                         ctr_stream_t stream);

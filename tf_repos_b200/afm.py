@@ -23,6 +23,11 @@ class AFM(CTRModel):
         self.att_layers, self.keep = ints(attention_layers), floats(dropout)
         if len(self.att_layers) != 1:
             raise NotImplementedError("one attention layer (the reference default '256')")
+        try:
+            ops.afm_pool_check(field_size * (field_size - 1) // 2, embedding_size)
+        except ops.CtrError as e:
+            raise ValueError(f"--field_size={field_size} gives more field pairs than the attention pooling kernels "
+                             f"take: {e}") from None
         super().__init__(field_size, feature_size, embedding_size, batch_size, l2_reg, learning_rate, optimizer,
                          update_mode, device, seed, world, epoch_steps)
 

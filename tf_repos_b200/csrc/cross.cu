@@ -216,7 +216,9 @@ int ctr_cross_bwd(const float* x0, const float* w, const float* b, const float* 
   CTR_REQUIRE(D % 4 == 0 && D <= 2048 && L <= 32, CTR_ERR_UNSUPPORTED,
               "ctr_cross_bwd: needs D %% 4 == 0, D <= 2048, L <= 32 (got D=%d L=%d)", D, L);
   const int wpc = bwd_warps_per_cta(D, L);
-  CTR_REQUIRE(wpc >= 1, CTR_ERR_UNSUPPORTED, "ctr_cross_bwd: L*D too large for the shared-memory slabs");
+  CTR_REQUIRE(wpc >= 1, CTR_ERR_UNSUPPORTED,
+              "ctr_cross_bwd: L*D too large for the shared-memory slabs (got D=%d L=%d)", D, L);
+  if (B == 0) return CTR_OK;
   CTR_REQUIRE(x0 && w && b && s && dxL && dx0 && dw && db, CTR_ERR_INVALID_ARG, "ctr_cross_bwd: null buffer");
   CTR_REQUIRE(ws && ws_bytes >= ctr_cross_bwd_workspace_bytes(B, D, L), CTR_ERR_WORKSPACE,
               "ctr_cross_bwd: workspace too small");

@@ -218,10 +218,11 @@ extern "C" {
 
 int ctr_pnn_product_fwd(const float* x, int B, int F, int K, int outer, float* z, ctr_stream_t stream) {
   CTR_REQUIRE(B >= 0 && F >= 2 && K > 0, CTR_ERR_INVALID_ARG, "ctr_pnn_product_fwd: bad shape");
+  const size_t smem = (size_t)PW_WARPS * F * (K + 1) * sizeof(float);
+  CTR_REQUIRE(smem <= 200 * 1024, CTR_ERR_UNSUPPORTED,
+              "ctr_pnn_product_fwd: F*K too large for shared memory (got F=%d K=%d)", F, K);
   if (B == 0) return CTR_OK;
   CTR_REQUIRE(x && z, CTR_ERR_INVALID_ARG, "ctr_pnn_product_fwd: null buffer");
-  const size_t smem = (size_t)PW_WARPS * F * (K + 1) * sizeof(float);
-  CTR_REQUIRE(smem <= 200 * 1024, CTR_ERR_UNSUPPORTED, "ctr_pnn_product_fwd: F*K too large for shared memory");
   cudaStream_t st = as_stream(stream);
   const int grid = (B + PW_WARPS - 1) / PW_WARPS;
   if (outer) {
@@ -238,10 +239,11 @@ int ctr_pnn_product_fwd(const float* x, int B, int F, int K, int outer, float* z
 int ctr_pnn_product_bwd(const float* x, const float* dz, int B, int F, int K, int outer, float* dX,
                         ctr_stream_t stream) {
   CTR_REQUIRE(B >= 0 && F >= 2 && K > 0, CTR_ERR_INVALID_ARG, "ctr_pnn_product_bwd: bad shape");
+  const size_t smem = (size_t)PW_WARPS * 2 * F * (K + 1) * sizeof(float);
+  CTR_REQUIRE(smem <= 200 * 1024, CTR_ERR_UNSUPPORTED,
+              "ctr_pnn_product_bwd: F*K too large for shared memory (got F=%d K=%d)", F, K);
   if (B == 0) return CTR_OK;
   CTR_REQUIRE(x && dz && dX, CTR_ERR_INVALID_ARG, "ctr_pnn_product_bwd: null buffer");
-  const size_t smem = (size_t)PW_WARPS * 2 * F * (K + 1) * sizeof(float);
-  CTR_REQUIRE(smem <= 200 * 1024, CTR_ERR_UNSUPPORTED, "ctr_pnn_product_bwd: F*K too large for shared memory");
   cudaStream_t st = as_stream(stream);
   const int grid = (B + PW_WARPS - 1) / PW_WARPS;
   if (outer) {
@@ -281,9 +283,10 @@ int ctr_afm_pairs_bwd(const float* x, const float* dpw, int B, int F, int K, flo
 int ctr_afm_pool_fwd(const float* pw, const float* logit, const float* mask, float keep, int B, int P, int K,
                      float* att, float* y_emb, ctr_stream_t stream) {
   CTR_REQUIRE(B >= 0 && P > 0 && K > 0, CTR_ERR_INVALID_ARG, "ctr_afm_pool_fwd: bad shape");
+  CTR_REQUIRE((size_t)P * 4 <= 40 * 1024, CTR_ERR_UNSUPPORTED,
+              "ctr_afm_pool_fwd: too many pairs (got P=%d, the limit is 10240)", P);
   if (B == 0) return CTR_OK;
   CTR_REQUIRE(pw && logit && att && y_emb, CTR_ERR_INVALID_ARG, "ctr_afm_pool_fwd: null buffer");
-  CTR_REQUIRE((size_t)P * 4 <= 40 * 1024, CTR_ERR_UNSUPPORTED, "ctr_afm_pool_fwd: too many pairs");
   afm_pool_fwd_kernel<<<B, 256, (size_t)P * 4, as_stream(stream)>>>(pw, logit, mask, keep, B, P, K, att, y_emb);
   CTR_LAUNCHED("ctr_afm_pool_fwd");
   return CTR_OK;
@@ -292,9 +295,10 @@ int ctr_afm_pool_fwd(const float* pw, const float* logit, const float* mask, flo
 int ctr_afm_pool_bwd(const float* pw, const float* att, const float* mask, float keep, const float* dy_emb, int B,
                      int P, int K, float* dpw, float* dlogit, ctr_stream_t stream) {
   CTR_REQUIRE(B >= 0 && P > 0 && K > 0, CTR_ERR_INVALID_ARG, "ctr_afm_pool_bwd: bad shape");
+  CTR_REQUIRE((size_t)P * 4 <= 40 * 1024, CTR_ERR_UNSUPPORTED,
+              "ctr_afm_pool_bwd: too many pairs (got P=%d, the limit is 10240)", P);
   if (B == 0) return CTR_OK;
   CTR_REQUIRE(pw && att && dy_emb && dpw && dlogit, CTR_ERR_INVALID_ARG, "ctr_afm_pool_bwd: null buffer");
-  CTR_REQUIRE((size_t)P * 4 <= 40 * 1024, CTR_ERR_UNSUPPORTED, "ctr_afm_pool_bwd: too many pairs");
   afm_pool_bwd_kernel<<<B, 256, (size_t)P * 4, as_stream(stream)>>>(pw, att, mask, keep, dy_emb, B, P, K, dpw, dlogit);
   CTR_LAUNCHED("ctr_afm_pool_bwd");
   return CTR_OK;

@@ -26,6 +26,13 @@ class DCN(CTRModel):
                  batch_norm_decay: float = 0.9):
         self.layers, self.keep, self.L = ints(deep_layers), floats(dropout), int(cross_layers)
         self.batch_norm, self.bn_decay = bool(batch_norm), float(batch_norm_decay)
+        try:
+            if self.L > 0:                               # with no cross layer no cross kernel runs
+                ops.cross_check(field_size * embedding_size, self.L)
+        except ops.CtrError as e:
+            raise ValueError(f"--field_size={field_size} x --embedding_size={embedding_size} (D = "
+                             f"{field_size * embedding_size}) with --cross_layers={self.L} is not supported by the "
+                             f"cross network kernels: {e}") from None
         super().__init__(field_size, feature_size, embedding_size, batch_size, l2_reg, learning_rate, optimizer,
                          update_mode, device, seed, world, epoch_steps)
         self.emb = self.V

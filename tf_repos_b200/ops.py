@@ -395,6 +395,25 @@ def axpby(a, alpha, b, beta, out):
                        _p(out, torch.float32, "out"), _stream()), "ctr_axpby")
 
 
+def pnn_product_check(F, K, outer):
+    """Raises CtrError if pnn_product_fwd or _bwd rejects (F, K).  Called with B = 0: launches nothing."""
+    check(_L.ctr_pnn_product_fwd(None, 0, F, K, int(outer), None, None), "ctr_pnn_product_fwd")
+    check(_L.ctr_pnn_product_bwd(None, None, 0, F, K, int(outer), None, None), "ctr_pnn_product_bwd")
+
+
+def afm_pool_check(P, K):
+    """Raises CtrError if afm_pool_fwd or _bwd rejects (P, K).  Called with B = 0: launches nothing."""
+    check(_L.ctr_afm_pool_fwd(None, None, None, 1.0, 0, P, K, None, None, None), "ctr_afm_pool_fwd")
+    check(_L.ctr_afm_pool_bwd(None, None, None, 1.0, None, 0, P, K, None, None, None), "ctr_afm_pool_bwd")
+
+
+def cross_check(D, L):
+    """Raises CtrError if cross_fwd or cross_bwd rejects (D, L).  Called with B = 0: launches nothing."""
+    check(_L.ctr_cross_fwd(None, None, None, 0, D, L, None, None, None), "ctr_cross_fwd")
+    check(_L.ctr_cross_bwd(None, None, None, None, None, None, 0, D, L, None, None, None, None, 0, None),
+          "ctr_cross_bwd")
+
+
 def pnn_product_fwd(x, B, F, K, outer, z):
     check(_L.ctr_pnn_product_fwd(_p(x, torch.float32, "x"), B, F, K, int(outer), _p(z, torch.float32, "z"), _stream()),
           "ctr_pnn_product_fwd")

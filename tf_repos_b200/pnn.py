@@ -20,6 +20,12 @@ class PNN(CTRModel):
         if model_type not in ("FNN", "Inner", "Outer"):
             raise NameError(f"model_type {model_type!r}: deep_inputs is undefined (PNN.py:139-167)")
         self.model_type = model_type
+        if model_type != "FNN":
+            try:
+                ops.pnn_product_check(field_size, embedding_size, model_type == "Outer")
+            except ops.CtrError as e:
+                raise ValueError(f"--embedding_size={embedding_size} with --field_size={field_size} is not supported "
+                                 f"by the {model_type} product kernels: {e}") from None
         self.layers, self.keep = ints(deep_layers), floats(dropout)
         self.batch_norm, self.bn_decay = bool(batch_norm), float(batch_norm_decay)
         super().__init__(field_size, feature_size, embedding_size, batch_size, l2_reg, learning_rate, optimizer,
