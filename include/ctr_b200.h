@@ -450,6 +450,44 @@ size_t ctr_parse_libsvm_device_workspace_bytes(size_t len, int64_t max_rows);
 int ctr_parse_libsvm_device(const char* text, size_t len, int F, int64_t max_rows, int final_chunk, int32_t* ids,
                             float* vals, float* labels, int64_t* info, void* ws, size_t ws_bytes, ctr_stream_t stream);
 
+/* ---- Criteo feature pipeline (deep_ctr/Feature_pipeline/get_criteo_feature.py; DESIGN.md §2.4) ----------------
+ * Raw Criteo TSV -> tr/va/te.libsvm + feature_map, byte for byte.  `text` is a chunk of whole lines (a last line
+ * without '\n' counts), len < 2^30; line_base = index of its first line in the file (error positions are file lines).
+ * Error word (device int64, ~0 = none; the smallest over the file is the one the reference raises first):
+ *   (class << 62) | (line << 16) | (column << 8) | code; class 0 = min/max pass, 1 = dictionary pass; column =
+ *   index into the line's '\t' split; code 1 = too few columns (IndexError), 2 = I value not [+-]?[0-9]+ (ValueError /
+ *   restriction), 3 = |I value| > 2^53, 4 = C value > 8 bytes, 5 = C value holds NUL, 6 = C value is "<unk>"
+ *   (restrictions), 7 = max == min and a non-empty I value (ZeroDivisionError).
+ * table: ctr_criteo_table_bytes(capacity) bytes, zeroed by the caller; open addressing on (field, value), capacity
+ *   slots (<= 2^31).
+ * stats (:74-85 min/max, :39-45 counts; train lines): minmax int64[26] = {min[13], max[13]}, initialised by the caller
+ *   to {sys.maxsize..., -sys.maxsize...} and folded into; info int64[3] = {lines, error word, values dropped because
+ *   no slot was found within min(capacity, 32768) probes -- non-zero means capacity is too small}.
+ * vocab (:46-51): count >= cutoff kept, sorted by (field, -count, value), ids 1..n per field written into the table
+ *   (all other values -> 0 = <unk>).  vocab_keys uint64[capacity]: the kept values field-major in id order, packed
+ *   big-endian and zero-padded; field_counts int64[26].  Run once, after the last stats call.
+ * emit (:127-167): plan then write, over the same text and ws.  test = 0: train lines, to_train uint8[lines] = the
+ *   split decision of each line (:148), column 0 is the label; test = 1: columns shifted by one, every line gets
+ *   label[0, label_len) (the last train line's label, :167).  num_min / num_den double[13] = float(min), float(max -
+ *   min); offsets int64[26] (:119-123).  plan: info int64[5] = {lines, error word, tr lines, tr bytes, va bytes};
+ *   write (only after a plan without error): lines to out_tr (or out_va when to_train is 0), each in input order. */
+size_t ctr_criteo_table_bytes(int64_t capacity);
+size_t ctr_criteo_stats_workspace_bytes(size_t len);
+int ctr_criteo_stats(const char* text, size_t len, int64_t line_base, void* table, int64_t capacity, int64_t* minmax,
+                     int64_t* info, void* ws, size_t ws_bytes, ctr_stream_t stream);
+size_t ctr_criteo_vocab_workspace_bytes(int64_t capacity);
+int ctr_criteo_vocab(void* table, int64_t capacity, int64_t cutoff, uint64_t* vocab_keys, int64_t* field_counts,
+                     void* ws, size_t ws_bytes, ctr_stream_t stream);
+size_t ctr_criteo_emit_workspace_bytes(size_t len);
+int ctr_criteo_emit_plan(const char* text, size_t len, int test, int64_t line_base, const uint8_t* to_train,
+                         const void* table, int64_t capacity, const double* num_min, const double* num_den,
+                         const int64_t* offsets, const char* label, int label_len, int64_t* info, void* ws,
+                         size_t ws_bytes, ctr_stream_t stream);
+int ctr_criteo_emit_write(const char* text, size_t len, int test, const uint8_t* to_train, const void* table,
+                          int64_t capacity, const double* num_min, const double* num_den, const int64_t* offsets,
+                          const char* label, int label_len, char* out_tr, char* out_va, const void* ws,
+                          size_t ws_bytes, ctr_stream_t stream);
+
 /* ---- table initialisation (glorot_normal_initializer, DeepFM.py:115-116; truncated at 2 sigma) --- */
 int ctr_init_trunc_normal(float* t, int64_t n, float stddev, uint64_t seed, ctr_stream_t stream);
 int ctr_fill(float* t, int64_t n, float value, ctr_stream_t stream);

@@ -110,6 +110,14 @@ SIGNATURES = {
     "ctr_libsvm_count_fields": (c_int, [c_char_p, c_size_t]),
     "ctr_parse_libsvm_device_workspace_bytes": (c_size_t, [c_size_t, c_int64]),
     "ctr_parse_libsvm_device": (c_int, [P, c_size_t, c_int, c_int64, c_int, P, P, P, P, P, c_size_t, P]),
+    "ctr_criteo_table_bytes": (c_size_t, [c_int64]),
+    "ctr_criteo_stats_workspace_bytes": (c_size_t, [c_size_t]),
+    "ctr_criteo_stats": (c_int, [P, c_size_t, c_int64, P, c_int64, P, P, P, c_size_t, P]),
+    "ctr_criteo_vocab_workspace_bytes": (c_size_t, [c_int64]),
+    "ctr_criteo_vocab": (c_int, [P, c_int64, c_int64, P, P, P, c_size_t, P]),
+    "ctr_criteo_emit_workspace_bytes": (c_size_t, [c_size_t]),
+    "ctr_criteo_emit_plan": (c_int, [P, c_size_t, c_int, c_int64, P, P, c_int64, P, P, P, P, c_int, P, P, c_size_t, P]),
+    "ctr_criteo_emit_write": (c_int, [P, c_size_t, c_int, P, P, c_int64, P, P, P, P, c_int, P, P, P, c_size_t, P]),
     "ctr_init_trunc_normal": (c_int, [P, c_int64, c_float, c_uint64, P]),
     "ctr_fill": (c_int, [P, c_int64, c_float, P]),
 }

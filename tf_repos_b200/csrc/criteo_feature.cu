@@ -1,0 +1,763 @@
+// criteo_feature.cu -- Criteo raw TSV -> libsvm feature pipeline on the GPU (Feature_pipeline/get_criteo_feature.py).
+//
+// Three passes, each over text chunks cut at line ends (the host reads the files; only the count table and the
+// vocabulary stay resident):
+//   stats  one thread per train line: the 13 integer columns fold their clipped min/max into int64[26] (shared-memory
+//          atomics per CTA, then global atomics: exact and order-free); the 26 categorical values count into an
+//          open-addressing table keyed by (field, 8-byte key).
+//   vocab  keep count >= cutoff, LSD radix sort by (field, -count, key) (13 passes of 8 bits over 104 key bits),
+//          write each id back into its table slot.
+//   emit   plan: one thread per line computes its output length (and raises what the reference raises); the tile
+//          sums are scanned; write: the same thread formats its line at its offset in the tr or va buffer.
+// Every order comes from a sort or a scan, every reduction is an integer one: two runs give the same bytes.
+//
+// Line grammar (get_criteo_feature.py:42,77,135,156): split on '\t' after dropping the '\n'; train lines are
+// label, I1..I13, C1..C26; test lines have no label; columns beyond those are ignored.
+// Restrictions (DESIGN.md §2.4; each raises): I values match [+-]?[0-9]+ with magnitude <= 2^53; train C values are
+// at most 8 bytes, hold no NUL and are not "<unk>", so a value packs big-endian, zero-padded into a uint64 whose
+// numeric order is Python's bytewise string order and 0 never is a key.
+#include "line_starts.cuh"
+
+namespace ctr {
+
+constexpr int CF_NI = 13, CF_NC = 26, CF_COLS = 1 + CF_NI + CF_NC;
+constexpr int CF_THREADS = 256;                       // per-line kernels: one line per thread, one tile per CTA
+constexpr int64_t CF_MAX_PROBE = 1 << 15;             // a key that finds no slot within this many probes overflows
+constexpr uint64_t CF_UNK = 0x3C756E6B3E000000ull;    // "<unk>" packed
+constexpr int64_t CF_MAXSIZE = 0x7FFFFFFFFFFFFFFFll;  // Python 2's sys.maxsize on LP64
+
+__constant__ int64_t kClip[CF_NI] = {20, 600, 100, 50, 64000, 500, 100, 50, 500, 10, 10, 10, 50};
+
+// error word: (class << 62) | (line << 16) | (column << 8) | code; the smallest one wins (atomicMin).  class 0 = the
+// reference's min/max pass (continuous columns), class 1 = its dictionary pass, so a min/max error anywhere in the
+// file comes first, as it does in the reference.
+enum { CF_E_COLUMNS = 1, CF_E_NOT_INT = 2, CF_E_RANGE = 3, CF_E_KEY_LONG = 4, CF_E_KEY_NUL = 5, CF_E_KEY_UNK = 6,
+       CF_E_ZERO_DIV = 7 };
+__device__ __forceinline__ uint64_t cf_err(int cls, int64_t line, int col, int code) {
+  return ((uint64_t)cls << 62) | ((uint64_t)line << 16) | ((uint64_t)col << 8) | (uint64_t)code;
+}
+
+// ---- count table: keys uint64[cap] | tags uint32[cap] (field + 1, 0 = empty) | vals uint32[cap] ----------------
+// vals holds the count after the stats pass and the id (0 = <unk>) after the vocab pass.
+struct CfTable {
+  uint64_t* keys;
+  uint32_t* tags;
+  uint32_t* vals;
+  int64_t cap;
+  CfTable() = default;
+  __host__ __device__ CfTable(void* base, int64_t c)
+      : keys(reinterpret_cast<uint64_t*>(base)),
+        tags(reinterpret_cast<uint32_t*>(reinterpret_cast<uint64_t*>(base) + c)),
+        vals(reinterpret_cast<uint32_t*>(reinterpret_cast<uint64_t*>(base) + c) + c),
+        cap(c) {}
+};
+
+__device__ __forceinline__ uint64_t cf_home(uint64_t key, int f, int64_t cap) {
+  uint64_t x = key ^ ((uint64_t)(f + 1) * 0x9E3779B97F4A7C15ull);   // splitmix64 finaliser
+  x ^= x >> 30; x *= 0xBF58476D1CE4E5B9ull;
+  x ^= x >> 27; x *= 0x94D049BB133111EBull;
+  x ^= x >> 31;
+  return __umul64hi(x, (uint64_t)cap);
+}
+
+// Linear probing without locks: a slot's key is set once (CAS 0 -> key), then its tag once (CAS 0 -> field + 1).
+// Every thread inserting (f, key) takes the same decision at every slot it visits (both words are final once
+// non-zero), so all of them end in the same slot.
+__device__ __forceinline__ bool cf_insert(const CfTable& T, uint64_t key, int f) {
+  const uint32_t tag = (uint32_t)f + 1;
+  uint64_t s = cf_home(key, f, T.cap);
+  const int64_t probes = T.cap < CF_MAX_PROBE ? T.cap : CF_MAX_PROBE;
+  for (int64_t i = 0; i < probes; ++i) {
+    uint64_t k = *reinterpret_cast<volatile uint64_t*>(T.keys + s);
+    if (k == 0) {
+      k = atomicCAS(reinterpret_cast<unsigned long long*>(T.keys + s), 0ull, (unsigned long long)key);
+      if (k == 0) k = key;
+    }
+    if (k == key) {
+      uint32_t t = *reinterpret_cast<volatile uint32_t*>(T.tags + s);
+      if (t == 0) {
+        t = atomicCAS(T.tags + s, 0u, tag);
+        if (t == 0) t = tag;
+      }
+      if (t == tag) { atomicAdd(T.vals + s, 1u); return true; }
+    }
+    if (++s == (uint64_t)T.cap) s = 0;
+  }
+  return false;
+}
+
+__device__ __forceinline__ uint32_t cf_lookup(const CfTable& T, uint64_t key, int f) {
+  const uint32_t tag = (uint32_t)f + 1;
+  uint64_t s = cf_home(key, f, T.cap);
+  const int64_t probes = T.cap < CF_MAX_PROBE ? T.cap : CF_MAX_PROBE;
+  for (int64_t i = 0; i < probes; ++i) {
+    const uint64_t k = T.keys[s];
+    if (k == 0) return 0;
+    if (k == key && T.tags[s] == tag) return T.vals[s];
+    if (++s == (uint64_t)T.cap) s = 0;
+  }
+  return 0;
+}
+
+// ---- tokens --------------------------------------------------------------------------------------------------
+// [+-]?[0-9]+ with magnitude <= 2^53 -> 0 and (neg, mag); CF_E_NOT_INT / CF_E_RANGE otherwise
+__device__ __forceinline__ int cf_parse_int(const unsigned char* __restrict__ t, int64_t q, int64_t e, bool& neg,
+                                            int64_t& mag) {
+  neg = false;
+  if (q < e && (t[q] == '+' || t[q] == '-')) { neg = t[q] == '-'; ++q; }
+  if (q == e) return CF_E_NOT_INT;
+  mag = 0;
+  bool big = false;
+  for (; q < e; ++q) {
+    const unsigned d = (unsigned)t[q] - '0';
+    if (d > 9) return CF_E_NOT_INT;
+    if (!big) { mag = mag * 10 + d; big = mag > (1ll << 53); }
+  }
+  return big ? CF_E_RANGE : 0;
+}
+
+// value of [q, e) packed big-endian and zero-padded -> 0, or the restriction it breaks
+__device__ __forceinline__ int cf_pack_key(const unsigned char* __restrict__ t, int64_t q, int64_t e, uint64_t& key) {
+  if (e - q > 8) return CF_E_KEY_LONG;
+  key = 0;
+  for (int i = 0; q + i < e; ++i) {
+    const unsigned c = t[q + i];
+    if (c == 0) return CF_E_KEY_NUL;
+    key |= (uint64_t)c << (56 - 8 * i);
+  }
+  return key == CF_UNK ? CF_E_KEY_UNK : 0;
+}
+
+__device__ __forceinline__ int64_t cf_col_end(const unsigned char* __restrict__ t, int64_t q, int64_t e) {
+  while (q < e && t[q] != '\t') ++q;
+  return q;
+}
+
+// line `row` of the chunk: [p, e), '\n' dropped
+__device__ __forceinline__ void cf_line(const unsigned char* __restrict__ text, int64_t len,
+                                        const int64_t* __restrict__ line_start, int64_t nn, int64_t row, int64_t& p,
+                                        int64_t& e) {
+  p = line_start[row];
+  e = row < nn ? line_start[row + 1] - 1 : len;
+}
+
+__device__ __forceinline__ int64_t cf_n_lines(const unsigned char* __restrict__ text, int64_t len, int64_t nn) {
+  return nn + ((len > 0 && text[len - 1] != '\n') ? 1 : 0);
+}
+
+// ---- formatting ----------------------------------------------------------------------------------------------
+template <bool W>
+__device__ __forceinline__ int cf_put_u64(uint64_t v, char* o) {
+  int nd = 1;
+  for (uint64_t x = v; x >= 10; x /= 10) ++nd;
+  if (W)
+    for (int i = nd - 1; i >= 0; --i) { o[i] = (char)('0' + v % 10); v /= 10; }
+  return nd;
+}
+
+// "{:.6f}".format(q).rstrip('0').rstrip('.'): the exact binary value of q rounded half-to-even at 1e-6.
+// q = m * 2^s; the integer part is m >> -s and the fraction fm / 2^-s is scaled by 10^6 in 128-bit integers.
+// In this pipeline |q| < 2^55 (|v - min| <= 2^54, |max - min| >= 1; min = sys.maxsize gives |q| ~ 0.5).
+template <bool W>
+__device__ __forceinline__ int cf_put_fixed6(double q, char* o) {
+  const uint64_t bits = (uint64_t)__double_as_longlong(q);
+  const int ex = (int)((bits >> 52) & 0x7FF);
+  const uint64_t m = (bits & 0xFFFFFFFFFFFFFull) | (ex ? (1ull << 52) : 0ull);
+  const int s = (ex ? ex : 1) - 1075;
+  uint64_t ip, fr = 0;
+  if (s >= 0) {
+    ip = m << s;
+  } else {
+    const int r = -s;
+    uint64_t fm;
+    if (r < 64) { ip = m >> r; fm = m & ((1ull << r) - 1); } else { ip = 0; fm = m; }
+    if (r < 100) {   // fm * 10^6 < 2^73: from 2^-100 down the scaled fraction is below one half (and no tie)
+      const unsigned __int128 F = (unsigned __int128)fm * 1000000u;
+      const unsigned __int128 qq = F >> r, rem = F - (qq << r), half = (unsigned __int128)1 << (r - 1);
+      fr = (uint64_t)qq;
+      if (rem > half || (rem == half && (fr & 1))) ++fr;   // 10^6 is even: the parity of the whole result is fr's
+      if (fr == 1000000) { fr = 0; ++ip; }
+    }
+  }
+  int n = 0;
+  if (bits >> 63) { if (W) o[n] = '-'; ++n; }
+  n += cf_put_u64<W>(ip, o + n);
+  if (fr) {
+    int nd = 6;
+    while (fr % 10 == 0) { fr /= 10; --nd; }
+    if (W) {
+      o[n] = '.';
+      for (int i = nd; i >= 1; --i) { o[n + i] = (char)('0' + fr % 10); fr /= 10; }
+    }
+    n += 1 + nd;
+  }
+  return n;
+}
+
+struct CfEmitArgs {
+  CfTable table;
+  const double* num_min;    // [13] float(min_i)
+  const double* num_den;    // [13] float(max_i - min_i)
+  const int64_t* offsets;   // [26] categorical offsets (offset[0] = 13)
+  const char* label;        // test mode: the label every line gets
+  int label_len;
+  int test;
+};
+
+// One output line (get_criteo_feature.py:135-151 train, :156-167 test).  Returns its length; W = write it to o.
+// Sets err (plan pass) for what the reference raises on this line: IndexError (too few columns), ValueError (I value
+// not an integer; here also the restriction), ZeroDivisionError (max == min and a non-empty I value).
+template <bool W>
+__device__ int64_t cf_emit_line(const unsigned char* __restrict__ t, int64_t p, int64_t e, const CfEmitArgs& a,
+                                int64_t line, uint64_t& err, char* o) {
+  int64_t n = 0;
+  const int shift = a.test ? 1 : 0, ncols = CF_COLS - shift;
+  if (a.test) {
+    if (W) for (int i = 0; i < a.label_len; ++i) o[i] = a.label[i];
+    n = a.label_len;
+  }
+  int col = 0;
+  int64_t q = p;
+  for (;;) {
+    const int64_t ce = cf_col_end(t, q, e);
+    const int j = col + shift;   // 0 = label, 1..13 = I, 14..39 = C
+    if (j == 0) {
+      if (W) for (int64_t i = q; i < ce; ++i) o[n + i - q] = (char)t[i];
+      n += ce - q;
+    } else if (j <= CF_NI) {
+      if (W) o[n] = ' ';
+      n += 1 + cf_put_u64<W>((uint64_t)j, o + n + 1);
+      if (W) o[n] = ':';
+      ++n;
+      double v = 0.0;
+      if (ce > q) {
+        bool neg;
+        int64_t mag;
+        const int code = cf_parse_int(t, q, ce, neg, mag);
+        if (code) { err = cf_err(0, line, col, code); return n; }
+        const double den = a.num_den[j - 1];
+        if (den == 0.0) { err = cf_err(0, line, col, CF_E_ZERO_DIV); return n; }
+        const double x = neg ? -(double)mag : (double)mag;   // float("-0") is -0.0
+        v = __ddiv_rn(__dsub_rn(x, a.num_min[j - 1]), den);
+      }
+      n += cf_put_fixed6<W>(v, o + n);
+    } else {
+      const int f = j - 1 - CF_NI;
+      uint64_t key;
+      // values the train dictionary cannot hold (empty, > 8 bytes, NUL, "<unk>") are <unk> = 0, as in the reference
+      const uint32_t id = (ce > q && cf_pack_key(t, q, ce, key) == 0) ? cf_lookup(a.table, key, f) : 0u;
+      if (W) o[n] = ' ';
+      n += 1 + cf_put_u64<W>((uint64_t)(a.offsets[f] + id), o + n + 1);
+      if (W) { o[n] = ':'; o[n + 1] = '1'; }
+      n += 2;
+    }
+    ++col;
+    if (ce >= e || col == ncols) break;
+    q = ce + 1;
+  }
+  if (col < ncols) { err = cf_err(0, line, col, CF_E_COLUMNS); return n; }
+  if (W) o[n] = '\n';
+  return n + 1;
+}
+
+// ---- kernels -------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(CF_THREADS) cf_stats_kernel(const unsigned char* __restrict__ t, int64_t len,
+                                                             const int64_t* __restrict__ line_start,
+                                                             const int64_t* __restrict__ n_newlines, int64_t line_base,
+                                                             CfTable table, int64_t* __restrict__ minmax,
+                                                             int64_t* __restrict__ info) {
+  __shared__ long long smin[CF_NI], smax[CF_NI];
+  if (threadIdx.x < CF_NI) { smin[threadIdx.x] = CF_MAXSIZE; smax[threadIdx.x] = -CF_MAXSIZE; }
+  __syncthreads();
+  const int64_t nn = n_newlines[0], n_lines = cf_n_lines(t, len, nn);
+  if (blockIdx.x == 0 && threadIdx.x == 0) info[0] = n_lines;
+  for (int64_t row = (int64_t)blockIdx.x * CF_THREADS + threadIdx.x; row < n_lines;
+       row += (int64_t)gridDim.x * CF_THREADS) {
+    int64_t p, e;
+    cf_line(t, len, line_start, nn, row, p, e);
+    const int64_t line = line_base + row;
+    uint64_t err = ~0ull;
+    int col = 0;
+    int64_t q = p;
+    for (;;) {
+      const int64_t ce = cf_col_end(t, q, e);
+      if (col >= 1 && col <= CF_NI) {   // :77-85
+        if (ce > q) {
+          bool neg;
+          int64_t mag;
+          const int code = cf_parse_int(t, q, ce, neg, mag);
+          if (code) { err = cf_err(0, line, col, code); break; }
+          int64_t v = neg ? -mag : mag;
+          if (v > kClip[col - 1]) v = kClip[col - 1];
+          atomicMin(&smin[col - 1], (long long)v);
+          atomicMax(&smax[col - 1], (long long)v);
+        }
+      } else if (col > CF_NI && ce > q) {   // :42-45
+        uint64_t key;
+        const int code = cf_pack_key(t, q, ce, key);
+        if (code) { err = cf_err(1, line, col, code); break; }
+        if (!cf_insert(table, key, col - 1 - CF_NI))
+          atomicAdd(reinterpret_cast<unsigned long long*>(&info[2]), 1ull);
+      }
+      ++col;
+      if (ce >= e || col == CF_COLS) break;
+      q = ce + 1;
+    }
+    if (err == ~0ull && col < CF_COLS) err = cf_err(col <= CF_NI ? 0 : 1, line, col, CF_E_COLUMNS);
+    if (err != ~0ull) atomicMin(reinterpret_cast<unsigned long long*>(&info[1]), (unsigned long long)err);
+  }
+  __syncthreads();
+  if (threadIdx.x < CF_NI) {
+    atomicMin(reinterpret_cast<long long*>(&minmax[threadIdx.x]), smin[threadIdx.x]);
+    atomicMax(reinterpret_cast<long long*>(&minmax[CF_NI + threadIdx.x]), smax[threadIdx.x]);
+  }
+}
+
+// exclusive scan of a[0, *count) in place (one CTA, tiles of 1024); total -> *total
+template <typename T>
+__global__ void __launch_bounds__(1024) cf_scan_kernel(T* __restrict__ a, const int64_t* __restrict__ count,
+                                                       int64_t* __restrict__ total) {
+  __shared__ int64_t warp_sum_s[32];
+  __shared__ int64_t carry_s;
+  const int64_t n = count[0];
+  if (threadIdx.x == 0) carry_s = 0;
+  __syncthreads();
+  for (int64_t base = 0; base < n; base += 1024) {
+    const int64_t i = base + threadIdx.x;
+    const int64_t v = i < n ? (int64_t)a[i] : 0;
+    int64_t x = v;
+    for (int o = 1; o < 32; o <<= 1) {
+      const int64_t y = __shfl_up_sync(FULL_MASK, x, o);
+      if ((threadIdx.x & 31) >= o) x += y;
+    }
+    if ((threadIdx.x & 31) == 31) warp_sum_s[threadIdx.x >> 5] = x;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+      int64_t w = warp_sum_s[threadIdx.x];
+      for (int o = 1; o < 32; o <<= 1) {
+        const int64_t y = __shfl_up_sync(FULL_MASK, w, o);
+        if (threadIdx.x >= o) w += y;
+      }
+      warp_sum_s[threadIdx.x] = w;
+    }
+    __syncthreads();
+    const int64_t before = carry_s + (threadIdx.x >= 32 ? warp_sum_s[(threadIdx.x >> 5) - 1] : 0) + (x - v);
+    if (i < n) a[i] = (T)before;
+    __syncthreads();
+    if (threadIdx.x == 1023) carry_s = before + v;
+    __syncthreads();
+  }
+  if (threadIdx.x == 0 && total) total[0] = carry_s;
+}
+
+// CTA-wide exclusive scan of two int64 values (CF_THREADS threads); returns the CTA totals through s_a / s_b
+__device__ __forceinline__ void cf_block_scan2(int64_t& a, int64_t& b, int64_t& s_a, int64_t& s_b) {
+  __shared__ int64_t wa[CF_THREADS / 32], wb[CF_THREADS / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int64_t xa = a, xb = b;
+  for (int o = 1; o < 32; o <<= 1) {
+    const int64_t ya = __shfl_up_sync(FULL_MASK, xa, o), yb = __shfl_up_sync(FULL_MASK, xb, o);
+    if (lane >= o) { xa += ya; xb += yb; }
+  }
+  if (lane == 31) { wa[warp] = xa; wb[warp] = xb; }
+  __syncthreads();
+  int64_t ba = 0, bb = 0;
+  s_a = 0; s_b = 0;
+  for (int w = 0; w < CF_THREADS / 32; ++w) {
+    if (w < warp) { ba += wa[w]; bb += wb[w]; }
+    s_a += wa[w]; s_b += wb[w];
+  }
+  a = ba + xa - a;
+  b = bb + xb - b;
+  __syncthreads();
+}
+
+// per line: output length; per tile of CF_THREADS lines: tr bytes, va bytes, tr lines
+__global__ void __launch_bounds__(CF_THREADS) cf_plan_kernel(const unsigned char* __restrict__ t, int64_t len,
+                                                            const int64_t* __restrict__ line_start,
+                                                            const int64_t* __restrict__ n_newlines, int64_t line_base,
+                                                            const uint8_t* __restrict__ to_train, CfEmitArgs a,
+                                                            int32_t* __restrict__ line_len, int64_t* __restrict__ tile_tr,
+                                                            int64_t* __restrict__ tile_va, int64_t* __restrict__ tile_trn,
+                                                            int64_t* __restrict__ n_tiles, int64_t* __restrict__ info) {
+  const int64_t nn = n_newlines[0], n_lines = cf_n_lines(t, len, nn);
+  if (blockIdx.x == 0 && threadIdx.x == 0) { info[0] = n_lines; n_tiles[0] = (n_lines + CF_THREADS - 1) / CF_THREADS; }
+  for (int64_t tile = blockIdx.x; tile * CF_THREADS < n_lines; tile += gridDim.x) {
+    const int64_t row = tile * CF_THREADS + threadIdx.x;
+    int64_t L = 0;
+    bool tr = true;
+    if (row < n_lines) {
+      int64_t p, e;
+      cf_line(t, len, line_start, nn, row, p, e);
+      uint64_t err = ~0ull;
+      L = cf_emit_line<false>(t, p, e, a, line_base + row, err, nullptr);
+      if (err != ~0ull) atomicMin(reinterpret_cast<unsigned long long*>(&info[1]), (unsigned long long)err);
+      line_len[row] = (int32_t)L;
+      tr = a.test || to_train[row];
+    }
+    int64_t x_tr = tr ? L : 0, x_va = tr ? 0 : L, s_tr, s_va;
+    cf_block_scan2(x_tr, x_va, s_tr, s_va);
+    const int n_tr = __syncthreads_count(row < n_lines && tr);
+    if (threadIdx.x == 0) { tile_tr[tile] = s_tr; tile_va[tile] = s_va; tile_trn[tile] = n_tr; }
+  }
+}
+
+__global__ void __launch_bounds__(CF_THREADS) cf_write_kernel(const unsigned char* __restrict__ t, int64_t len,
+                                                             const int64_t* __restrict__ line_start,
+                                                             const int64_t* __restrict__ n_newlines,
+                                                             const uint8_t* __restrict__ to_train, CfEmitArgs a,
+                                                             const int32_t* __restrict__ line_len,
+                                                             const int64_t* __restrict__ tile_tr,
+                                                             const int64_t* __restrict__ tile_va, char* __restrict__ out_tr,
+                                                             char* __restrict__ out_va) {
+  const int64_t nn = n_newlines[0], n_lines = cf_n_lines(t, len, nn);
+  for (int64_t tile = blockIdx.x; tile * CF_THREADS < n_lines; tile += gridDim.x) {
+    const int64_t row = tile * CF_THREADS + threadIdx.x;
+    const bool live = row < n_lines, tr = !live || a.test || to_train[row];
+    const int64_t L = live ? line_len[row] : 0;
+    int64_t x_tr = tr ? L : 0, x_va = tr ? 0 : L, s_tr, s_va;
+    cf_block_scan2(x_tr, x_va, s_tr, s_va);
+    if (live) {
+      int64_t p, e;
+      cf_line(t, len, line_start, nn, row, p, e);
+      uint64_t err = ~0ull;
+      char* o = tr ? out_tr + tile_tr[tile] + x_tr : out_va + tile_va[tile] + x_va;
+      cf_emit_line<true>(t, p, e, a, row, err, o);
+    }
+  }
+}
+
+// ---- vocabulary ----------------------------------------------------------------------------------------------
+constexpr int VC_TILE = 16 * CF_THREADS;   // items per CTA in the radix passes
+constexpr int VC_PASSES = 13;              // 8 digits of the key, then 5 of (field << 32 | ~count)
+
+// kept slots -> (lo = key, hi = field << 32 | ~count, slot); vals are cleared to the <unk> id 0
+__global__ void __launch_bounds__(CF_THREADS) vc_compact_kernel(CfTable T, int64_t cutoff, uint64_t* __restrict__ lo,
+                                                               uint64_t* __restrict__ hi, uint32_t* __restrict__ sl,
+                                                               int64_t* __restrict__ n_kept,
+                                                               int64_t* __restrict__ field_counts) {
+  __shared__ int cnt[CF_NC];
+  if (threadIdx.x < CF_NC) cnt[threadIdx.x] = 0;
+  __syncthreads();
+  const int64_t stride = (int64_t)gridDim.x * CF_THREADS, n_iter = (T.cap + stride - 1) / stride;
+  for (int64_t it = 0; it < n_iter; ++it) {   // uniform trip count: the warp-aggregated atomic below needs whole warps
+    const int64_t s = (it * gridDim.x + blockIdx.x) * CF_THREADS + threadIdx.x;
+    bool keep = false;
+    uint32_t tag = 0, c = 0;
+    if (s < T.cap) {
+      tag = T.tags[s];
+      if (tag) {
+        c = T.vals[s];
+        T.vals[s] = 0;
+        keep = (int64_t)c >= cutoff;
+      }
+    }
+    const uint32_t ballot = __ballot_sync(FULL_MASK, keep);
+    unsigned long long base = 0;
+    if ((threadIdx.x & 31) == 0 && ballot)
+      base = atomicAdd(reinterpret_cast<unsigned long long*>(n_kept), (unsigned long long)__popc(ballot));
+    base = __shfl_sync(FULL_MASK, base, 0);
+    if (keep) {
+      const int64_t pos = (int64_t)base + __popc(ballot & ((1u << (threadIdx.x & 31)) - 1));
+      lo[pos] = T.keys[s];
+      hi[pos] = ((uint64_t)(tag - 1) << 32) | (uint64_t)(0xFFFFFFFFu - c);
+      sl[pos] = (uint32_t)s;
+      atomicAdd(&cnt[tag - 1], 1);
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x < CF_NC && cnt[threadIdx.x])
+    atomicAdd(reinterpret_cast<unsigned long long*>(&field_counts[threadIdx.x]), (unsigned long long)cnt[threadIdx.x]);
+}
+
+__device__ __forceinline__ int vc_digit(uint64_t lo, uint64_t hi, int pass) {
+  return (int)(((pass < 8 ? lo >> (8 * pass) : hi >> (8 * (pass - 8)))) & 0xFF);
+}
+
+// hist[d * nb + b] = items of CTA b with digit d; nb = ceil(n / VC_TILE)
+__global__ void __launch_bounds__(CF_THREADS) vc_hist_kernel(const uint64_t* __restrict__ lo, const uint64_t* __restrict__ hi,
+                                                            const int64_t* __restrict__ n_kept, int pass,
+                                                            int32_t* __restrict__ hist, int64_t* __restrict__ hist_count) {
+  __shared__ int h[256];
+  const int64_t n = n_kept[0], nb = (n + VC_TILE - 1) / VC_TILE;
+  if (blockIdx.x == 0 && threadIdx.x == 0) hist_count[0] = 256 * nb;
+  if (blockIdx.x >= nb) return;
+  h[threadIdx.x] = 0;
+  __syncthreads();
+  for (int r = 0; r < VC_TILE / CF_THREADS; ++r) {
+    const int64_t i = (int64_t)blockIdx.x * VC_TILE + r * CF_THREADS + threadIdx.x;
+    if (i < n) atomicAdd(&h[vc_digit(lo[i], hi[i], pass)], 1);
+  }
+  __syncthreads();
+  hist[(int64_t)threadIdx.x * nb + blockIdx.x] = h[threadIdx.x];
+}
+
+// stable scatter by digit: within a CTA the items go in index order (warp match + per-warp digit counts)
+__global__ void __launch_bounds__(CF_THREADS) vc_scatter_kernel(const uint64_t* __restrict__ lo, const uint64_t* __restrict__ hi,
+                                                               const uint32_t* __restrict__ sl,
+                                                               const int64_t* __restrict__ n_kept, int pass,
+                                                               const int32_t* __restrict__ hist, uint64_t* __restrict__ lo2,
+                                                               uint64_t* __restrict__ hi2, uint32_t* __restrict__ sl2) {
+  constexpr int NW = CF_THREADS / 32;
+  __shared__ int base[256];
+  __shared__ int wcnt[NW][256];
+  const int64_t n = n_kept[0], nb = (n + VC_TILE - 1) / VC_TILE;
+  if (blockIdx.x >= nb) return;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  base[threadIdx.x] = hist[(int64_t)threadIdx.x * nb + blockIdx.x];
+  for (int w = 0; w < NW; ++w) wcnt[w][threadIdx.x] = 0;
+  __syncthreads();
+  for (int r = 0; r < VC_TILE / CF_THREADS; ++r) {
+    const int64_t i = (int64_t)blockIdx.x * VC_TILE + r * CF_THREADS + threadIdx.x;
+    const bool live = i < n;
+    uint64_t l = 0, h = 0;
+    uint32_t s = 0;
+    int d = 256;   // no digit: dead lanes match only each other and are not counted
+    if (live) { l = lo[i]; h = hi[i]; s = sl[i]; d = vc_digit(l, h, pass); }
+    const uint32_t peers = __match_any_sync(FULL_MASK, d);
+    const int rank = __popc(peers & ((1u << lane) - 1));
+    if (live && rank == 0) wcnt[warp][d] = __popc(peers);
+    __syncthreads();
+    if (live) {
+      int pos = base[d] + rank;
+      for (int w = 0; w < warp; ++w) pos += wcnt[w][d];
+      lo2[pos] = l; hi2[pos] = h; sl2[pos] = s;
+    }
+    __syncthreads();
+    int add = 0;
+    for (int w = 0; w < NW; ++w) { add += wcnt[w][threadIdx.x]; wcnt[w][threadIdx.x] = 0; }
+    base[threadIdx.x] += add;
+    __syncthreads();
+  }
+}
+
+// sorted position p of field f -> id p - start(f) + 1, written into the slot; keys -> vocab_keys
+__global__ void __launch_bounds__(CF_THREADS) vc_assign_kernel(CfTable T, const uint64_t* __restrict__ lo,
+                                                              const uint64_t* __restrict__ hi, const uint32_t* __restrict__ sl,
+                                                              const int64_t* __restrict__ n_kept,
+                                                              const int64_t* __restrict__ field_counts,
+                                                              uint64_t* __restrict__ vocab_keys) {
+  __shared__ int64_t start[CF_NC];
+  if (threadIdx.x == 0) {
+    int64_t s = 0;
+    for (int f = 0; f < CF_NC; ++f) { start[f] = s; s += field_counts[f]; }
+  }
+  __syncthreads();
+  const int64_t n = n_kept[0];
+  for (int64_t p = (int64_t)blockIdx.x * CF_THREADS + threadIdx.x; p < n; p += (int64_t)gridDim.x * CF_THREADS) {
+    const int f = (int)(hi[p] >> 32);
+    T.vals[sl[p]] = (uint32_t)(p - start[f] + 1);
+    vocab_keys[p] = lo[p];
+  }
+}
+
+// ---- workspace layouts -----------------------------------------------------------------------------------------
+static inline size_t cf_align(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// line starts of a chunk: block_counts int32[nb] | n_newlines int64[2] | line_start int64[len + 2]
+struct CfLines {
+  int32_t* block_counts;
+  int64_t* n_newlines;
+  int64_t* line_start;
+  int n_blocks;
+  size_t bytes;
+  CfLines(void* ws, size_t len) {
+    uint8_t* b = reinterpret_cast<uint8_t*>(ws);
+    n_blocks = (int)((len + LS_BLOCK_BYTES - 1) / LS_BLOCK_BYTES);
+    size_t o = 0;
+    block_counts = reinterpret_cast<int32_t*>(b + o); o += cf_align((size_t)n_blocks * 4);
+    n_newlines = reinterpret_cast<int64_t*>(b + o); o += cf_align(16);
+    line_start = reinterpret_cast<int64_t*>(b + o); o += cf_align((len + 2) * 8);
+    bytes = o;
+  }
+};
+
+// emit: CfLines | line_len int32[len + 1] | tile_tr, tile_va, tile_trn int64[nt] | n_tiles int64[2]
+struct CfEmitWs {
+  CfLines lines;
+  int32_t* line_len;
+  int64_t *tile_tr, *tile_va, *tile_trn, *n_tiles;
+  size_t bytes;
+  CfEmitWs(void* ws, size_t len) : lines(ws, len) {
+    uint8_t* b = reinterpret_cast<uint8_t*>(ws);
+    const size_t nt = (len + 1 + CF_THREADS - 1) / CF_THREADS;
+    size_t o = lines.bytes;
+    line_len = reinterpret_cast<int32_t*>(b + o); o += cf_align((len + 1) * 4);
+    tile_tr = reinterpret_cast<int64_t*>(b + o); o += cf_align(nt * 8);
+    tile_va = reinterpret_cast<int64_t*>(b + o); o += cf_align(nt * 8);
+    tile_trn = reinterpret_cast<int64_t*>(b + o); o += cf_align(nt * 8);
+    n_tiles = reinterpret_cast<int64_t*>(b + o); o += cf_align(16);
+    bytes = o;
+  }
+};
+
+// vocab: n_kept, hist_count int64 | hist int32[256 * nb] | lo, hi uint64[2][cap] | sl uint32[2][cap]
+struct CfVocabWs {
+  int64_t *n_kept, *hist_count;
+  int32_t* hist;
+  uint64_t *lo[2], *hi[2];
+  uint32_t* sl[2];
+  size_t bytes;
+  CfVocabWs(void* ws, int64_t cap) {
+    uint8_t* b = reinterpret_cast<uint8_t*>(ws);
+    const size_t nb = (size_t)ceil_div64(cap, VC_TILE), c = (size_t)cap;
+    size_t o = 0;
+    n_kept = reinterpret_cast<int64_t*>(b + o); hist_count = n_kept + 1; o += cf_align(16);
+    hist = reinterpret_cast<int32_t*>(b + o); o += cf_align(256 * nb * 4);
+    for (int k = 0; k < 2; ++k) { lo[k] = reinterpret_cast<uint64_t*>(b + o); o += cf_align(c * 8); }
+    for (int k = 0; k < 2; ++k) { hi[k] = reinterpret_cast<uint64_t*>(b + o); o += cf_align(c * 8); }
+    for (int k = 0; k < 2; ++k) { sl[k] = reinterpret_cast<uint32_t*>(b + o); o += cf_align(c * 4); }
+    bytes = o;
+  }
+};
+
+// chunk buffers the per-line kernels accept: len < 2^30 keeps block offsets and line lengths in int32
+constexpr size_t CF_MAX_LEN = (size_t)1 << 30;
+constexpr int64_t CF_MAX_CAP = (int64_t)1 << 31;   // slot numbers are uint32, sort positions int32
+
+static int cf_line_starts(const unsigned char* t, size_t len, const CfLines& L, cudaStream_t st, const char* what) {
+  ls_count_kernel<<<L.n_blocks, LS_THREADS, 0, st>>>(t, (int64_t)len, L.block_counts);
+  CTR_LAUNCHED(what);
+  ls_scan_kernel<<<1, 1024, 0, st>>>(L.block_counts, L.n_blocks, L.n_newlines);
+  CTR_LAUNCHED(what);
+  ls_emit_kernel<<<L.n_blocks, LS_THREADS, 0, st>>>(t, (int64_t)len, L.block_counts, (int64_t)len + 1, L.line_start);
+  CTR_LAUNCHED(what);
+  return CTR_OK;
+}
+
+static unsigned cf_grid(int64_t items) {
+  const int64_t want = ceil_div64(items, CF_THREADS), cap = (int64_t)sm_count() * 16;
+  return (unsigned)(want < 1 ? 1 : (want < cap ? want : cap));
+}
+
+}  // namespace ctr
+
+using namespace ctr;
+
+extern "C" {
+
+size_t ctr_criteo_table_bytes(int64_t capacity) { return capacity > 0 ? (size_t)capacity * 16 : 0; }
+
+size_t ctr_criteo_stats_workspace_bytes(size_t len) { return CfLines(nullptr, len).bytes; }
+
+int ctr_criteo_stats(const char* text, size_t len, int64_t line_base, void* table, int64_t capacity, int64_t* minmax,
+                     int64_t* info, void* ws, size_t ws_bytes, ctr_stream_t stream) {
+  CTR_REQUIRE(info && minmax && table && capacity > 0 && line_base >= 0 && (len == 0 || text), CTR_ERR_INVALID_ARG,
+              "ctr_criteo_stats: bad arguments");
+  CTR_REQUIRE(capacity <= CF_MAX_CAP, CTR_ERR_INVALID_ARG, "ctr_criteo_stats: capacity > 2^31");
+  CTR_REQUIRE(len < CF_MAX_LEN, CTR_ERR_INVALID_ARG, "ctr_criteo_stats: chunk too large (len < 2^30)");
+  CTR_REQUIRE(ws && ws_bytes >= ctr_criteo_stats_workspace_bytes(len), CTR_ERR_WORKSPACE,
+              "ctr_criteo_stats: workspace too small");
+  cudaStream_t st = as_stream(stream);
+  CTR_REQUIRE(cudaMemsetAsync(info, 0, 3 * sizeof(int64_t), st) == cudaSuccess &&
+                  cudaMemsetAsync(info + 1, 0xFF, sizeof(int64_t), st) == cudaSuccess,
+              CTR_ERR_CUDA, "ctr_criteo_stats: memset failed");
+  if (len == 0) return CTR_OK;
+  const unsigned char* t = reinterpret_cast<const unsigned char*>(text);
+  CfLines L(ws, len);
+  if (int rc = cf_line_starts(t, len, L, st, "ctr_criteo_stats(lines)")) return rc;
+  cf_stats_kernel<<<cf_grid((int64_t)len + 1), CF_THREADS, 0, st>>>(t, (int64_t)len, L.line_start, L.n_newlines,
+                                                                    line_base, CfTable(table, capacity), minmax, info);
+  CTR_LAUNCHED("ctr_criteo_stats");
+  return CTR_OK;
+}
+
+size_t ctr_criteo_vocab_workspace_bytes(int64_t capacity) {
+  return capacity > 0 ? CfVocabWs(nullptr, capacity).bytes : 0;
+}
+
+int ctr_criteo_vocab(void* table, int64_t capacity, int64_t cutoff, uint64_t* vocab_keys, int64_t* field_counts,
+                     void* ws, size_t ws_bytes, ctr_stream_t stream) {
+  CTR_REQUIRE(table && capacity > 0 && vocab_keys && field_counts, CTR_ERR_INVALID_ARG, "ctr_criteo_vocab: bad arguments");
+  CTR_REQUIRE(capacity <= CF_MAX_CAP, CTR_ERR_INVALID_ARG, "ctr_criteo_vocab: capacity > 2^31");
+  CTR_REQUIRE(ws && ws_bytes >= ctr_criteo_vocab_workspace_bytes(capacity), CTR_ERR_WORKSPACE,
+              "ctr_criteo_vocab: workspace too small");
+  cudaStream_t st = as_stream(stream);
+  CfVocabWs V(ws, capacity);
+  CfTable T(table, capacity);
+  CTR_REQUIRE(cudaMemsetAsync(V.n_kept, 0, 16, st) == cudaSuccess &&
+                  cudaMemsetAsync(field_counts, 0, CF_NC * sizeof(int64_t), st) == cudaSuccess,
+              CTR_ERR_CUDA, "ctr_criteo_vocab: memset failed");
+  vc_compact_kernel<<<cf_grid(capacity), CF_THREADS, 0, st>>>(T, cutoff, V.lo[0], V.hi[0], V.sl[0], V.n_kept,
+                                                             field_counts);
+  CTR_LAUNCHED("ctr_criteo_vocab(compact)");
+  const unsigned nb = (unsigned)ceil_div64(capacity, VC_TILE);
+  int cur = 0;
+  for (int pass = 0; pass < VC_PASSES; ++pass, cur ^= 1) {
+    vc_hist_kernel<<<nb, CF_THREADS, 0, st>>>(V.lo[cur], V.hi[cur], V.n_kept, pass, V.hist, V.hist_count);
+    CTR_LAUNCHED("ctr_criteo_vocab(hist)");
+    cf_scan_kernel<int32_t><<<1, 1024, 0, st>>>(V.hist, V.hist_count, nullptr);
+    CTR_LAUNCHED("ctr_criteo_vocab(scan)");
+    vc_scatter_kernel<<<nb, CF_THREADS, 0, st>>>(V.lo[cur], V.hi[cur], V.sl[cur], V.n_kept, pass, V.hist,
+                                                 V.lo[cur ^ 1], V.hi[cur ^ 1], V.sl[cur ^ 1]);
+    CTR_LAUNCHED("ctr_criteo_vocab(scatter)");
+  }
+  vc_assign_kernel<<<cf_grid(capacity), CF_THREADS, 0, st>>>(T, V.lo[cur], V.hi[cur], V.sl[cur], V.n_kept, field_counts,
+                                                            vocab_keys);
+  CTR_LAUNCHED("ctr_criteo_vocab(assign)");
+  return CTR_OK;
+}
+
+size_t ctr_criteo_emit_workspace_bytes(size_t len) { return CfEmitWs(nullptr, len).bytes; }
+
+static int cf_emit_args(const void* table, int64_t capacity, const double* num_min, const double* num_den,
+                        const int64_t* offsets, const char* label, int label_len, int test, CfEmitArgs& a) {
+  CTR_REQUIRE(table && capacity > 0 && capacity <= CF_MAX_CAP && num_min && num_den && offsets && label_len >= 0 &&
+                  (label_len == 0 || label),
+              CTR_ERR_INVALID_ARG, "ctr_criteo_emit: bad arguments");
+  a = CfEmitArgs{CfTable(const_cast<void*>(table), capacity), num_min, num_den, offsets, label, label_len, test ? 1 : 0};
+  return CTR_OK;
+}
+
+int ctr_criteo_emit_plan(const char* text, size_t len, int test, int64_t line_base, const uint8_t* to_train,
+                         const void* table, int64_t capacity, const double* num_min, const double* num_den,
+                         const int64_t* offsets, const char* label, int label_len, int64_t* info, void* ws,
+                         size_t ws_bytes, ctr_stream_t stream) {
+  CTR_REQUIRE(info && line_base >= 0 && (len == 0 || text) && (test || to_train), CTR_ERR_INVALID_ARG,
+              "ctr_criteo_emit_plan: bad arguments");
+  CTR_REQUIRE(len < CF_MAX_LEN, CTR_ERR_INVALID_ARG, "ctr_criteo_emit_plan: chunk too large (len < 2^30)");
+  CTR_REQUIRE(ws && ws_bytes >= ctr_criteo_emit_workspace_bytes(len), CTR_ERR_WORKSPACE,
+              "ctr_criteo_emit_plan: workspace too small");
+  CfEmitArgs a;
+  if (int rc = cf_emit_args(table, capacity, num_min, num_den, offsets, label, label_len, test, a)) return rc;
+  cudaStream_t st = as_stream(stream);
+  CTR_REQUIRE(cudaMemsetAsync(info, 0, 5 * sizeof(int64_t), st) == cudaSuccess &&
+                  cudaMemsetAsync(info + 1, 0xFF, sizeof(int64_t), st) == cudaSuccess,
+              CTR_ERR_CUDA, "ctr_criteo_emit_plan: memset failed");
+  if (len == 0) return CTR_OK;
+  const unsigned char* t = reinterpret_cast<const unsigned char*>(text);
+  CfEmitWs E(ws, len);
+  if (int rc = cf_line_starts(t, len, E.lines, st, "ctr_criteo_emit_plan(lines)")) return rc;
+  cf_plan_kernel<<<cf_grid((int64_t)len + 1), CF_THREADS, 0, st>>>(t, (int64_t)len, E.lines.line_start,
+                                                                   E.lines.n_newlines, line_base, to_train, a, E.line_len,
+                                                                   E.tile_tr, E.tile_va, E.tile_trn, E.n_tiles, info);
+  CTR_LAUNCHED("ctr_criteo_emit_plan");
+  cf_scan_kernel<int64_t><<<1, 1024, 0, st>>>(E.tile_tr, E.n_tiles, info + 3);
+  CTR_LAUNCHED("ctr_criteo_emit_plan(scan)");
+  cf_scan_kernel<int64_t><<<1, 1024, 0, st>>>(E.tile_va, E.n_tiles, info + 4);
+  CTR_LAUNCHED("ctr_criteo_emit_plan(scan)");
+  cf_scan_kernel<int64_t><<<1, 1024, 0, st>>>(E.tile_trn, E.n_tiles, info + 2);
+  CTR_LAUNCHED("ctr_criteo_emit_plan(scan)");
+  return CTR_OK;
+}
+
+int ctr_criteo_emit_write(const char* text, size_t len, int test, const uint8_t* to_train, const void* table,
+                          int64_t capacity, const double* num_min, const double* num_den, const int64_t* offsets,
+                          const char* label, int label_len, char* out_tr, char* out_va, const void* ws,
+                          size_t ws_bytes, ctr_stream_t stream) {
+  CTR_REQUIRE((len == 0 || text) && (test || to_train), CTR_ERR_INVALID_ARG, "ctr_criteo_emit_write: bad arguments");
+  CTR_REQUIRE(len < CF_MAX_LEN, CTR_ERR_INVALID_ARG, "ctr_criteo_emit_write: chunk too large (len < 2^30)");
+  CTR_REQUIRE(ws && ws_bytes >= ctr_criteo_emit_workspace_bytes(len), CTR_ERR_WORKSPACE,
+              "ctr_criteo_emit_write: workspace too small");
+  CfEmitArgs a;
+  if (int rc = cf_emit_args(table, capacity, num_min, num_den, offsets, label, label_len, test, a)) return rc;
+  if (len == 0) return CTR_OK;
+  CfEmitWs E(const_cast<void*>(ws), len);
+  cf_write_kernel<<<cf_grid((int64_t)len + 1), CF_THREADS, 0, as_stream(stream)>>>(
+      reinterpret_cast<const unsigned char*>(text), (int64_t)len, E.lines.line_start, E.lines.n_newlines, to_train, a,
+      E.line_len, E.tile_tr, E.tile_va, out_tr, out_va);
+  CTR_LAUNCHED("ctr_criteo_emit_write");
+  return CTR_OK;
+}
+
+}  // extern "C"
