@@ -6,13 +6,8 @@ Sub-classes implement
     _forward(ids, vals, train, masks) -> (bias, y_a, y_b, y_c)   logit terms, summed left to right
     _backward(ids, vals)                                          from self.dy: fill self.g_rows
                                                                   (+ self.g_w) and the dense gradients
-update_mode
-  "exact": TensorFlow semantics -- every table row moves every step (dense L2 gradient + non-lazy
-           sparse Adam, SURVEY.md A.4): full-table sweep each step (HBM-bound).
-  "exact_deferred": bit-identical state to "exact"; rows nothing gathered are replayed lazily
-           (csrc/epoch.cu): one pass over HBM per `epoch_steps` steps.  The l2*l2_loss terms of `loss`
-           become available at the end of each epoch (`epoch_reg_terms`).
-  "lazy" : only gathered rows are updated (what LazyAdam would do); NOT the reference's result.
+The update modes (exact / exact_deferred / lazy) and their step schedule: engine.SparseUpdater.  In
+exact_deferred mode the l2*l2_loss terms of `loss` become available at the end of each epoch (`epoch_reg_terms`).
 Data parallel (world > 1): tables are replicated; every rank all-gathers the per-occurrence sparse
 gradients and applies the identical de-duplicated update; dense gradients + loss ride in one
 all-reduce.  Synchronous DP replaces the reference's asynchronous parameter server
@@ -25,7 +20,7 @@ from typing import Dict, List, Optional
 import torch
 
 from . import ops
-from .engine import DenseVars, OptimizerState, SparseUpdater, Table
+from .engine import DenseVars, OptimizerState, SparseModel, SparseUpdater, Table
 
 
 def ints(s) -> List[int]:
@@ -36,7 +31,7 @@ def floats(s) -> List[float]:
     return [float(t) for t in s.split(",")] if isinstance(s, str) else list(s)
 
 
-class CTRModel:
+class CTRModel(SparseModel):
     replayed_launches = 0               # kernels launched through CUDA-graph replays (train_step_graphed)
     batch_norm, bn_decay = False, 0.9   # --batch_norm / --batch_norm_decay (set by the sub-class before _build)
     table_name = "emb"          # TF variable name of the [N,K] table
@@ -45,9 +40,8 @@ class CTRModel:
     def __init__(self, field_size: int, feature_size: int, embedding_size: int, batch_size: int,
                  l2_reg: float, learning_rate: float, optimizer: str, update_mode: str = "exact",
                  device="cuda", seed: int = 0, world: int = 1, epoch_steps: int = 8):
-        assert update_mode in ("exact", "exact_deferred", "lazy")
         self.F, self.N, self.K, self.B = field_size, feature_size, embedding_size, batch_size
-        self.l2_reg, self.update_mode = float(l2_reg), update_mode
+        self.l2_reg = float(l2_reg)
         self.device = torch.device(device)
         self.world, self.seed = world, seed
         dev = self.device
@@ -64,22 +58,16 @@ class CTRModel:
         self.g_w = torch.empty(B * F, **f32) if self.W is not None else None
         self.oob = torch.zeros(2, dtype=torch.int32, device=dev)
         G = world
-        self.updater = SparseUpdater(G * B * F, self.N, K, self.opt, dev, with_scalar_table=self.W is not None)
+        self.updater = SparseUpdater(G * B * F, self.N, K, self.opt, dev, self.W is not None, self.tables, update_mode,
+                                     epoch_steps, l2_reg)
         if G > 1:
             self.ids_all = torch.empty(G * B * F, dtype=torch.int32, device=dev)
             self.g_rows_all = torch.empty(G * B * F, K, **f32)
             self.g_w_all = torch.empty(G * B * F, **f32) if self.W is not None else None
         self.global_step = 0
-        self.epoch_steps, self.epoch_pos = epoch_steps, 0
         self.dense: DenseVars = None  # set by the sub-class (_build)
         self._build()
         self.loss_ce = self.dense.tail[0:1]
-        if update_mode == "exact_deferred":
-            # Adagrad/Momentum/Ftrl with l2_reg == 0 are truly sparse in TF: nothing to defer
-            if self.l2_reg == 0.0 and optimizer != "Adam":
-                self.update_mode = "exact"
-            else:
-                self.updater.enable_epochs(epoch_steps, self.tables)
 
     # ---- to be provided --------------------------------------------------------------------------------
     def _build(self):
@@ -94,22 +82,6 @@ class CTRModel:
     def _dense_reg_terms(self) -> Optional[torch.Tensor]:
         """l2*l2_loss of regularised DENSE variables (DCN's cross_w/cross_b), device tensor or None."""
         return None
-
-    # ---- deferred-mode plumbing ----------------------------------------------------------------------------
-    def flush(self):
-        """exact_deferred: bring every row to the current step (no-op otherwise)."""
-        if self.update_mode == "exact_deferred" and self.epoch_pos > self.updater.flush_pos:
-            self.updater.epoch_sweep(self.tables, self.epoch_pos, reset=False, l2_reg=self.l2_reg)
-
-    def set_update_mode(self, mode: str):
-        """Switch between exact / exact_deferred / lazy on a live model (state stays consistent)."""
-        assert mode in ("exact", "exact_deferred", "lazy")
-        if self.update_mode == "exact_deferred" and self.epoch_pos > 0:
-            self.updater.epoch_sweep(self.tables, self.epoch_pos, reset=True, l2_reg=self.l2_reg)
-            self.epoch_pos = 0
-        if mode == "exact_deferred" and not hasattr(self.updater, "ep"):
-            self.updater.enable_epochs(self.epoch_steps, self.tables)
-        self.update_mode = mode
 
     def epoch_reg_terms(self) -> torch.Tensor:
         """exact_deferred: [n_tables, epoch_steps] l2*l2_loss(table) for every step of the epoch that just
@@ -127,20 +99,6 @@ class CTRModel:
         if mlp is not None:
             out.update(mlp.bn_state)      # non-trainable moving_mean / moving_variance (batch_norm=True)
         return out
-
-    def load_variables(self, values: Dict[str, torch.Tensor]):
-        vs = self.variables()
-        for name, v in values.items():
-            vs[name].copy_(v.to(self.device, torch.float32).reshape(vs[name].shape))
-
-    def check_ids(self):
-        """TF raises InvalidArgumentError for ids outside [0, feature_size); we count them on device."""
-        self.updater.check_list_overflow()
-        cnt, first = self.oob.tolist()
-        if cnt:
-            self.oob.zero_()
-            raise IndexError(f"{cnt} feature ids outside [0, {self.N}) (first: {first}); "
-                             "TensorFlow would raise InvalidArgumentError")
 
     # ---- modes --------------------------------------------------------------------------------------------------
     def predict(self, ids: torch.Tensor, vals: torch.Tensor) -> torch.Tensor:
@@ -160,21 +118,14 @@ class CTRModel:
         assert B == self.B or self.world == 1, "partial batches are not supported under data parallelism"
         deferred = self.update_mode == "exact_deferred"
         upd = self.updater
-        if deferred:
-            j = self.epoch_pos
-            if j == 0:
-                upd.epoch_begin()
-            self.opt.tick_epoch(j)
-            ids_u = ids.reshape(-1)
-            if self.world > 1:
-                import torch.distributed as dist
-                dist.all_gather_into_tensor(self.ids_all, ids_u)
-                ids_u = self.ids_all
-            # gathered rows (of every rank) must hold the state at the start of this step
-            upd.unique(ids_u)
-            upd.epoch_rows([(t, None) for t in self.tables], j, apply=False)
-        else:
-            self.opt.tick()
+        upd.begin_step()
+        ids_u = ids.reshape(-1)
+        if deferred and self.world > 1:
+            import torch.distributed as dist
+            dist.all_gather_into_tensor(self.ids_all, ids_u)
+            ids_u = self.ids_all
+        # gathered rows (of every rank) must hold the state at the start of this step
+        upd.catch_up(ids_u)
         bias, y_a, y_b, y_c = self._forward(ids, vals, train=True, masks=masks)
         ops.logit_loss(bias, y_a, y_b, y_c, labels, B, y=self.y[:B], pred=self.pred[:B], loss_ce=self.loss_ce,
                        dy=self.dy[:B], dbias=(self.dense.grads[self.bias_name] if self.bias_name else None),
@@ -191,17 +142,7 @@ class CTRModel:
                 dist.all_gather_into_tensor(self.g_w_all, g_w)
             dist.all_reduce(self.dense.grad)  # dense gradients + the loss tail, summed over ranks
             g_rows, g_w = self.g_rows_all, (self.g_w_all if g_w is not None else None)
-        if deferred:
-            upd.segment_sum(g_rows, g_w)
-            tg = [(self.V, upd.g_uniq)] + ([(self.W, upd.gw_uniq)] if self.W is not None else [])
-            upd.epoch_rows(tg, self.epoch_pos, apply=True)
-            self.epoch_pos += 1
-            if self.epoch_pos == self.epoch_steps:
-                upd.epoch_sweep(self.tables, self.epoch_steps, reset=True, l2_reg=self.l2_reg)
-                self.epoch_pos = 0
-        else:
-            upd.dedup(self.ids_all if self.world > 1 else ids.reshape(-1), g_rows, g_w)
-            upd.apply(self.V, self.W, exact=(self.update_mode == "exact"), l2_reg=self.l2_reg)
+        upd.finish_step(self.ids_all if self.world > 1 else ids.reshape(-1), g_rows, g_w)
         dense_reg = self._dense_reg_terms()
         self.dense.apply()
         self.global_step += 1
@@ -251,7 +192,7 @@ class CTRModel:
             with torch.cuda.graph(g):
                 out = self.train_step(*self._gin)
             # capture ran the host code (bookkeeping advanced) but launched nothing: rewind, then replay below
-            self.epoch_pos, self.global_step = pos, step
+            self.updater.epoch_pos, self.global_step = pos, step
             self._graphs[key], self._graph_out[key] = g, out
             self._graph_launches = getattr(self, "_graph_launches", {})
             self._graph_launches[key] = _lib.launch_count() - n0     # kernels of libctr_b200.so inside this graph
@@ -260,7 +201,7 @@ class CTRModel:
         self.replayed_launches += self._graph_launches[key]
         self.global_step += 1
         if deferred:
-            self.epoch_pos += 1
+            self.updater.epoch_pos += 1
         return self._graph_out[key]
 
     def predict_graphed(self, ids: torch.Tensor, vals: torch.Tensor) -> torch.Tensor:

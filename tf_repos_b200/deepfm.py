@@ -3,7 +3,8 @@
 Same parameters (`field_size, feature_size, embedding_size, l2_reg, learning_rate, deep_layers,
 dropout`, DeepFM.py:329-338), same variable names (`fm_bias, fm_w, fm_v, Deep-part/mlp{i}/...`),
 same modes (TRAIN / EVAL / PREDICT).  Everything numerical runs in hand-written sm_90a kernels
-through the C ABI; see tf_repos_b200/base.py for the update modes and data parallelism.
+through the C ABI; see tf_repos_b200/engine.py (SparseUpdater) for the update modes and
+tf_repos_b200/base.py for data parallelism.
 """
 from __future__ import annotations
 

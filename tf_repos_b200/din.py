@@ -23,20 +23,19 @@ import torch
 
 from . import ops
 from .base import floats, ints
-from .engine import DenseVars, OptimizerState, SparseUpdater, Table
+from .engine import DenseVars, OptimizerState, SparseModel, SparseUpdater, Table
 from .mlp import MLP
 
 FIELDS = ("cat", "shop", "brand", "int")
 ATT = "Field-wise-Pooling-layer"
 
 
-class DIN:
+class DIN(SparseModel):
     def __init__(self, field_size: int, feature_size: int, embedding_size: int, batch_size: int, max_len: int,
                  max_a_int: int = 8, deep_layers="256,128,64", dropout="0.5,0.5,0.5", attention_layers="256",
                  attention_pooling: bool = True, l2_reg: float = 1e-4, learning_rate: float = 5e-4,
                  optimizer: str = "Adam", update_mode: str = "exact", device="cuda", seed: int = 0,
                  epoch_steps: int = 8, batch_norm: bool = False, batch_norm_decay: float = 0.9):
-        assert update_mode in ("exact", "exact_deferred", "lazy")
         if batch_norm and attention_pooling:
             # DIN.py:166 calls batch_norm_layer(train_phase=train_phase) inside attention_unit, where train_phase is
             # not defined (it is assigned later, DIN.py:189-193): the reference raises NameError (quirk Q5)
@@ -47,7 +46,7 @@ class DIN:
         self.layers, self.keep = ints(deep_layers), floats(dropout)
         self.H = self.layers[0]                     # quirk Q5: width = deep_layers[0]
         self.attention_pooling = attention_pooling
-        self.l2_reg, self.update_mode = float(l2_reg), update_mode
+        self.l2_reg = float(l2_reg)
         self.device = dev = torch.device(device)
         self.seed = seed
         B, Fp, K, P, H = self.B, self.Fp, self.K, self.P, self.H
@@ -90,7 +89,7 @@ class DIN:
         self.n_total = o
         self.ids_all = torch.zeros(o, dtype=torch.int32, device=dev)
         self.g_all = torch.zeros(o, K, **f32)
-        self.updater = SparseUpdater(o, self.N, K, self.opt, dev, with_scalar_table=False)
+        self.updater = SparseUpdater(o, self.N, K, self.opt, dev, False, self.tables, update_mode, epoch_steps, l2_reg)
         if attention_pooling:
             self.E = [torch.empty(B * P, K, **f32) for _ in range(4)]
             self.Hh = [torch.empty(B * P, H, **f32) for _ in range(4)]
@@ -119,36 +118,14 @@ class DIN:
                                           ops.fc1_bwd_workspace_bytes(B * P, H, 0), 16), dtype=torch.uint8, device=dev)
         self.d_aint = torch.empty(B, K, **f32)
         self.global_step = 0
-        self.epoch_steps, self.epoch_pos = epoch_steps, 0
-        if update_mode == "exact_deferred":
-            if self.l2_reg == 0.0 and optimizer != "Adam":
-                self.update_mode = "exact"
-            else:
-                self.updater.enable_epochs(epoch_steps, self.tables)
 
     # ---- plumbing -------------------------------------------------------------------------------------
-    def flush(self):
-        if self.update_mode == "exact_deferred" and self.epoch_pos > self.updater.flush_pos:
-            self.updater.epoch_sweep(self.tables, self.epoch_pos, reset=False, l2_reg=self.l2_reg)
-
     def variables(self) -> Dict[str, torch.Tensor]:
         self.flush()
         out = {"embeddings": self.V.var}
         out.update(self.dense.views)
         out.update(self.mlp.bn_state)
         return out
-
-    def load_variables(self, values: Dict[str, torch.Tensor]):
-        vs = self.variables()
-        for name, v in values.items():
-            vs[name].copy_(v.to(self.device, torch.float32).reshape(vs[name].shape))
-
-    def check_ids(self):
-        self.updater.check_list_overflow()
-        cnt, first = self.oob.tolist()
-        if cnt:
-            self.oob.zero_()
-            raise IndexError(f"{cnt} feature ids outside [0, {self.N}) (first: {first})")
 
     def _stage_ids(self, batch):
         """ids of every embedding_lookup of the step, in gradient-segment order."""
@@ -276,17 +253,9 @@ class DIN:
         takes g = 0 + l2*var, which is the untouched-row update it would have taken anyway).  Not with --batch_norm
         (the padded rows would enter the batch moments)."""
         upd = self.updater
-        deferred = self.update_mode == "exact_deferred"
         self._stage_ids(batch)
-        if deferred:
-            j = self.epoch_pos
-            if j == 0:
-                upd.epoch_begin()
-            self.opt.tick_epoch(j)
-            upd.unique(self.ids_all)
-            upd.epoch_rows([(self.V, None)], j, apply=False)
-        else:
-            self.opt.tick()
+        upd.begin_step()
+        upd.catch_up(self.ids_all)
         y_d = self._forward(batch, train=True, masks=masks)
         n = self.B if n_valid is None else int(n_valid)
         assert 0 < n <= self.B
@@ -297,16 +266,7 @@ class DIN:
         ops.logit_loss(None, y_d[:n], None, None, labels[:n], n, y=self.y[:n], pred=self.pred[:n], loss_ce=self.loss_ce,
                        dy=self.dy[:n])
         self._backward(batch)
-        if deferred:
-            upd.segment_sum(self.g_all, None)
-            upd.epoch_rows([(self.V, upd.g_uniq)], self.epoch_pos, apply=True)
-            self.epoch_pos += 1
-            if self.epoch_pos == self.epoch_steps:
-                upd.epoch_sweep(self.tables, self.epoch_steps, reset=True, l2_reg=self.l2_reg)
-                self.epoch_pos = 0
-        else:
-            upd.dedup(self.ids_all, self.g_all, None)
-            upd.apply(self.V, None, exact=(self.update_mode == "exact"), l2_reg=self.l2_reg)
+        upd.finish_step(self.ids_all, self.g_all)
         self.dense.apply()
         self.global_step += 1
         return torch.cat([self.loss_ce, upd.reg[0:1]])

@@ -95,15 +95,39 @@ class Table:
         return self.slots[i] if i < len(self.slots) else None
 
 
-class SparseUpdater:
-    """K3 + K4 for a group of tables that are all gathered with the SAME ids (DeepFM: fm_v and fm_w).
+UPDATE_MODES = ("exact", "exact_deferred", "lazy")
 
-    exact mode (TensorFlow semantics, SURVEY.md A.4): gathered rows are computed first into a stage
-    buffer from the pre-step state, the dense sweep then advances every row with g = l2*var, and
-    the staged rows are patched back.  lazy mode updates the gathered rows only.
+
+def _check_mode(mode: str):
+    if mode not in UPDATE_MODES:
+        raise ValueError(f"update_mode {mode!r} is not one of {', '.join(UPDATE_MODES)}")
+
+
+class SparseUpdater:
+    """K3 + K4 for a group of tables that are all gathered with the SAME ids (DeepFM: fm_v and fm_w; the first
+    table is [N,K], an optional second one the [N] first-order weights), and the step schedule of its update mode.
+
+    update_mode
+      "exact": TensorFlow semantics (SURVEY.md A.4) -- every table row moves every step (dense L2 gradient +
+               non-lazy sparse Adam): gathered rows are computed first into a stage buffer from the pre-step
+               state, the dense sweep then advances every row with g = l2*var, and the staged rows are patched
+               back (HBM-bound).
+      "exact_deferred": bit-identical state to "exact"; rows nothing gathered are replayed lazily
+               (csrc/epoch.cu): one pass over HBM per `epoch_steps` steps.  The l2*l2_loss terms of `loss`
+               become available at the end of each epoch.  Adagrad/Momentum/Ftrl with l2_reg == 0 are truly
+               sparse in TF: there is nothing to defer, and the mode becomes "exact".
+      "lazy" : only gathered rows are updated (what LazyAdam would do); NOT the reference's result.
+
+    A model's train step calls begin_step(), catch_up(ids) before the forward reads any row, and
+    finish_step(ids, g_rows, g_w) with the per-occurrence gradient rows; predict() and variable reads call flush().
+    `tables` are the tables it steps ([N,K] first, then the [N] table when with_scalar_table); without them only the
+    buffers are built.
     """
 
-    def __init__(self, n_ids: int, N: int, K: int, opt: OptimizerState, device, with_scalar_table: bool):
+    def __init__(self, n_ids: int, N: int, K: int, opt: OptimizerState, device, with_scalar_table: bool,
+                 tables: Sequence[Table] = (), update_mode: str = "exact", epoch_steps: int = 8, l2_reg: float = 0.0):
+        _check_mode(update_mode)
+        self.tables = list(tables)
         self.n, self.N, self.K, self.opt = n_ids, N, K, opt
         self.uw = ops.UniqueWorkspace(n_ids, N, device)
         f32 = dict(dtype=torch.float32, device=device)
@@ -119,10 +143,64 @@ class SparseUpdater:
         self.reg = torch.zeros(2, **f32)
         self.sweep_events = None  # set to [] to collect (start, end) CUDA events around the V sweep
         self.sweep_steps = []     # parallel to sweep_events: steps replayed by each pass (deferred mode)
+        self.l2_reg = float(l2_reg)
+        self.epoch_steps, self.epoch_pos = epoch_steps, 0
+        self.update_mode = update_mode
+        if update_mode == "exact_deferred":
+            if self.l2_reg == 0.0 and opt.name != "Adam":
+                self.update_mode = "exact"
+            else:
+                self.enable_epochs(epoch_steps, self.tables)
 
-    def dedup(self, ids_flat: torch.Tensor, g_rows: torch.Tensor, g_w: Optional[torch.Tensor]):
-        ops.unique_segment(ids_flat, self.uw)
-        ops.segment_sum_rows(g_rows, g_w, self.uw, self.K, self.g_uniq, self.gw_uniq if g_w is not None else None)
+    # ---- the step schedule -----------------------------------------------------------------------------------
+    def begin_step(self):
+        """Start of a train step: the optimizer tick (exact_deferred: also records lr_t at the epoch position)."""
+        if self.update_mode != "exact_deferred":
+            self.opt.tick()
+            return
+        if self.epoch_pos == 0:
+            for e in self.ep.values():
+                ops.fill(e["reg"], 0.0)
+        self.opt.tick_epoch(self.epoch_pos)
+
+    def catch_up(self, ids_flat: torch.Tensor):
+        """exact_deferred: the rows `ids_flat` gathers are brought to the start of this step (no-op otherwise)."""
+        if self.update_mode == "exact_deferred":
+            ops.unique_segment(ids_flat, self.uw)
+            self.epoch_rows([(t, None) for t in self.tables], self.epoch_pos, apply=False)
+
+    def finish_step(self, ids_flat: torch.Tensor, g_rows: torch.Tensor, g_w: Optional[torch.Tensor] = None):
+        """The table update of this step from the per-occurrence gradient rows of `ids_flat` (g_w: those of the
+        scalar table).  exact_deferred reuses the de-duplication catch_up() made of the same ids, and closes the
+        epoch with the sweep of every row after its last step."""
+        gw_uniq = self.gw_uniq if g_w is not None else None
+        if self.update_mode == "exact_deferred":
+            ops.segment_sum_rows(g_rows, g_w, self.uw, self.K, self.g_uniq, gw_uniq)
+            self.epoch_rows(list(zip(self.tables, (self.g_uniq, self.gw_uniq))), self.epoch_pos, apply=True)
+            self.epoch_pos += 1
+            if self.epoch_pos == self.epoch_steps:
+                self.epoch_sweep(self.epoch_steps, reset=True)
+                self.epoch_pos = 0
+        else:
+            ops.unique_segment(ids_flat, self.uw)
+            ops.segment_sum_rows(g_rows, g_w, self.uw, self.K, self.g_uniq, gw_uniq)
+            self.apply(exact=(self.update_mode == "exact"))
+
+    def flush(self):
+        """exact_deferred: bring every row to the current step (no-op otherwise)."""
+        if self.update_mode == "exact_deferred" and self.epoch_pos > self.flush_pos:
+            self.epoch_sweep(self.epoch_pos, reset=False)
+
+    def set_mode(self, mode: str):
+        """Switch between exact / exact_deferred / lazy on a live model (state stays consistent).  Unlike the
+        constructor, this keeps exact_deferred for every optimizer."""
+        _check_mode(mode)
+        if self.update_mode == "exact_deferred" and self.epoch_pos > 0:
+            self.epoch_sweep(self.epoch_pos, reset=True)
+            self.epoch_pos = 0
+        if mode == "exact_deferred" and not hasattr(self, "ep"):
+            self.enable_epochs(self.epoch_steps, self.tables)
+        self.update_mode = mode
 
     # ---- exact-deferred ("epoch") mode: csrc/epoch.cu ------------------------------------------------
     def enable_epochs(self, P: int, tables: Sequence[Table]):
@@ -149,12 +227,6 @@ class SparseUpdater:
                 partials=torch.zeros(pmax * self.n_epart, dtype=torch.float64, device=dev),
                 reg=torch.zeros(pmax, dtype=torch.float32, device=dev))
 
-    def unique(self, ids_flat: torch.Tensor):
-        ops.unique_segment(ids_flat, self.uw)
-
-    def segment_sum(self, g_rows, g_w):
-        ops.segment_sum_rows(g_rows, g_w, self.uw, self.K, self.g_uniq, self.gw_uniq if g_w is not None else None)
-
     def epoch_rows(self, tables_g, j: int, apply: bool):
         """tables_g: [(Table, g_uniq or None)].  apply=False: catch the gathered rows up to the start of
         step j; apply=True: take step j with the de-duplicated gradient."""
@@ -171,10 +243,10 @@ class SparseUpdater:
             ops.epoch_rows(o.opt, apply, t.var, t.slot(0), t.slot(1), e["last"], uw.uniq, uw.n_uniq,
                            g if apply else None, self.n, t.K, o.record(HYPER_TABLE), o.lr_table, j, e["ss"])
 
-    def epoch_sweep(self, tables: Sequence[Table], upto: int, reset: bool, l2_reg: float):
+    def epoch_sweep(self, upto: int, reset: bool):
         """All rows -> state after `upto` steps of this epoch; per-step l2*l2_loss terms -> ep[.]['reg']."""
         o = self.opt
-        for t in tables:
+        for t in self.tables:
             e = self.ep[t.name]
             ev = None
             if self.sweep_events is not None and t.K > 1:
@@ -188,7 +260,7 @@ class SparseUpdater:
                 self.sweep_events.append(ev)
                 self.sweep_steps.append(upto - self.flush_pos)   # optimizer steps this pass replayed per element
             # accumulate: a mid-epoch flush and the epoch-end sweep each contribute their share
-            ops.epoch_reg_loss(e["ss"], e["partials"], self.n_epart, upto, 0.5 * l2_reg, e["reg"], accumulate=True)
+            ops.epoch_reg_loss(e["ss"], e["partials"], self.n_epart, upto, 0.5 * self.l2_reg, e["reg"], accumulate=True)
         self.flush_pos = 0 if reset else upto
 
     def check_list_overflow(self):
@@ -200,19 +272,15 @@ class SparseUpdater:
             raise RuntimeError(f"exact-deferred epoch sweep: {n} gathered rows did not fit in the row list and were "
                                "not caught up; the table state is invalid")
 
-    def epoch_begin(self):
-        for e in self.ep.values():
-            ops.fill(e["reg"], 0.0)
-
-    def apply(self, V: Table, W: Optional[Table], exact: bool, l2_reg: float):
+    def apply(self, exact: bool):
         o, uw, hyper = self.opt, self.uw, self.opt.record(HYPER_TABLE)
-        n = self.n
+        n, l2_reg = self.n, self.l2_reg
         # TF's sparse Adagrad/Momentum/Ftrl touch only gathered rows unless the dense L2 gradient
         # makes every row an index; sparse Adam decays every row regardless.
         sweep = exact and (l2_reg != 0.0 or o.name == "Adam")
-        tabs = [(V, self.g_uniq, self.stage_v, self.partials_v, 0)]
-        if W is not None:
-            tabs.append((W, self.gw_uniq, self.stage_w, self.partials_w, 1))
+        tabs = [(self.tables[0], self.g_uniq, self.stage_v, self.partials_v, 0)]
+        if len(self.tables) > 1:
+            tabs.append((self.tables[1], self.gw_uniq, self.stage_w, self.partials_w, 1))
         for t, g, stage, partials, ri in tabs:
             ops.opt_sparse_rows(o.opt, t.var, t.slot(0), t.slot(1), uw.uniq, uw.n_uniq, g, n, t.K, hyper,
                                 stage if sweep else None)
@@ -227,6 +295,38 @@ class SparseUpdater:
                     self.sweep_events.append(ev)
                 ops.opt_patch_rows(t.var, t.slot(0), t.slot(1), uw.uniq, uw.n_uniq, stage, n, t.K, o.n_slots)
                 ops.reduce_sum(partials, 0.5 * l2_reg, self.reg[ri:ri + 1], self.red_ws)
+
+
+class SparseModel:
+    """What every model trained through a SparseUpdater shares.  The model sets `updater`, `N` (the global
+    vocabulary), `oob` (the device [count, first] of the out-of-range ids its lookups met) and `device`, and
+    provides variables() (TF name -> tensor) where it has one."""
+
+    update_mode = property(lambda self: self.updater.update_mode)
+    epoch_pos = property(lambda self: self.updater.epoch_pos)
+    epoch_steps = property(lambda self: self.updater.epoch_steps)
+
+    def flush(self):
+        """exact_deferred: bring every row to the current step (no-op otherwise)."""
+        self.updater.flush()
+
+    def set_update_mode(self, mode: str):
+        """Switch between exact / exact_deferred / lazy on a live model (state stays consistent)."""
+        self.updater.set_mode(mode)
+
+    def check_ids(self):
+        """TF raises InvalidArgumentError for ids outside [0, feature_size); we count them on device."""
+        self.updater.check_list_overflow()
+        cnt, first = self.oob.tolist()
+        if cnt:
+            self.oob.zero_()
+            raise IndexError(f"{cnt} feature ids outside [0, {self.N}) (first: {first}); "
+                             "TensorFlow would raise InvalidArgumentError")
+
+    def load_variables(self, values: Dict[str, torch.Tensor]):
+        vs = self.variables()
+        for name, v in values.items():
+            vs[name].copy_(v.to(self.device, torch.float32).reshape(vs[name].shape))
 
 
 class DenseVars:

@@ -23,26 +23,25 @@ import torch
 
 from . import ops
 from .base import floats, ints
-from .engine import DenseVars, OptimizerState, SparseUpdater, Table
+from .engine import DenseVars, OptimizerState, SparseModel, SparseUpdater, Table
 from .mlp import MLP
 
 BAGS = ("u_cat", "u_shop", "u_brand", "u_int", "a_int")
 TOWERS = ("cvr", "ctr")          # creation order of DeepCvrMTL.py:166-203
 
 
-class ESMM:
+class ESMM(SparseModel):
     def __init__(self, field_size: int, feature_size: int, embedding_size: int, batch_size: int, occ_capacity: int,
                  deep_layers="256,128,64", dropout="0.5,0.5,0.5", ctr_task_wgt: float = 0.5, l2_reg: float = 1e-4,
                  learning_rate: float = 5e-4, optimizer: str = "Adam", update_mode: str = "exact", device="cuda",
                  seed: int = 0, epoch_steps: int = 8, batch_norm: bool = False, batch_norm_decay: float = 0.9):
-        assert update_mode in ("exact", "exact_deferred", "lazy")
         self.Fp, self.N, self.K, self.B = field_size, feature_size, embedding_size, batch_size
         self.cap = int(occ_capacity)
         self.layers, self.keep = ints(deep_layers), floats(dropout)
         self.ctr_task_wgt = float(ctr_task_wgt)
         # TF turns the Python constants w and 1 - w into fp32 constants separately (:223)
         self.w_ctr, self.w_cvr = self.ctr_task_wgt, 1.0 - self.ctr_task_wgt
-        self.l2_reg, self.update_mode = float(l2_reg), update_mode
+        self.l2_reg = float(l2_reg)
         self.device = dev = torch.device(device)
         self.seed = seed
         B, Fp, K = self.B, self.Fp, self.K
@@ -72,21 +71,12 @@ class ESMM:
         self.n_total = self.n_fixed + self.cap
         self.ids_all = torch.zeros(self.n_total, dtype=torch.int32, device=dev)
         self.g_all = torch.zeros(self.n_total, K, **f32)
-        self.updater = SparseUpdater(self.n_total, self.N, K, self.opt, dev, with_scalar_table=False)
+        self.updater = SparseUpdater(self.n_total, self.N, K, self.opt, dev, False, self.tables, update_mode,
+                                     epoch_steps, l2_reg)
         self._a = {}
         self.global_step = 0
-        self.epoch_steps, self.epoch_pos = epoch_steps, 0
-        if update_mode == "exact_deferred":
-            if self.l2_reg == 0.0 and optimizer != "Adam":
-                self.update_mode = "exact"
-            else:
-                self.updater.enable_epochs(epoch_steps, self.tables)
 
     # ---- plumbing -------------------------------------------------------------------------------------
-    def flush(self):
-        if self.update_mode == "exact_deferred" and self.epoch_pos > self.updater.flush_pos:
-            self.updater.epoch_sweep(self.tables, self.epoch_pos, reset=False, l2_reg=self.l2_reg)
-
     def variables(self) -> Dict[str, torch.Tensor]:
         self.flush()
         out = {"embeddings": self.V.var}
@@ -94,18 +84,6 @@ class ESMM:
         for t in TOWERS:
             out.update(self.towers[t].bn_state)
         return out
-
-    def load_variables(self, values: Dict[str, torch.Tensor]):
-        vs = self.variables()
-        for name, v in values.items():
-            vs[name].copy_(v.to(self.device, torch.float32).reshape(vs[name].shape))
-
-    def check_ids(self):
-        self.updater.check_list_overflow()
-        cnt, first = self.oob.tolist()
-        if cnt:
-            self.oob.zero_()
-            raise IndexError(f"{cnt} feature ids outside [0, {self.N}) (first: {first})")
 
     def _stage_ids(self, batch):
         """ids of every lookup of the step in gradient-row order; unused occurrence slots repeat the batch's first
@@ -158,17 +136,9 @@ class ESMM:
         so the step equals TensorFlow's step on the smaller batch (not with --batch_norm: the padded rows would enter
         the batch moments)."""
         upd = self.updater
-        deferred = self.update_mode == "exact_deferred"
         self._stage_ids(batch)
-        if deferred:
-            j = self.epoch_pos
-            if j == 0:
-                upd.epoch_begin()
-            self.opt.tick_epoch(j)
-            upd.unique(self.ids_all)
-            upd.epoch_rows([(self.V, None)], j, apply=False)
-        else:
-            self.opt.tick()
+        upd.begin_step()
+        upd.catch_up(self.ids_all)
         y = self._forward(batch, train=True, masks=masks)
         n = self.B if n_valid is None else int(n_valid)
         assert 0 < n <= self.B
@@ -177,16 +147,7 @@ class ESMM:
         ops.esmm_head(y["ctr"], y["cvr"], labels[0], labels[1], n, self.w_ctr, self.w_cvr, self.pctr, self.pcvr,
                       self.pctcvr, self.losses, self.dy["ctr"], self.dy["cvr"])
         self._backward(batch)
-        if deferred:
-            upd.segment_sum(self.g_all, None)
-            upd.epoch_rows([(self.V, upd.g_uniq)], self.epoch_pos, apply=True)
-            self.epoch_pos += 1
-            if self.epoch_pos == self.epoch_steps:
-                upd.epoch_sweep(self.tables, self.epoch_steps, reset=True, l2_reg=self.l2_reg)
-                self.epoch_pos = 0
-        else:
-            upd.dedup(self.ids_all, self.g_all, None)
-            upd.apply(self.V, None, exact=(self.update_mode == "exact"), l2_reg=self.l2_reg)
+        upd.finish_step(self.ids_all, self.g_all)
         self.dense.apply()
         self.global_step += 1
         return torch.cat([self.losses, upd.reg[0:1]])

@@ -108,5 +108,5 @@ def define_common(num_threads=16, embedding_size=32, batch_size=64, learning_rat
     DEFINE_string("task_type", "train", "task type {train, infer, eval, export}")
     DEFINE_boolean("clear_existing_model", False, "clear existing model or not")
     # engine-only flag (not in the reference): how the TF-exact table update is scheduled
-    DEFINE_string("update_mode", "exact_deferred", "{exact, exact_deferred, lazy}: see tf_repos_b200/base.py")
+    DEFINE_string("update_mode", "exact_deferred", "{exact, exact_deferred, lazy}: see tf_repos_b200/engine.py (SparseUpdater)")
     DEFINE_string("input_parse", "device", "{device, host}: where the libsvm text is tokenised (same values)")

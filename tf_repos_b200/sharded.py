@@ -22,7 +22,7 @@ import torch.distributed as dist
 
 from . import ops
 from .base import floats, ints
-from .engine import DenseVars, OptimizerState, SparseUpdater, Table
+from .engine import DenseVars, OptimizerState, SparseModel, SparseUpdater, Table
 from .mlp import MLP
 
 
@@ -31,17 +31,16 @@ def local_rows(N: int, G: int, rank: int) -> int:
     return (N - rank + G - 1) // G
 
 
-class ShardedDeepFM:
+class ShardedDeepFM(SparseModel):
     def __init__(self, field_size, feature_size, embedding_size, batch_size, deep_layers="256,128,64",
                  dropout="0.5,0.5,0.5", l2_reg=1e-4, learning_rate=5e-4, optimizer="Adam", update_mode="exact",
                  device="cuda", seed=0, epoch_steps=8, group=None):
-        assert update_mode in ("exact", "exact_deferred", "lazy")
         self.group = group
         self.G = dist.get_world_size(group) if dist.is_initialized() else 1
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
         self.F, self.N, self.K, self.B = field_size, feature_size, embedding_size, batch_size
         self.layers, self.keep = ints(deep_layers), floats(dropout)
-        self.l2_reg, self.update_mode = float(l2_reg), update_mode
+        self.l2_reg = float(l2_reg)
         self.device = dev = torch.device(device)
         self.seed = seed
         G, B, F, K = self.G, self.B, self.F, self.K
@@ -80,14 +79,9 @@ class ShardedDeepFM:
         self.recv_ids = torch.zeros(R, **i32)
         self.rows_v = torch.empty(R, K, **f32); self.rows_w = torch.empty(R, **f32)
         self.recv_g = torch.empty(R, K, **f32); self.recv_gw = torch.empty(R, **f32)
-        self.updater = SparseUpdater(R, self.N_local, K, self.opt, dev, with_scalar_table=True)
+        self.updater = SparseUpdater(R, self.N_local, K, self.opt, dev, True, self.tables, update_mode,
+                                     epoch_steps, l2_reg)
         self.global_step = 0
-        self.epoch_steps, self.epoch_pos = epoch_steps, 0
-        if update_mode == "exact_deferred":
-            if self.l2_reg == 0.0 and optimizer != "Adam":
-                self.update_mode = "exact"
-            else:
-                self.updater.enable_epochs(epoch_steps, self.tables)
 
     # ---- helpers ---------------------------------------------------------------------------------------
     def _a2a(self, out, inp, out_splits, in_splits):
@@ -95,10 +89,6 @@ class ShardedDeepFM:
             out[: inp.shape[0]].copy_(inp)
         else:
             dist.all_to_all_single(out, inp, out_splits, in_splits, group=self.group)
-
-    def flush(self):
-        if self.update_mode == "exact_deferred" and self.epoch_pos > self.updater.flush_pos:
-            self.updater.epoch_sweep(self.tables, self.epoch_pos, reset=False, l2_reg=self.l2_reg)
 
     def load_global_tables(self, fm_v: torch.Tensor, fm_w: torch.Tensor):
         """test helper: take my rows (id % G == rank) of full tables"""
@@ -119,7 +109,7 @@ class ShardedDeepFM:
             out_v[r:: self.G] = bv; out_w[r:: self.G] = bw
         return out_v, out_w
 
-    def _lookup(self, ids: torch.Tensor, deferred_j=None):
+    def _lookup(self, ids: torch.Tensor, catch_up: bool = False):
         """unique -> route -> fetch rows into the cache; returns (U, send_splits, recv_splits, R)."""
         G, n = self.G, ids.numel()
         ops.shard_keys(ids.reshape(-1), self.N, G, self.keys[:n], self.oob)
@@ -138,9 +128,8 @@ class ShardedDeepFM:
         self._mark("count all-gather + host sync")
         self._a2a(self.recv_ids[:R], self.local_ids[:U], recv, send)
         self._mark("a2a ids")
-        if deferred_j is not None:   # owners bring the requested rows to the start of this step
-            self.updater.unique(self.recv_ids[:R])
-            self.updater.epoch_rows([(t, None) for t in self.tables], deferred_j, apply=False)
+        if catch_up:   # owners bring the requested rows to the start of this step
+            self.updater.catch_up(self.recv_ids[:R])
         self._mark("owner: unique + catch-up rows")
         ops.gather_scale_rows(self.recv_ids[:R], None, self.V.var, self.rows_v, 1, self.K, self.oob)
         ops.gather_scalar(self.recv_ids[:R], self.W.var, self.rows_w[:R])
@@ -230,18 +219,10 @@ class ShardedDeepFM:
     def train_step(self, ids, vals, labels, masks=None):
         B, F, K, G = ids.shape[0], self.F, self.K, self.G
         assert B == self.B
-        n = B * F
-        deferred = self.update_mode == "exact_deferred"
         upd = self.updater
         self._mark("begin")
-        if deferred:
-            j = self.epoch_pos
-            if j == 0:
-                upd.epoch_begin()
-            self.opt.tick_epoch(j)
-        else:
-            self.opt.tick()
-        U, send, recv, R = self._lookup(ids, deferred_j=(self.epoch_pos if deferred else None))
+        upd.begin_step()
+        U, send, recv, R = self._lookup(ids, catch_up=True)
         self._compute(vals, labels, masks)
         self._mark("compute segment (K1, MLP, loss, K2, seg sums)")
         self._a2a(self.recv_g[:R], self.g_cache[:U], recv, send)
@@ -249,26 +230,9 @@ class ShardedDeepFM:
         if G > 1:
             dist.all_reduce(self.dense.grad, group=self.group)
         self._mark("a2a grads (v, w) + all-reduce dense")
-        if deferred:
-            # upd.uw already holds unique(recv_ids) from the catch-up
-            upd.segment_sum(self.recv_g[:R], self.recv_gw[:R])
-            upd.epoch_rows([(self.V, upd.g_uniq), (self.W, upd.gw_uniq)], self.epoch_pos, apply=True)
-            self.epoch_pos += 1
-            if self.epoch_pos == self.epoch_steps:
-                upd.epoch_sweep(self.tables, self.epoch_steps, reset=True, l2_reg=self.l2_reg)
-                self.epoch_pos = 0
-        else:
-            upd.dedup(self.recv_ids[:R], self.recv_g[:R], self.recv_gw[:R])
-            upd.apply(self.V, self.W, exact=(self.update_mode == "exact"), l2_reg=self.l2_reg)
+        upd.finish_step(self.recv_ids[:R], self.recv_g[:R], self.recv_gw[:R])
         self._mark("owner: seg sums + row apply (+ sweep at epoch end)")
         self.dense.apply()
         self.global_step += 1
         self._mark("dense apply")
         return torch.cat([self.loss_ce, upd.reg[1:2], upd.reg[0:1]])   # reg terms: this rank's shard only
-
-    def check_ids(self):
-        self.updater.check_list_overflow()
-        cnt, first = self.oob.tolist()
-        if cnt:
-            self.oob.zero_()
-            raise IndexError(f"{cnt} ids out of range (first {first})")

@@ -20,7 +20,7 @@ import torch
 
 from . import ops
 from .base import ints
-from .engine import HYPER_TABLE, DenseVars, OptimizerState, SparseUpdater, Table
+from .engine import HYPER_TABLE, DenseVars, OptimizerState, Table
 from .mlp import MLP
 
 N_NUM, N_CAT, NUM_BUCKETS = 13, 26, 10000
@@ -48,7 +48,10 @@ class WideDeep:
         self.D = N_CAT * K + N_NUM
         self.num_perm = torch.tensor(NUM_SORTED, dtype=torch.int32, device=dev)
         self.flat_ids = torch.empty(n, dtype=torch.int32, device=dev)
-        self.upd = SparseUpdater(n, N_CAT * NUM_BUCKETS, K, self.opt_dnn, dev, with_scalar_table=True)
+        # both parts look up the same flat ids: one de-duplication, gradients summed per unique id
+        self.uw = ops.UniqueWorkspace(n, N_CAT * NUM_BUCKETS, dev)
+        self.g_uniq = torch.empty(n * K, **f32)
+        self.gw_uniq = torch.empty(n, **f32)
         self.y = torch.empty(B, **f32); self.pred = torch.empty(B, **f32); self.dy = torch.empty(B, **f32)
         self.loss = torch.zeros(1, **f32)
         self.zero_bias = torch.zeros(1, **f32)
@@ -132,22 +135,22 @@ class WideDeep:
                          self.g_cat[:n] if self.has_linear else None,
                          self.dense_lin.grads["linear/numeric"] if self.has_linear else None,
                          self.dense_lin.grads["linear/linear_model/bias_weights"] if self.has_linear else None)
-        upd, uw = self.upd, self.upd.uw
+        uw = self.uw
         uw.n_active = n
         ops.unique_segment(self.flat_ids[:n], uw)
         if self.has_dnn:
-            ops.segment_sum_rows(self.g_rows[:n], self.g_cat[:n] if self.has_linear else None, uw, self.K, upd.g_uniq,
-                                 upd.gw_uniq if self.has_linear else None)
+            ops.segment_sum_rows(self.g_rows[:n], self.g_cat[:n] if self.has_linear else None, uw, self.K, self.g_uniq,
+                                 self.gw_uniq if self.has_linear else None)
             o = self.opt_dnn
-            ops.opt_sparse_rows(o.opt, self.emb.var, self.emb.slot(0), None, uw.uniq, uw.n_uniq, upd.g_uniq, upd.n, self.K,
+            ops.opt_sparse_rows(o.opt, self.emb.var, self.emb.slot(0), None, uw.uniq, uw.n_uniq, self.g_uniq, uw.n, self.K,
                                 o.record(HYPER_TABLE), None)
             self.dense_dnn.apply()
         if self.has_linear:
             if not self.has_dnn:   # scalar rows only: the K=1 flavour of the segment sum
-                ops.segment_sum_rows(self.g_cat[:n].view(-1, 1), None, uw, 1, upd.gw_uniq, None)
+                ops.segment_sum_rows(self.g_cat[:n].view(-1, 1), None, uw, 1, self.gw_uniq, None)
             o = self.opt_lin
             ops.opt_sparse_rows(o.opt, self.wide_cat.var, self.wide_cat.slot(0), self.wide_cat.slot(1), uw.uniq, uw.n_uniq,
-                                upd.gw_uniq, upd.n, 1, o.record(HYPER_TABLE), None)
+                                self.gw_uniq, uw.n, 1, o.record(HYPER_TABLE), None)
             self.dense_lin.apply()
         self.global_step += 1
         return self.loss
