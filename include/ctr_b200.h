@@ -488,6 +488,38 @@ int ctr_criteo_emit_write(const char* text, size_t len, int test, const uint8_t*
                           const char* label, int label_len, char* out_tr, char* out_va, const void* ws,
                           size_t ws_bytes, ctr_stream_t stream);
 
+/* ---- TFRecord input of DIN / ESMM (DIN.py:57-99, DeepCvrMTL.py:63-105; DESIGN.md §2.5) ------------------------
+ * frame (HOST buffers): walks the records of buf_host[0, len) -- uint64 length | uint32 masked CRC-32C of the length |
+ *   data | uint32 masked CRC-32C of the data -- checking every header CRC, up to max_records.  rec_off[i] = byte offset
+ *   of record i's header.  info (host int64[5]) = { records, bytes consumed (whole records only), error class, error
+ *   offset, bytes the next record needs }; class 0 = none, 1 = truncated header, 2 = header CRC mismatch, 3 = truncated
+ *   record, 4 = record longer than 2^31 - 17 bytes.  A tail too short for the next record is an error only when
+ *   final_chunk != 0 (otherwise it is left unconsumed).
+ * scan (device): one warp per framed record of chunk (records from ctr_tfrecord_frame over the same bytes): the data
+ *   CRC, the protobuf walk and decode_tfrecord_files' checks.  labels_mask: bit 0 = y required (always), bit 1 = z
+ *   (ESMM).  lens int32 [n_rec][5] = value counts of u_catids, u_shopids, u_brandids, u_intids, a_intids.  err (device
+ *   uint64, set to ~0 by the caller once) is min-folded with (record_base + i) << 16 | check << 8 | arg; check 0 = data
+ *   CRC, 1 = malformed protobuf, 2 = required key missing or empty (arg = key: 0 y, 1 z, 2 feat_ids, 3 a_catids,
+ *   4 a_shopids, 5 a_brandids), 3 = feat_ids count != F, 4 = u_*ids / u_*vals lengths differ (arg = 0 cat, 1 shop,
+ *   2 brand, 3 int), 5 = wrong or several Feature kinds, 6 = id outside [0, 2^31) (arg = schema key: 0 y, 1 z,
+ *   2 feat_ids, 3-5 a_cat/shop/brandids, 6 a_intids, 7-10 u_cat/shop/brand/intids, 11-14 u_cat/shop/brand/intvals).
+ * emit (device): one batch of B slots; slot b's record data is stage[slot_off[b], + slot_len[b]) and must have passed
+ *   the scan.  Writes din_main.make_batch's tensors (feat_ids [B,F], a_ids [3,B], a_int_ids, u_ids [4,B,P] and u_wgt
+ *   [4,B,P] zero-padded, y [B]) at the caller's a_int_off [B+1], or esmm_main.make_batch's (feat_ids, a_ids, bag_ids,
+ *   bag_wgt, y, z) at the caller's bag_off [5B+1]. */
+enum { CTR_TFR_OK = 0, CTR_TFR_TRUNCATED_HEADER = 1, CTR_TFR_CORRUPTED_LENGTH = 2, CTR_TFR_TRUNCATED_RECORD = 3,
+       CTR_TFR_TOO_LARGE = 4 };
+int ctr_tfrecord_frame(const void* buf_host, size_t len, int final_chunk, int64_t* rec_off, int64_t max_records,
+                       int64_t* info);
+int ctr_tfrecord_scan(const void* chunk, size_t len, const int64_t* rec_off, int64_t n_rec, int64_t record_base, int F,
+                      int labels_mask, int32_t* lens, uint64_t* err, ctr_stream_t stream);
+int ctr_tfrecord_emit_din(const void* stage, const int64_t* slot_off, const int32_t* slot_len, int B, int F, int P,
+                          const int32_t* a_int_off, int32_t* feat_ids, int32_t* a_ids, int32_t* a_int_ids,
+                          int32_t* u_ids, float* u_wgt, float* y, ctr_stream_t stream);
+int ctr_tfrecord_emit_esmm(const void* stage, const int64_t* slot_off, const int32_t* slot_len, int B, int F,
+                           const int32_t* bag_off, int32_t* feat_ids, int32_t* a_ids, int32_t* bag_ids, float* bag_wgt,
+                           float* y, float* z, ctr_stream_t stream);
+
 /* ---- table initialisation (glorot_normal_initializer, DeepFM.py:115-116; truncated at 2 sigma) --- */
 int ctr_init_trunc_normal(float* t, int64_t n, float stddev, uint64_t seed, ctr_stream_t stream);
 int ctr_fill(float* t, int64_t n, float value, ctr_stream_t stream);

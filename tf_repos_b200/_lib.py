@@ -118,6 +118,10 @@ SIGNATURES = {
     "ctr_criteo_emit_workspace_bytes": (c_size_t, [c_size_t]),
     "ctr_criteo_emit_plan": (c_int, [P, c_size_t, c_int, c_int64, P, P, c_int64, P, P, P, P, c_int, P, P, c_size_t, P]),
     "ctr_criteo_emit_write": (c_int, [P, c_size_t, c_int, P, P, c_int64, P, P, P, P, c_int, P, P, P, c_size_t, P]),
+    "ctr_tfrecord_frame": (c_int, [P, c_size_t, c_int, P, c_int64, P]),
+    "ctr_tfrecord_scan": (c_int, [P, c_size_t, P, c_int64, c_int64, c_int, c_int, P, P, P]),
+    "ctr_tfrecord_emit_din": (c_int, [P, P, P, c_int, c_int, c_int, P, P, P, P, P, P, P, P]),
+    "ctr_tfrecord_emit_esmm": (c_int, [P, P, P, c_int, c_int, P, P, P, P, P, P, P, P]),
     "ctr_init_trunc_normal": (c_int, [P, c_int64, c_float, c_uint64, P]),
     "ctr_fill": (c_int, [P, c_int64, c_float, P]),
 }

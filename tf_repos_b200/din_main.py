@@ -63,14 +63,24 @@ def decode_tfrecord_files(files: Sequence[str], field_size: int, labels: Sequenc
     return d
 
 
+def sample_lengths(d: Dict[str, list]) -> np.ndarray:
+    """int64 [n, 5]: every sample's u_cat, u_shop, u_brand, u_int list lengths and its a_int bag length."""
+    keys = ["u_%sids" % f for f in U_FIELDS] + ["a_int"]
+    return np.asarray([[len(x) for x in d[k]] for k in keys], dtype=np.int64).T.reshape(-1, 5)
+
+
+def max_lengths_of(*lens: np.ndarray) -> Tuple[int, int]:
+    """(P, max_a_int) of sample_lengths arrays: the longest behaviour list / a_int bag (>= 1)."""
+    P = A = 1
+    for x in lens:
+        if len(x):
+            P, A = max(P, int(x[:, :4].max())), max(A, int(x[:, 4].max()))
+    return P, A
+
+
 def max_lengths(*datasets: Dict[str, list]) -> Tuple[int, int]:
     """(P, max_a_int): the longest behaviour list / a_int bag anywhere in the inputs (>= 1)."""
-    P = A = 1
-    for d in datasets:
-        for f in U_FIELDS:
-            P = max([P] + [len(x) for x in d["u_%sids" % f]])
-        A = max([A] + [len(x) for x in d["a_int"]])
-    return P, A
+    return max_lengths_of(*(sample_lengths(d) for d in datasets))
 
 
 def make_batch(d: Dict[str, list], idx: Sequence[int], B: int, P: int, device) -> Tuple[Dict[str, torch.Tensor], torch.Tensor, int]:
@@ -133,10 +143,11 @@ def run():
             print(e, "at clear_existing_model")
         else:
             print("existing model cleaned at %s" % FLAGS.model_dir)
+    from .tfrecord_device import TFRecordIndex
     F, B = FLAGS.field_size, FLAGS.batch_size
-    tr = decode_tfrecord_files(tr_files, F) if FLAGS.task_type == "train" else None
-    te = decode_tfrecord_files(te_files, F) if te_files else None
-    P, A = max_lengths(*[x for x in (tr, te) if x is not None])
+    tr = TFRecordIndex.build(tr_files, F) if FLAGS.task_type == "train" else None       # decoded on the GPU
+    te = TFRecordIndex.build(te_files, F) if te_files else None
+    P, A = max_lengths_of(*[x.lens for x in (tr, te) if x is not None])
     meta_path = os.path.join(FLAGS.model_dir, "din_shapes.json")
     if os.path.exists(meta_path):     # buffers are sized at first training; later tasks must not shrink them
         m = json.load(open(meta_path))
@@ -146,12 +157,10 @@ def run():
                 l2_reg=FLAGS.l2_reg, learning_rate=FLAGS.learning_rate, optimizer=FLAGS.optimizer,
                 update_mode=FLAGS.update_mode, batch_norm=FLAGS.batch_norm, batch_norm_decay=FLAGS.batch_norm_decay)
     restore_checkpoint(model, FLAGS.model_dir)
-    dev = model.device
 
     def score(d) -> Tuple[np.ndarray, np.ndarray]:
         preds, labs = [], []
-        for idx in index_stream(len(d["y"]), 1, B):
-            batch, labels, n = make_batch(d, idx, B, P, dev)
+        for batch, labels, n in d.batches(1, B, "din", P):
             preds.append(model.predict(batch)[:n].cpu().numpy().copy()); labs.append(labels[:n].cpu().numpy())
         model.check_ids()
         return (np.concatenate(preds), np.concatenate(labs)) if preds else (np.zeros(0, np.float32), np.zeros(0, np.float32))
@@ -166,8 +175,7 @@ def run():
 
     if FLAGS.task_type == "train":
         t0, s0, last = time.time(), model.global_step, None
-        for idx in index_stream(len(tr["y"]), FLAGS.num_epochs, B):
-            batch, labels, n = make_batch(tr, idx, B, P, dev)
+        for batch, labels, n in tr.batches(FLAGS.num_epochs, B, "din", P):
             last = model.train_step(batch, labels, n_valid=n)      # the final batch may be partial (kept, DIN.py:93-94)
             if model.global_step % FLAGS.log_steps == 0:
                 dt = time.time() - t0

@@ -42,7 +42,11 @@ def sample_occurrences(d: Dict[str, list]) -> np.ndarray:
 
 def max_batch_occurrences(d: Dict[str, list], num_epochs: int, B: int) -> int:
     """the largest occurrence count of any batch index_stream(n, num_epochs, B) yields, the padded last one included"""
-    occ = sample_occurrences(d)
+    return batch_occurrence_max(sample_occurrences(d), num_epochs, B)
+
+
+def batch_occurrence_max(occ: np.ndarray, num_epochs: int, B: int) -> int:
+    """max_batch_occurrences of the per-sample occurrence counts `occ`"""
     n = len(occ)
     if n == 0 or num_epochs <= 0:
         return 0
@@ -106,11 +110,12 @@ def run():
     if FLAGS.task_type == "export":                  # DeepCvrMTL.py:383-384
         print("Not Implemented, Do It Yourself!")
         return None
+    from .tfrecord_device import TFRecordIndex
     F, B = FLAGS.field_size, FLAGS.batch_size
-    tr = decode(tr_files, F) if FLAGS.task_type == "train" else None
-    te = decode(te_files, F) if te_files else None
-    cap = max([1] + ([max_batch_occurrences(tr, FLAGS.num_epochs, B)] if tr else []) +
-              ([max_batch_occurrences(te, 1, B)] if te else []))
+    tr = TFRecordIndex.build(tr_files, F, ("y", "z")) if FLAGS.task_type == "train" else None   # decoded on the GPU
+    te = TFRecordIndex.build(te_files, F, ("y", "z")) if te_files else None
+    cap = max([1] + ([tr.max_batch_occurrences(FLAGS.num_epochs, B)] if tr is not None else []) +
+              ([te.max_batch_occurrences(1, B)] if te is not None else []))
     meta_path = os.path.join(FLAGS.model_dir, "esmm_shapes.json")
     if os.path.exists(meta_path):     # sized at first training; later tasks must not shrink it
         cap = max(cap, json.load(open(meta_path))["occ_capacity"])
@@ -123,8 +128,7 @@ def run():
 
     def score(d, with_loss: bool):
         out, losses = {"pctr": [], "pcvr": [], "pctcvr": [], "y": [], "z": []}, []
-        for idx in index_stream(len(d["y"]), 1, B):
-            batch, (y, z), n = make_batch(d, idx, B, dev)
+        for batch, (y, z), n in d.batches(1, B, "esmm"):
             p = model.predict(batch, (y, z) if with_loss else None, n)
             for k, v in zip(("pctr", "pcvr", "pctcvr"), p):
                 out[k].append(v[:n].cpu().numpy().copy())
@@ -150,8 +154,7 @@ def run():
 
     if FLAGS.task_type == "train":
         t0, s0, last = time.time(), model.global_step, None
-        for idx in index_stream(len(tr["y"]), FLAGS.num_epochs, B):
-            batch, labels, n = make_batch(tr, idx, B, dev)
+        for batch, labels, n in tr.batches(FLAGS.num_epochs, B, "esmm"):
             last = model.train_step(batch, labels, n_valid=n)      # the final batch may be partial (kept, :97-98)
             if model.global_step % FLAGS.log_steps == 0:
                 dt = time.time() - t0

@@ -622,6 +622,44 @@ def parse_libsvm_device(text: torch.Tensor, F: int, max_rows: int, final_chunk: 
     return ids[:rows], vals[:rows], labels[:rows], consumed, bool(blank or bad or host)
 
 
+def tfrecord_frame(buf, final_chunk: bool, max_records: int):
+    """Frames the TFRecords of a host uint8 numpy buffer (ctr_tfrecord_frame).  Returns (rec_off int64 [records],
+    consumed, error class, error offset, bytes the next record needs)."""
+    import numpy as np
+    rec_off = np.empty(max(max_records, 1), dtype=np.int64)
+    info = np.zeros(5, dtype=np.int64)
+    check(_L.ctr_tfrecord_frame(buf.ctypes.data, buf.nbytes, int(final_chunk), rec_off.ctypes.data, max_records,
+                                info.ctypes.data), "ctr_tfrecord_frame")
+    n, consumed, cls, at, need = (int(x) for x in info)
+    return rec_off[:n], consumed, cls, at, need
+
+
+def tfrecord_scan(chunk, rec_off, record_base: int, F: int, labels_mask: int, lens, err):
+    """Pass 1 over the framed records of a uint8 CUDA chunk: lens int32 [n,5], err uint64-as-int64 [1] (min-folded)."""
+    n = rec_off.numel()
+    check(_L.ctr_tfrecord_scan(_p(chunk, torch.uint8, "chunk"), chunk.numel(), _p(rec_off, torch.int64, "rec_off"), n,
+                               record_base, F, labels_mask, _p(lens, torch.int32, "lens"), _p(err, torch.int64, "err"),
+                               _stream()), "ctr_tfrecord_scan")
+
+
+def tfrecord_emit_din(stage, slot_off, slot_len, B, F, P, a_int_off, feat_ids, a_ids, a_int_ids, u_ids, u_wgt, y):
+    check(_L.ctr_tfrecord_emit_din(_p(stage, torch.uint8, "stage"), _p(slot_off, torch.int64, "slot_off"),
+                                   _p(slot_len, torch.int32, "slot_len"), B, F, P, _p(a_int_off, torch.int32, "a_int_off"),
+                                   _p(feat_ids, torch.int32, "feat_ids"), _p(a_ids, torch.int32, "a_ids"),
+                                   _p(a_int_ids, torch.int32, "a_int_ids"), _p(u_ids, torch.int32, "u_ids"),
+                                   _p(u_wgt, torch.float32, "u_wgt"), _p(y, torch.float32, "y"), _stream()),
+          "ctr_tfrecord_emit_din")
+
+
+def tfrecord_emit_esmm(stage, slot_off, slot_len, B, F, bag_off, feat_ids, a_ids, bag_ids, bag_wgt, y, z):
+    check(_L.ctr_tfrecord_emit_esmm(_p(stage, torch.uint8, "stage"), _p(slot_off, torch.int64, "slot_off"),
+                                    _p(slot_len, torch.int32, "slot_len"), B, F, _p(bag_off, torch.int32, "bag_off"),
+                                    _p(feat_ids, torch.int32, "feat_ids"), _p(a_ids, torch.int32, "a_ids"),
+                                    _p(bag_ids, torch.int32, "bag_ids"), _p(bag_wgt, torch.float32, "bag_wgt"),
+                                    _p(y, torch.float32, "y"), _p(z, torch.float32, "z"), _stream()),
+          "ctr_tfrecord_emit_esmm")
+
+
 def init_trunc_normal(t, stddev: float, seed: int):
     check(_L.ctr_init_trunc_normal(_p(t, torch.float32, "t"), t.numel(), float(stddev), int(seed), _stream()),
           "ctr_init_trunc_normal")
