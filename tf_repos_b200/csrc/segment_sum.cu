@@ -137,24 +137,47 @@ segsum_long_kernel(const float* __restrict__ g_rows, const float* __restrict__ g
 
 // Long runs split into chunks of SEG_CHUNK occurrences (the 13 continuous-feature ids of the Criteo layout occur B
 // times; DIN's padding id occurs ~10^6 times per step): segsum_long_plan_kernel gives every long run a range of partial
-// rows (base from an atomic counter -- which rows a run gets may differ from launch to launch, what is stored in them and
-// the order they are added in does not), segsum_long_split_kernel sums chunk c of run li with the lane-group striding +
-// fixed tree, segsum_long_final_kernel adds a run's partials in chunk order.  A run that does not get a range (scratch
-// exhausted) is summed by one CTA in the same kernel.  Fixed shapes => bit-reproducible.
+// rows, segsum_long_split_kernel sums chunk c of run li with the lane-group striding + fixed tree,
+// segsum_long_final_kernel adds a run's partials in chunk order.  A run that does not get a range (scratch exhausted)
+// is summed by one CTA in the same kernel -- a different tree, so which runs get a range must not depend on launch
+// order: long_list is filled by atomics in no fixed order, so the plan hands out rows in ascending u instead.  A run's
+// base is the chunk count of all long runs with a smaller u; it gets no range when base + chunks > cap_rows.  Fixed
+// shapes and a plan that is a function of the segments alone => bit-reproducible.
 constexpr int SEG_CHUNK = 1024;
 
-// plan[0] = partial rows handed out; then per long run li: plan[1 + 2*li] = base row, plan[2 + 2*li] = number of chunks
-__global__ void segsum_long_plan_kernel(const int32_t* __restrict__ seg_offsets, const int32_t* __restrict__ long_list,
-                                        int max_long, int cap_rows, int32_t* __restrict__ plan) {
+// per long run li: plan[1 + 2*li] = base row (-1: no range), plan[2 + 2*li] = number of chunks.  One CTA; each run
+// counts the chunks of the runs before it in u order from shared-memory tiles of long_list (n_long^2 / 256
+// shared-memory adds per thread; n_long is 13 in the Criteo layout and 1 in DIN's).
+constexpr int PLAN_THREADS = 256;
+__device__ __forceinline__ int seg_chunks(const int32_t* __restrict__ seg_offsets, int u) {
+  return (seg_offsets[u + 1] - seg_offsets[u] + SEG_CHUNK - 1) / SEG_CHUNK;
+}
+__global__ void __launch_bounds__(PLAN_THREADS)
+segsum_long_plan_kernel(const int32_t* __restrict__ seg_offsets, const int32_t* __restrict__ long_list, int max_long,
+                        int cap_rows, int32_t* __restrict__ plan) {
+  __shared__ int su[PLAN_THREADS], sc[PLAN_THREADS];
   const int n_long = min(long_list[0], max_long);
-  for (int li = blockIdx.x * blockDim.x + threadIdx.x; li < n_long; li += gridDim.x * blockDim.x) {
-    const int u = long_list[1 + li];
-    const int len = seg_offsets[u + 1] - seg_offsets[u];
-    int chunks = (len + SEG_CHUNK - 1) / SEG_CHUNK;
-    int base = atomicAdd(&plan[0], chunks);
-    if (base + chunks > cap_rows) { base = -1; chunks = 1; }   // no room: whole run by one CTA, straight to the output
-    plan[1 + 2 * li] = base;
-    plan[2 + 2 * li] = chunks;
+  for (int li0 = 0; li0 < n_long; li0 += PLAN_THREADS) {
+    const int li = li0 + threadIdx.x;
+    const int u = li < n_long ? long_list[1 + li] : 0;
+    int chunks = li < n_long ? seg_chunks(seg_offsets, u) : 0;
+    int base = 0;
+    for (int t0 = 0; t0 < n_long; t0 += PLAN_THREADS) {
+      __syncthreads();
+      const int tj = t0 + threadIdx.x;
+      if (tj < n_long) {
+        su[threadIdx.x] = long_list[1 + tj];
+        sc[threadIdx.x] = seg_chunks(seg_offsets, su[threadIdx.x]);
+      }
+      __syncthreads();
+      const int m = min(PLAN_THREADS, n_long - t0);
+      for (int j = 0; j < m; ++j) base += su[j] < u ? sc[j] : 0;
+    }
+    if (li < n_long) {
+      if (base + chunks > cap_rows) { base = -1; chunks = 1; }   // no room: whole run by one CTA, straight to the output
+      plan[1 + 2 * li] = base;
+      plan[2 + 2 * li] = chunks;
+    }
   }
 }
 
@@ -275,7 +298,7 @@ extern "C" int ctr_segment_sum_rows(const float* g_rows, const float* g_w, const
   cudaStream_t st = as_stream(stream);
   const int long_grid = 2 * sm_count();
   // optional scratch (the K3 workspace is free by now): long runs are cut into chunks of SEG_CHUNK occurrences.
-  // layout: int32 plan[1 + 2*max_long] | float partial[cap_rows][K+4]
+  // layout: int32 plan[1 + 2*max_long] (plan[0] unused) | float partial[cap_rows][K+4]
   const int64_t max_long = n / (CTR_LONG_SEG + 1) + 1;
   const size_t plan_bytes = ((size_t)(1 + 2 * max_long) * sizeof(int32_t) + 15) & ~(size_t)15;
   const int64_t want_rows = n / SEG_CHUNK + max_long;       // every run: its full chunks + at most one partial chunk
@@ -293,8 +316,8 @@ extern "C" int ctr_segment_sum_rows(const float* g_rows, const float* g_w, const
                                                           n, g_uniq, gw_uniq);                      \
     CTR_LAUNCHED("segsum_short");                                                                   \
     if (split) {                                                                                    \
-      cudaMemsetAsync(plan, 0, sizeof(int32_t), st);                                                \
-      segsum_long_plan_kernel<<<8, 256, 0, st>>>(seg_offsets, long_list, (int)max_long, (int)cap_rows, plan); \
+      segsum_long_plan_kernel<<<1, PLAN_THREADS, 0, st>>>(seg_offsets, long_list, (int)max_long, (int)cap_rows, \
+                                                          plan);                                    \
       CTR_LAUNCHED("segsum_long_plan");                                                             \
       segsum_long_split_kernel<LPR, VEC><<<dim3(64, 16), 256, 0, st>>>(                             \
           g_rows, g_w, perm, seg_offsets, long_list, (int)max_long, plan, partial, g_uniq, gw_uniq); \
