@@ -520,6 +520,30 @@ int ctr_tfrecord_emit_esmm(const void* stage, const int64_t* slot_off, const int
                            const int32_t* bag_off, int32_t* feat_ids, int32_t* a_ids, int32_t* bag_ids, float* bag_wgt,
                            float* y, float* z, ctr_stream_t stream);
 
+/* ---- Ali-CCP TFRecord writer (deep_ctr/Feature_pipeline/get_aliccp_tfrecord.py; DESIGN.md §2.6) ----------------
+ * Joined Ali-CCP lines `id,y,z,field:fid:val ...` -> framed tf.Example records, byte-identical to
+ * tfrecord.write_records(path, [tfrecord.encode_example(features) ...]) of the features gen_tfrecords builds.  `text` is
+ * a chunk of whole lines (a last line without '\n' counts), len <= 2^31; line_base = index of its first line in the
+ * file.  plan, declines and write share one workspace of ctr_aliccp_workspace_bytes(len) bytes and run over the same
+ * text, in that order.
+ * plan (replaces :42-94, the per-line parse): info int64[4] = {lines, error word, output bytes, declined numbers}.
+ *   Error word (~0 = none) = the smallest (line_base + line) << 8 | code; code 1 = NUL byte in the line, 2 = token
+ *   count not a multiple of 3 (the reference's reshape raises), 3 = empty token, 4 = kept field's fid not [0-9]+ below
+ *   2^63 (restrictions; a non-integer fid also raises in the reference).
+ * declines (only when info[3] > 0): spans int64[info[3]][3] = (line in the chunk, start, end) of every y, z and user
+ *   multi-hot value the device does not convert (anything but plain decimal with mantissa <= 2^53 and |exponent| <=
+ *   22), in line order.
+ * write (replaces :48-98, the Example and the TFRecordWriter; only after a plan without error): decl_vals float[info[3]]
+ *   = float32(float(token)) of every declined span (null when there are none); out[info[2]] = the records of the
+ *   chunk's 4-field lines, in line order. */
+size_t ctr_aliccp_workspace_bytes(size_t len);
+int ctr_aliccp_plan(const char* text, size_t len, int64_t line_base, int64_t* info, void* ws, size_t ws_bytes,
+                    ctr_stream_t stream);
+int ctr_aliccp_declines(const char* text, size_t len, const void* ws, size_t ws_bytes, int64_t* spans,
+                        ctr_stream_t stream);
+int ctr_aliccp_write(const char* text, size_t len, const float* decl_vals, void* out, const void* ws, size_t ws_bytes,
+                     ctr_stream_t stream);
+
 /* ---- table initialisation (glorot_normal_initializer, DeepFM.py:115-116; truncated at 2 sigma) --- */
 int ctr_init_trunc_normal(float* t, int64_t n, float stddev, uint64_t seed, ctr_stream_t stream);
 int ctr_fill(float* t, int64_t n, float value, ctr_stream_t stream);

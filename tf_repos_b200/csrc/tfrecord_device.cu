@@ -21,12 +21,12 @@
 //   4 u_*ids / u_*vals lengths differ (arg = field) | 5 wrong or several Feature kinds (arg = key) |
 //   6 id outside [0, 2^31) (arg = key)
 #include "common.cuh"
+#include "crc32c.cuh"
 
 namespace ctr {
 
 constexpr int TR_KEYS = 15;
 constexpr int TR_THREADS = 256, TR_WARPS = TR_THREADS / 32;
-constexpr uint32_t TR_POLY = 0x82F63B78u;  // CRC-32C, reflected
 constexpr int TR_ALL = 0x7FFFFFFF;
 enum { TK_Y = 0, TK_Z = 1, TK_FEAT = 2, TK_ACAT = 3, TK_AINT = 6, TK_UIDS = 7, TK_UVALS = 11 };
 enum { TE_CRC = 0, TE_MALFORMED = 1, TE_REQUIRED = 2, TE_COUNT = 3, TE_MISMATCH = 4, TE_KIND = 5, TE_RANGE = 6 };
@@ -48,41 +48,9 @@ __device__ __forceinline__ float tr_float(uint32_t bits) {   // float -> Python 
   return __uint_as_float(bits);
 }
 
-// ---- CRC-32C: each lane CRCs 1/32 of the record, the 32 remainders are combined with x^(8n) mod P ---------------
-__device__ __forceinline__ uint32_t gf_mul(uint32_t a, uint32_t b) {   // reflected GF(2)[x] / P: bit 31 is x^0
-  uint32_t p = 0;
-#pragma unroll 4
-  for (int i = 0; i < 32; ++i) {
-    if (a & 0x80000000u) p ^= b;
-    a <<= 1;
-    b = (b & 1) ? (b >> 1) ^ TR_POLY : b >> 1;
-  }
-  return p;
-}
-__device__ __forceinline__ uint32_t gf_x8n(const uint32_t* x8, uint64_t n) {   // x^(8n) mod P; x8[k] = x^(8*2^k)
-  uint32_t r = 0x80000000u;
-  for (int k = 0; n; ++k, n >>= 1)
-    if (n & 1) r = gf_mul(r, x8[k]);
-  return r;
-}
-// The data is read as 32 equal segments of a stream with 32*seg - L zero bytes in front: leading zeros leave a CRC
-// with zero initial value unchanged, so every segment is shifted by a multiple of seg bytes and the tree needs one
-// constant per level.
-__device__ uint32_t tr_crc32c(const uint8_t* d, int64_t L, const uint32_t* tab, const uint32_t* x8) {
-  const int lane = tr_lane();
-  const int64_t seg = (L + 31) >> 5, z = 32 * seg - L;
-  int64_t lo = lane * seg - z, hi = lo + seg;
-  lo = lo < 0 ? 0 : lo;
-  uint32_t c = 0;
-  for (int64_t p = lo; p < hi; ++p) c = tab[(c ^ tr_byte(d, p)) & 0xFF] ^ (c >> 8);
-  uint32_t M = gf_x8n(x8, (uint64_t)seg);
-  for (int k = 1; k < 32; k <<= 1) {
-    const uint32_t partner = __shfl_down_sync(FULL_MASK, c, k);
-    if ((lane & (2 * k - 1)) == 0) c = gf_mul(c, M) ^ partner;
-    M = gf_mul(M, M);
-  }
-  c = __shfl_sync(FULL_MASK, c, 0);
-  return c ^ gf_mul(0xFFFFFFFFu, gf_x8n(x8, (uint64_t)L)) ^ 0xFFFFFFFFu;
+// ---- CRC-32C (crc32c.cuh): each lane CRCs 1/32 of the record ---------------------------------------------------
+__device__ __forceinline__ uint32_t tr_crc32c(const uint8_t* d, int64_t L, const uint32_t* tab, const uint32_t* x8) {
+  return crc32c_warp(d, L, tab, x8, CrcLdg{});
 }
 
 // ---- protobuf wire format (warp-uniform: every lane calls these with the same arguments) -------------------------
@@ -332,19 +300,6 @@ __device__ int tr_checks(const TrSlot* slot, int F, int labels_mask) {
   for (int k = 0; k < TR_KEYS; ++k)
     if (slot[k].fs >= 0 && slot[k].r.range_bad) return TE_RANGE << 8 | k;
   return -1;
-}
-
-__device__ void tr_crc_tables(uint32_t* tab, uint32_t* x8) {
-  for (int i = threadIdx.x; i < 256; i += blockDim.x) {
-    uint32_t c = i;
-    for (int k = 0; k < 8; ++k) c = (c & 1) ? (c >> 1) ^ TR_POLY : c >> 1;
-    tab[i] = c;
-  }
-  if (threadIdx.x == 0) {
-    x8[0] = 0x00800000u;   // x^8
-    for (int k = 1; k < 64; ++k) x8[k] = gf_mul(x8[k - 1], x8[k - 1]);
-  }
-  __syncthreads();
 }
 
 __global__ void __launch_bounds__(TR_THREADS) tr_scan_kernel(const uint8_t* __restrict__ chunk,
