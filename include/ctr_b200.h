@@ -544,6 +544,65 @@ int ctr_aliccp_declines(const char* text, size_t len, const void* ws, size_t ws_
 int ctr_aliccp_write(const char* text, size_t len, const float* decl_vals, void* out, const void* ws, size_t ws_bytes,
                      ctr_stream_t stream);
 
+/* ---- Ali-CCP sample stage (DeepMTL/Feature_pipeline/get_join_*.py, get_stat_*.py, get_remap_mapper.py; DESIGN.md
+ * §2.7) --------------------------------------------------------------------------------------------------------------
+ * Raw Tianchi lines -> `r_i\tsample_id,y,z,field:id:val ...` part files and feat_cnts.  Tables: the count table
+ * (ctr_aliccp_sample_count_table_bytes(cap), zeroed) keys (field, fid) of the train set; the md5 table
+ * (ctr_aliccp_sample_md5_table_bytes(cap): its first 72 * cap bytes zeroed, the last 8 * cap set to 0xFF) keys the md5s
+ * of one set.  Chunks are whole lines (a last line without '\n' counts), len < 2^30, n_lines = the chunk's line count.
+ * classify (replaces get_join_mapper.py:15-40 and, mode 2, get_stat_mapper.py:16-19 over each sample's own tokens;
+ *   mode 0 = classify only, 1 = insert md5s, 2 = also count): info int64[9] = {lines, first restricted line in the chunk
+ *   (~0 = none), y=0/z=1 samples, skipped lines, count-table overflows, md5-table overflows, common records, their
+ *   feat_list bytes, kept samples}.  The workspace (ctr_aliccp_sample_chunk_workspace_bytes) then feeds place.
+ * place (get_join_reducer.py:18-22): common records' feat_lists -> arena[arena_base ...], rec_off / rec_len / rec_slot
+ *   from rec_base on, each md5's record = its last one; samples -> s_rec (md5 slot), s_key (part << 31 | r_i).
+ * resolve (get_join_reducer.py:26-33): s_rec := the slot's record (-1: none); mult[r] = samples joined to record r;
+ *   info int64[2] = {samples without a record, superseded records}.
+ * count_commons (get_stat_mapper.py:17-19 over the joined common tokens): each token of record r adds mult[r];
+ *   info[0] = count-table overflows.
+ * vocab (get_stat_reducer.py, get_remap_mapper.py:10-21 under DESIGN.md §2.7's rule): vocab uint64[cap] = the fids
+ *   with a (field, fid) count >= cutoff, ascending (id = 20 + index); info int64[5] = {entries, kept (field, fid),
+ *   kept fids, -, feat_cnts bytes}.  feat_cnts (after vocab, same workspace): the feat_cnts text.
+ * render: out == null: r_off int64[n + 1] = exclusive scan of each record's remapped text length (0 unless mult > 0);
+ *   else the texts at r_off.
+ * emit (get_remap_mapper.py:28-40): out == null: s_val[k] = the output line size of sample k, info[0] = lines with an
+ *   empty feature field; else every sample with lo <= s_val[k] < hi (s_val = offsets from order) written at
+ *   out + s_val[k] - lo.
+ * order: s_key sorted stably (so ties keep line order), s_val sizes -> offsets in (part, r_i, line) order,
+ *   part_bytes int64[parts]. */
+size_t ctr_aliccp_sample_count_table_bytes(int64_t capacity);
+size_t ctr_aliccp_sample_md5_table_bytes(int64_t capacity);
+size_t ctr_aliccp_sample_chunk_workspace_bytes(size_t len, int64_t n_lines);
+int ctr_aliccp_sample_classify(const char* text, size_t len, int64_t n_lines, int mode, void* count_table,
+                               int64_t count_capacity, void* md5_table, int64_t md5_capacity, int64_t* info,
+                               void* ws, size_t ws_bytes, ctr_stream_t stream);
+int ctr_aliccp_sample_place(const char* text, size_t len, int64_t n_lines, int64_t line_base, uint64_t seed,
+                            int64_t parts, void* md5_table, int64_t md5_capacity, uint8_t* arena, int64_t arena_base,
+                            int64_t* rec_off, int32_t* rec_len, int32_t* rec_slot, int64_t rec_base, int32_t* s_rec,
+                            uint64_t* s_key, int64_t sample_base, const void* ws, size_t ws_bytes,
+                            ctr_stream_t stream);
+int ctr_aliccp_sample_resolve(const void* md5_table, int64_t md5_capacity, int32_t* s_rec, int64_t n_samples,
+                              const int32_t* rec_slot, int64_t n_records, uint32_t* mult, int64_t* info,
+                              ctr_stream_t stream);
+int ctr_aliccp_sample_count_commons(const uint8_t* arena, const int64_t* rec_off, const int32_t* rec_len,
+                                    const uint32_t* mult, int64_t n_records, void* count_table, int64_t count_capacity,
+                                    int64_t* info, ctr_stream_t stream);
+size_t ctr_aliccp_sample_vocab_workspace_bytes(int64_t count_capacity);
+int ctr_aliccp_sample_vocab(const void* count_table, int64_t count_capacity, int64_t cutoff, uint64_t* vocab,
+                            int64_t* info, void* ws, size_t ws_bytes, ctr_stream_t stream);
+int ctr_aliccp_sample_feat_cnts(char* out, const void* ws, size_t ws_bytes, int64_t count_capacity,
+                                ctr_stream_t stream);
+int ctr_aliccp_sample_render(const uint8_t* arena, const int64_t* rec_off, const int32_t* rec_len,
+                             const uint32_t* mult, int64_t n_records, const uint64_t* vocab, int64_t n_vocab,
+                             int64_t* r_off, char* out, ctr_stream_t stream);
+int ctr_aliccp_sample_emit(const char* text, size_t len, int64_t n_lines, int64_t line_base, uint64_t seed,
+                           const int32_t* s_rec, int64_t sample_base, const int64_t* r_off, const char* rendered,
+                           const uint64_t* vocab, int64_t n_vocab, int64_t* s_val, int64_t lo, int64_t hi, char* out,
+                           int64_t* info, void* ws, size_t ws_bytes, ctr_stream_t stream);
+size_t ctr_aliccp_sample_order_workspace_bytes(int64_t n_samples);
+int ctr_aliccp_sample_order(uint64_t* s_key, int64_t* s_val, int64_t n_samples, int64_t parts, int64_t* part_bytes,
+                            void* ws, size_t ws_bytes, ctr_stream_t stream);
+
 /* ---- table initialisation (glorot_normal_initializer, DeepFM.py:115-116; truncated at 2 sigma) --- */
 int ctr_init_trunc_normal(float* t, int64_t n, float stddev, uint64_t seed, ctr_stream_t stream);
 int ctr_fill(float* t, int64_t n, float value, ctr_stream_t stream);

@@ -126,6 +126,22 @@ SIGNATURES = {
     "ctr_aliccp_plan": (c_int, [P, c_size_t, c_int64, P, P, c_size_t, P]),
     "ctr_aliccp_declines": (c_int, [P, c_size_t, P, c_size_t, P, P]),
     "ctr_aliccp_write": (c_int, [P, c_size_t, P, P, P, c_size_t, P]),
+    "ctr_aliccp_sample_count_table_bytes": (c_size_t, [c_int64]),
+    "ctr_aliccp_sample_md5_table_bytes": (c_size_t, [c_int64]),
+    "ctr_aliccp_sample_chunk_workspace_bytes": (c_size_t, [c_size_t, c_int64]),
+    "ctr_aliccp_sample_classify": (c_int, [P, c_size_t, c_int64, c_int, P, c_int64, P, c_int64, P, P, c_size_t, P]),
+    "ctr_aliccp_sample_place": (c_int, [P, c_size_t, c_int64, c_int64, c_uint64, c_int64, P, c_int64, P, c_int64, P, P,
+                                        P, c_int64, P, P, c_int64, P, c_size_t, P]),
+    "ctr_aliccp_sample_resolve": (c_int, [P, c_int64, P, c_int64, P, c_int64, P, P, P]),
+    "ctr_aliccp_sample_count_commons": (c_int, [P, P, P, P, c_int64, P, c_int64, P, P]),
+    "ctr_aliccp_sample_vocab_workspace_bytes": (c_size_t, [c_int64]),
+    "ctr_aliccp_sample_vocab": (c_int, [P, c_int64, c_int64, P, P, P, c_size_t, P]),
+    "ctr_aliccp_sample_feat_cnts": (c_int, [P, P, c_size_t, c_int64, P]),
+    "ctr_aliccp_sample_render": (c_int, [P, P, P, P, c_int64, P, c_int64, P, P, P]),
+    "ctr_aliccp_sample_emit": (c_int, [P, c_size_t, c_int64, c_int64, c_uint64, P, c_int64, P, P, P, c_int64, P, c_int64,
+                                       c_int64, P, P, P, c_size_t, P]),
+    "ctr_aliccp_sample_order_workspace_bytes": (c_size_t, [c_int64]),
+    "ctr_aliccp_sample_order": (c_int, [P, P, c_int64, c_int64, P, P, c_size_t, P]),
     "ctr_init_trunc_normal": (c_int, [P, c_int64, c_float, c_uint64, P]),
     "ctr_fill": (c_int, [P, c_int64, c_float, P]),
 }
