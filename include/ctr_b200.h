@@ -184,6 +184,16 @@ int ctr_epoch_rows2(int opt, int apply, float* var, float* slot0, float* slot1, 
                     float* w_slot1, uint8_t* w_last, const int32_t* uniq, const int32_t* n_uniq, const float* g_uniq,
                     const float* gw_uniq, int64_t n_max, int K, const float* hyper, const float* lr_table, int j, double* ss,
                     double* ss_w, ctr_stream_t stream);
+/* ctr_epoch_rows2 with the catch-up (apply=0) and the apply (apply=1) of the same step j handing the rows over through
+ * stage (device float[n_max * 3K]) and w_stage (device float[n_max * 3]), indexed by unique row: the catch-up writes
+ * the caught-up var | slot0 | slot1 there and only var back to the tables; the apply reads them from there and writes
+ * every row, slot and `last` byte.  Same results as ctr_epoch_rows2.  Both calls of a step must use the same uniq /
+ * n_uniq and stage, and between them only var of the gathered rows may be read (the slots and `last` are stale). */
+int ctr_epoch_rows2_staged(int opt, int apply, float* var, float* slot0, float* slot1, uint8_t* last, float* w_var,
+                           float* w_slot0, float* w_slot1, uint8_t* w_last, const int32_t* uniq, const int32_t* n_uniq,
+                           const float* g_uniq, const float* gw_uniq, int64_t n_max, int K, const float* hyper,
+                           const float* lr_table, int j, double* ss, double* ss_w, float* stage, float* w_stage,
+                           ctr_stream_t stream);
 /* All rows -> state after `upto` steps of this epoch.  Rows whose `last` byte equals `from` (nothing gathered
  * them since the previous sweep; from = 0 after an epoch-end sweep) replay steps from..upto-1; the others replay
  * last..upto-1.  reset != 0: epoch end, every `last` byte returns to 0; reset == 0: mid-epoch flush, `last` = upto.
@@ -210,6 +220,19 @@ int ctr_epoch_sweep_ovf(int opt, float* var, float* slot0, float* slot1, uint8_t
                         const float* hyper, const float* lr_table, int from, int upto, int reset, double* ss_partials,
                         int* n_partials_host, int32_t* list, int64_t list_cap, int32_t* list_count, double* ss_rows,
                         int32_t* list_overflow, ctr_stream_t stream);
+/* ctr_epoch_sweep_ovf for the [N,K] table AND a scalar table [N] gathered with the same ids (fm_v + fm_w) that share
+ * ONE `last` byte per row (pass the same `last` to ctr_epoch_rows2 as both last and w_last): one launch sweeps both
+ * tables, rows gathered since `from` go to one list, and its catch-up steps both tables.  Adam with the packed sweep
+ * only (ctr_epoch_sweep2_supported: K in {4, 8, ..., 256}, n_rows % 4 == 0, CTR_EPOCH_SCALAR unset); otherwise keep
+ * one `last` array per table and call ctr_epoch_sweep_ovf per table.  ss_partials / w_ss_partials and ss_rows /
+ * w_ss_rows are each table's as in ctr_epoch_sweep.  CAPACITY: as ctr_epoch_sweep; the list holds each gathered ROW
+ * once (not once per table), so the same list_cap covers both tables, and list_overflow counts dropped rows. */
+int ctr_epoch_sweep2_supported(int opt, int64_t n_rows, int K);
+int ctr_epoch_sweep2(int opt, float* var, float* slot0, float* slot1, float* w_var, float* w_slot0, float* w_slot1,
+                     uint8_t* last, int64_t n_rows, int K, const float* hyper, const float* lr_table, int from, int upto,
+                     int reset, double* ss_partials, double* w_ss_partials, int* n_partials_host, int32_t* list,
+                     int64_t list_cap, int32_t* list_count, double* ss_rows, double* w_ss_rows, int32_t* list_overflow,
+                     ctr_stream_t stream);
 /* reg[s] (+)= scale*(ss_rows[s] + sum_b ss_partials[s][b]) for s < upto; clears ss_rows[s] */
 int ctr_epoch_reg_loss(double* ss_rows, const double* ss_partials, int n_partials, int upto, float scale,
                        float* reg, int accumulate, ctr_stream_t stream);

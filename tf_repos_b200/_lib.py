@@ -50,10 +50,15 @@ SIGNATURES = {
     "ctr_epoch_tick": (c_int, [P, P, c_int, P, c_int, c_int, P]),
     "ctr_epoch_rows": (c_int, [c_int, c_int, P, P, P, P, P, P, P, c_int64, c_int, P, P, c_int, P, P]),
     "ctr_epoch_rows2": (c_int, [c_int, c_int, P, P, P, P, P, P, P, P, P, P, P, P, c_int64, c_int, P, P, c_int, P, P, P]),
+    "ctr_epoch_rows2_staged": (c_int, [c_int, c_int, P, P, P, P, P, P, P, P, P, P, P, P, c_int64, c_int, P, P, c_int, P,
+                                       P, P, P, P]),
     "ctr_epoch_sweep": (c_int, [c_int, P, P, P, P, c_int64, c_int, P, P, c_int, c_int, c_int, P,
                                 ctypes.POINTER(c_int), P, c_int64, P, P, P]),
     "ctr_epoch_sweep_ovf": (c_int, [c_int, P, P, P, P, c_int64, c_int, P, P, c_int, c_int, c_int, P,
                                     ctypes.POINTER(c_int), P, c_int64, P, P, P, P]),
+    "ctr_epoch_sweep2_supported": (c_int, [c_int, c_int64, c_int]),
+    "ctr_epoch_sweep2": (c_int, [c_int, P, P, P, P, P, P, P, c_int64, c_int, P, P, c_int, c_int, c_int, P, P,
+                                 ctypes.POINTER(c_int), P, c_int64, P, P, P, P, P]),
     "ctr_epoch_reg_loss": (c_int, [P, P, c_int, c_int, c_float, P, c_int, P]),
     "ctr_selftest_divsqrt": (c_int, [c_uint64, c_int64, P, P]),
     "ctr_selftest_adam_packed": (c_int, [c_int, c_uint64, c_int64, c_int, c_float, c_float, P, P]),

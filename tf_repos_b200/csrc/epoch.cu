@@ -24,10 +24,12 @@ namespace ctr {
 constexpr int EPOCH_MAX = 32;  // max steps per epoch (lr table / ss table size)
 
 // epoch_adam.cu: Adam sweep on the packed fp32 pipe (rows nothing gathered since `from`; the others go to `list`)
+// w_*: an optional scalar table [n_rows] that shares `last` and is swept in the same launch
 bool launch_epoch_sweep_adam(float* var, float* slot0, float* slot1, const uint8_t* last, int64_t n_rows, int K,
                              const float* hyper, const float* lr_table, int from, int upto, double* ss_partials,
                              int n_partials, int32_t* list, int32_t* list_count, int64_t list_cap,
-                             int32_t* list_overflow, int grid, cudaStream_t st);
+                             int32_t* list_overflow, int grid, cudaStream_t st, float* w_var = nullptr,
+                             float* w_slot0 = nullptr, float* w_slot1 = nullptr, double* w_ss_partials = nullptr);
 
 __device__ __forceinline__ float sq4(const float4& x) {
   return (x.x * x.x + x.y * x.y) + (x.z * x.z + x.w * x.w);
@@ -36,12 +38,23 @@ __device__ __forceinline__ float sq4(const float4& x) {
 // Rows uniq[0..n_uniq): replay the untouched-row step for steps last[row]..j-1 so that the stored
 // state is the state at the START of step j; then (APPLY) take step j with the summed gradient.
 // ss[s] (double) accumulates sum(var^2) of the state each replayed/applied step started from.
-// second scalar table gathered with the same ids (DeepFM: fm_w next to fm_v): lane 0 of a row carries its element
+// second scalar table gathered with the same ids (DeepFM: fm_w next to fm_v): lane 0 of a row carries its element.
+// last == nullptr: the two tables share the [N,K] table's `last` bytes (they are always gathered together)
+// stage / w_stage (STAGED): per unique row u, the state at the start of step j -- stage[u*3K ..] = var | slot0 | slot1
+// of the [N,K] row, w_stage[3u ..] = those of the scalar element
 struct RowsW {
   float* var; float* slot0; float* slot1; uint8_t* last; const float* g_uniq; double* ss;
+  float* stage = nullptr; float* w_stage = nullptr;
 };
 
-template <int OPT, int LPR, int VEC, bool APPLY, bool WITH_W = false>
+// STAGED (WITH_W only): the catch-up and the apply of one step hand the rows over through `stage`, in unique-row
+// order, instead of through the tables.  The catch-up (!APPLY) stores the caught-up state in `stage` and writes only
+// `var` back (the forward gathers it); slot0 / slot1 and `last` keep their old values until the apply (APPLY) of the
+// same step reads `stage`, takes step j and writes the whole row and last = j + 1.  Per row, that replaces two random
+// slot writes and a `last` write in the catch-up, and every random read of the apply, with sequential stage traffic.
+// Between the two calls the tables hold the caught-up `var` next to the old slots: nothing but the step's forward
+// may read them.
+template <int OPT, int LPR, int VEC, bool APPLY, bool WITH_W = false, bool STAGED = false>
 __global__ void __launch_bounds__(256)
 epoch_rows_kernel(float* __restrict__ var, float* __restrict__ slot0, float* __restrict__ slot1,
                   uint8_t* __restrict__ last, const int32_t* __restrict__ uniq,
@@ -60,21 +73,36 @@ epoch_rows_kernel(float* __restrict__ var, float* __restrict__ slot0, float* __r
   const bool active = u < n_max && u < n_uniq[0];
   Hyper h = load_hyper(hyper);
   const AdamConsts ac = adam_consts(h);
+  constexpr bool from_stage = STAGED && APPLY;
   const int64_t id = active ? uniq[u] : 0;
-  const int l0 = active ? last[id] : j;
+  const int l0 = (active && !from_stage) ? last[id] : j;
   const int64_t row = id * K;
+  float* const srow = STAGED ? w.stage + u * (3 * K) : nullptr;
   float4 x[VEC], a[VEC], b[VEC];
 #pragma unroll
   for (int v = 0; v < VEC; ++v) {
     const int64_t e = row + (c + v * LPR) * 4;
-    x[v] = active ? *reinterpret_cast<const float4*>(var + e) : f4_zero();
-    a[v] = active ? *reinterpret_cast<const float4*>(slot0 + e) : f4_zero();
-    b[v] = (active && two) ? *reinterpret_cast<const float4*>(slot1 + e) : f4_zero();
+    const int k = (c + v * LPR) * 4;
+    if (from_stage) {
+      x[v] = active ? *reinterpret_cast<const float4*>(srow + k) : f4_zero();
+      a[v] = active ? *reinterpret_cast<const float4*>(srow + K + k) : f4_zero();
+      b[v] = (active && two) ? *reinterpret_cast<const float4*>(srow + 2 * K + k) : f4_zero();
+    } else {
+      x[v] = active ? *reinterpret_cast<const float4*>(var + e) : f4_zero();
+      a[v] = active ? *reinterpret_cast<const float4*>(slot0 + e) : f4_zero();
+      b[v] = (active && two) ? *reinterpret_cast<const float4*>(slot1 + e) : f4_zero();
+    }
   }
   const bool wact = WITH_W && active && c == 0;
   int l0w = j;
   float xw = 0.f, aw = 0.f, bw = 0.f;
-  if (wact) { l0w = w.last[id]; xw = w.var[id]; aw = w.slot0[id]; bw = two ? w.slot1[id] : 0.f; }
+  if (wact) {
+    if (from_stage) {
+      xw = w.w_stage[3 * u]; aw = w.w_stage[3 * u + 1]; bw = two ? w.w_stage[3 * u + 2] : 0.f;
+    } else {
+      l0w = w.last ? w.last[id] : l0; xw = w.var[id]; aw = w.slot0[id]; bw = two ? w.slot1[id] : 0.f;
+    }
+  }
   // warp-uniform trip count (the body reduces across the warp); a lane joins at its own row's `last`
   const int lmin = __reduce_min_sync(FULL_MASK, min(l0, l0w));
 #pragma unroll 1
@@ -122,11 +150,34 @@ epoch_rows_kernel(float* __restrict__ var, float* __restrict__ slot0, float* __r
       if (lane == 0 && qw != 0.f) atomicAdd(&ssw_blk[j], qw);
     }
   }
+  if (STAGED && !APPLY) {   // hand the caught-up rows to the apply; only `var` goes back to the tables
+    if (active) {
+#pragma unroll
+      for (int v = 0; v < VEC; ++v) {
+        const int k = (c + v * LPR) * 4;
+        *reinterpret_cast<float4*>(srow + k) = x[v];
+        *reinterpret_cast<float4*>(srow + K + k) = a[v];
+        if (two) *reinterpret_cast<float4*>(srow + 2 * K + k) = b[v];
+        if (l0 < j) *reinterpret_cast<float4*>(var + row + k) = x[v];
+      }
+    }
+    if (wact) {
+      w.w_stage[3 * u] = xw; w.w_stage[3 * u + 1] = aw;
+      if (two) w.w_stage[3 * u + 2] = bw;
+      if (l0w < j) w.var[id] = xw;
+    }
+  }
+  if (STAGED && !APPLY) {
+    __syncthreads();
+    if (threadIdx.x < EPOCH_MAX && ss_blk[threadIdx.x] != 0.f) atomicAdd(&ss[threadIdx.x], (double)ss_blk[threadIdx.x]);
+    if (threadIdx.x < EPOCH_MAX && ssw_blk[threadIdx.x] != 0.f) atomicAdd(&w.ss[threadIdx.x], (double)ssw_blk[threadIdx.x]);
+    return;
+  }
   if (WITH_W && wact && (APPLY || l0w < j)) {
     w.var[id] = xw; w.slot0[id] = aw;
     if (two) w.slot1[id] = bw;
   }
-  if (WITH_W && wact && (APPLY || l0w < j || set_last >= 0)) w.last[id] = (uint8_t)(set_last >= 0 ? set_last : (APPLY ? j + 1 : j));
+  if (WITH_W && wact && w.last && (APPLY || l0w < j || set_last >= 0)) w.last[id] = (uint8_t)(set_last >= 0 ? set_last : (APPLY ? j + 1 : j));
   const bool wrote = active && (APPLY || l0 < j);
   const uint8_t new_last = (uint8_t)(set_last >= 0 ? set_last : (APPLY ? j + 1 : j));
   if (wrote) {
@@ -600,24 +651,19 @@ int ctr_epoch_rows(int opt, int apply, float* var, float* slot0, float* slot1, u
 
 // The [N,K] table and a scalar table [N] gathered with the same ids (fm_v + fm_w), in ONE launch: lane 0 of every row
 // carries the scalar table's element.  Same arithmetic as two ctr_epoch_rows calls.
-int ctr_epoch_rows2(int opt, int apply, float* var, float* slot0, float* slot1, uint8_t* last, float* w_var, float* w_slot0,
-                    float* w_slot1, uint8_t* w_last, const int32_t* uniq, const int32_t* n_uniq, const float* g_uniq,
-                    const float* gw_uniq, int64_t n_max, int K, const float* hyper, const float* lr_table, int j, double* ss,
-                    double* ss_w, ctr_stream_t stream) {
-  CTR_REQUIRE(n_max >= 0 && j >= 0 && j < EPOCH_MAX, CTR_ERR_INVALID_ARG, "ctr_epoch_rows2: bad n_max/j");
-  CTR_REQUIRE(epoch_rows2_supported(K), CTR_ERR_UNSUPPORTED, "ctr_epoch_rows2: K=%d (supported: 4..256 powers of two)", K);
-  if (n_max == 0) return CTR_OK;
-  CTR_REQUIRE(var && slot0 && last && w_var && w_slot0 && w_last && uniq && n_uniq && hyper && lr_table && ss && ss_w,
-              CTR_ERR_INVALID_ARG, "ctr_epoch_rows2: null buffer");
-  CTR_REQUIRE(!apply || (g_uniq && gw_uniq), CTR_ERR_INVALID_ARG, "ctr_epoch_rows2: gradients required when apply != 0");
-  CTR_REQUIRE(n_slots_of(opt) == 1 || (slot1 && w_slot1), CTR_ERR_INVALID_ARG, "ctr_epoch_rows2: slot1 required");
-  cudaStream_t st = as_stream(stream);
-  RowsW w;
-  w.var = w_var; w.slot0 = w_slot0; w.slot1 = w_slot1; w.last = w_last; w.g_uniq = gw_uniq; w.ss = ss_w;
+static int launch_epoch_rows2(int opt, int apply, float* var, float* slot0, float* slot1, uint8_t* last,
+                              const RowsW& w, const int32_t* uniq, const int32_t* n_uniq, const float* g_uniq,
+                              int64_t n_max, int K, const float* hyper, const float* lr_table, int j, double* ss,
+                              int set_last, cudaStream_t st) {
+  const bool staged = w.stage != nullptr;
 #define ER2_K(OPT, AP, KK, LPR, VEC)                                                                       \
   case KK:                                                                                                 \
-    epoch_rows_kernel<OPT, LPR, VEC, AP, true><<<(unsigned)ceil_div64(n_max * LPR, 256), 256, 0, st>>>(    \
-        var, slot0, slot1, last, uniq, n_uniq, g_uniq, n_max, hyper, lr_table, j, ss, -1, w);              \
+    if (staged)                                                                                            \
+      epoch_rows_kernel<OPT, LPR, VEC, AP, true, true><<<(unsigned)ceil_div64(n_max * LPR, 256), 256, 0, st>>>( \
+          var, slot0, slot1, last, uniq, n_uniq, g_uniq, n_max, hyper, lr_table, j, ss, set_last, w);      \
+    else                                                                                                   \
+      epoch_rows_kernel<OPT, LPR, VEC, AP, true><<<(unsigned)ceil_div64(n_max * LPR, 256), 256, 0, st>>>(  \
+          var, slot0, slot1, last, uniq, n_uniq, g_uniq, n_max, hyper, lr_table, j, ss, set_last, w);      \
     break;
 #define ER2_AP(OPT, AP)                                                                                    \
   switch (K) {                                                                                             \
@@ -633,6 +679,111 @@ int ctr_epoch_rows2(int opt, int apply, float* var, float* slot0, float* slot1, 
   return CTR_OK;
 }
 
+// The [N,K] table and a scalar table [N] gathered with the same ids (fm_v + fm_w), in ONE launch: lane 0 of every row
+// carries the scalar table's element.  Same arithmetic as two ctr_epoch_rows calls.  w_last == last: the tables share
+// one `last` byte per row (ctr_epoch_sweep2).
+static int epoch_rows2_checked(int opt, int apply, float* var, float* slot0, float* slot1, uint8_t* last, float* w_var,
+                               float* w_slot0, float* w_slot1, uint8_t* w_last, const int32_t* uniq,
+                               const int32_t* n_uniq, const float* g_uniq, const float* gw_uniq, int64_t n_max, int K,
+                               const float* hyper, const float* lr_table, int j, double* ss, double* ss_w,
+                               float* stage, float* w_stage, ctr_stream_t stream) {
+  CTR_REQUIRE(n_max >= 0 && j >= 0 && j < EPOCH_MAX, CTR_ERR_INVALID_ARG, "ctr_epoch_rows2: bad n_max/j");
+  CTR_REQUIRE(epoch_rows2_supported(K), CTR_ERR_UNSUPPORTED, "ctr_epoch_rows2: K=%d (supported: 4..256 powers of two)", K);
+  if (n_max == 0) return CTR_OK;
+  CTR_REQUIRE(var && slot0 && last && w_var && w_slot0 && w_last && uniq && n_uniq && hyper && lr_table && ss && ss_w,
+              CTR_ERR_INVALID_ARG, "ctr_epoch_rows2: null buffer");
+  CTR_REQUIRE(!apply || (g_uniq && gw_uniq), CTR_ERR_INVALID_ARG, "ctr_epoch_rows2: gradients required when apply != 0");
+  CTR_REQUIRE(n_slots_of(opt) == 1 || (slot1 && w_slot1), CTR_ERR_INVALID_ARG, "ctr_epoch_rows2: slot1 required");
+  RowsW w;
+  w.var = w_var; w.slot0 = w_slot0; w.slot1 = w_slot1; w.last = (w_last == last) ? nullptr : w_last; w.g_uniq = gw_uniq;
+  w.ss = ss_w; w.stage = stage; w.w_stage = w_stage;
+  return launch_epoch_rows2(opt, apply, var, slot0, slot1, last, w, uniq, n_uniq, g_uniq, n_max, K, hyper, lr_table, j,
+                            ss, -1, as_stream(stream));
+}
+
+// The [N,K] table and a scalar table [N] gathered with the same ids (fm_v + fm_w), in ONE launch: lane 0 of every row
+// carries the scalar table's element.  Same arithmetic as two ctr_epoch_rows calls.  w_last == last: the tables share
+// one `last` byte per row (ctr_epoch_sweep2).
+int ctr_epoch_rows2(int opt, int apply, float* var, float* slot0, float* slot1, uint8_t* last, float* w_var, float* w_slot0,
+                    float* w_slot1, uint8_t* w_last, const int32_t* uniq, const int32_t* n_uniq, const float* g_uniq,
+                    const float* gw_uniq, int64_t n_max, int K, const float* hyper, const float* lr_table, int j, double* ss,
+                    double* ss_w, ctr_stream_t stream) {
+  return epoch_rows2_checked(opt, apply, var, slot0, slot1, last, w_var, w_slot0, w_slot1, w_last, uniq, n_uniq, g_uniq,
+                             gw_uniq, n_max, K, hyper, lr_table, j, ss, ss_w, nullptr, nullptr, stream);
+}
+
+int ctr_epoch_rows2_staged(int opt, int apply, float* var, float* slot0, float* slot1, uint8_t* last, float* w_var,
+                           float* w_slot0, float* w_slot1, uint8_t* w_last, const int32_t* uniq, const int32_t* n_uniq,
+                           const float* g_uniq, const float* gw_uniq, int64_t n_max, int K, const float* hyper,
+                           const float* lr_table, int j, double* ss, double* ss_w, float* stage, float* w_stage,
+                           ctr_stream_t stream) {
+  CTR_REQUIRE(stage && w_stage, CTR_ERR_INVALID_ARG, "ctr_epoch_rows2_staged: null stage");
+  return epoch_rows2_checked(opt, apply, var, slot0, slot1, last, w_var, w_slot0, w_slot1, w_last, uniq, n_uniq, g_uniq,
+                             gw_uniq, n_max, K, hyper, lr_table, j, ss, ss_w, stage, w_stage, stream);
+}
+
+// CTR_EPOCH_SCALAR=1 (read once per process) routes Adam through the scalar sweep kernels (A/B against the packed one)
+static bool epoch_force_scalar() {
+  static int force = -1;
+  if (force < 0) {
+    const char* f = getenv("CTR_EPOCH_SCALAR");
+    force = f ? atoi(f) : 0;
+  }
+  return force != 0;
+}
+
+int ctr_epoch_sweep2_supported(int opt, int64_t n_rows, int K) {
+  return opt == CTR_OPT_ADAM && !epoch_force_scalar() && epoch_rows2_supported(K) && n_rows > 0 && n_rows % 4 == 0;
+}
+
+int ctr_epoch_sweep2(int opt, float* var, float* slot0, float* slot1, float* w_var, float* w_slot0, float* w_slot1,
+                     uint8_t* last, int64_t n_rows, int K, const float* hyper, const float* lr_table, int from, int upto,
+                     int reset, double* ss_partials, double* w_ss_partials, int* n_partials_host, int32_t* list,
+                     int64_t list_cap, int32_t* list_count, double* ss_rows, double* w_ss_rows, int32_t* list_overflow,
+                     ctr_stream_t stream) {
+  CTR_REQUIRE(n_rows >= 0 && from >= 0 && from <= upto && upto <= EPOCH_MAX, CTR_ERR_INVALID_ARG,
+              "ctr_epoch_sweep2: bad n_rows/from/upto");
+  CTR_REQUIRE(ctr_epoch_sweep2_supported(opt, n_rows, K), CTR_ERR_UNSUPPORTED,
+              "ctr_epoch_sweep2: needs Adam, K in {4..256} powers of two, n_rows %% 4 == 0 and the packed sweep "
+              "(K=%d, n_rows=%lld)", K, (long long)n_rows);
+  const int n_partials = sm_count() * 6;
+  if (n_partials_host) *n_partials_host = n_partials;
+  if (upto == 0) return CTR_OK;
+  CTR_REQUIRE(var && slot0 && slot1 && w_var && w_slot0 && w_slot1 && last && hyper && lr_table && ss_partials &&
+              w_ss_partials && list && list_count && ss_rows && w_ss_rows && list_cap > 0, CTR_ERR_INVALID_ARG,
+              "ctr_epoch_sweep2: null buffer");
+  CTR_REQUIRE(((uintptr_t)last & 3) == 0, CTR_ERR_INVALID_ARG, "ctr_epoch_sweep2: `last` must be 4-byte aligned");
+  cudaStream_t st = as_stream(stream);
+  if (from == upto) {   // nothing to replay (a flush reached upto already): no step's partials, `last` -> 0 on reset
+    const size_t bytes = (size_t)upto * n_partials * sizeof(double);
+    CTR_REQUIRE(cudaMemsetAsync(ss_partials, 0, bytes, st) == cudaSuccess &&
+                cudaMemsetAsync(w_ss_partials, 0, bytes, st) == cudaSuccess, CTR_ERR_CUDA, "ctr_epoch_sweep2: memset failed");
+    if (reset) {
+      epoch_last_kernel<<<sm_count() * 3, 256, 0, st>>>(last, n_rows, upto, reset);
+      CTR_LAUNCHED("ctr_epoch_sweep2(last)");
+    }
+    return CTR_OK;
+  }
+  CTR_REQUIRE(cudaMemsetAsync(list_count, 0, sizeof(int32_t), st) == cudaSuccess, CTR_ERR_CUDA,
+              "ctr_epoch_sweep2: memset failed");
+  const bool ok = launch_epoch_sweep_adam(var, slot0, slot1, last, n_rows, K, hyper, lr_table, from, upto, ss_partials,
+                                          n_partials, list, list_count, list_cap, list_overflow, 0, st, w_var, w_slot0,
+                                          w_slot1, w_ss_partials);
+  CTR_REQUIRE(ok, CTR_ERR_UNSUPPORTED, "ctr_epoch_sweep2: packed path refused K=%d", K);
+  CTR_LAUNCHED("ctr_epoch_sweep2(adam)");
+  // rows gathered since `from`, both tables: catch up from their own `last` to upto; they get their final `last` here
+  RowsW w;
+  w.var = w_var; w.slot0 = w_slot0; w.slot1 = w_slot1; w.last = nullptr; w.g_uniq = nullptr; w.ss = w_ss_rows;
+  const int rc = launch_epoch_rows2(opt, 0, var, slot0, slot1, last, w, list, list_count, nullptr, list_cap, K, hyper,
+                                    lr_table, upto, ss_rows, reset ? 0 : upto, st);
+  if (rc != CTR_OK) return rc;
+  if (!(reset && from == 0)) {   // untouched rows hold `from`: rewrite (an epoch-end sweep leaves their 0 alone)
+    epoch_last_kernel<<<sm_count() * 3, 256, 0, st>>>(last, n_rows, upto, reset);
+    CTR_LAUNCHED("ctr_epoch_sweep2(last)");
+  }
+  return CTR_OK;
+}
+
 int ctr_epoch_sweep_ovf(int opt, float* var, float* slot0, float* slot1, uint8_t* last, int64_t n_rows, int K,
                         const float* hyper, const float* lr_table, int from, int upto, int reset, double* ss_partials,
                         int* n_partials_host, int32_t* list, int64_t list_cap, int32_t* list_count, double* ss_rows,
@@ -641,14 +792,13 @@ int ctr_epoch_sweep_ovf(int opt, float* var, float* slot0, float* slot1, uint8_t
               "ctr_epoch_sweep: bad n_rows/K/from/upto");
   // tuning hook (tools/tune_epoch.py): CTR_EPOCH_CFG selects (unroll, CTAs/SM) of the scalar K%4==0 kernel;
   // CTR_EPOCH_SCALAR=1 routes Adam through the scalar kernels as well (A/B against the packed sweep)
-  static int cfg = -1, force_scalar = 0;
+  static int cfg = -1;
   if (cfg < 0) {
     const char* e = getenv("CTR_EPOCH_CFG");
     cfg = e ? atoi(e) : 4;
     if (cfg < 0 || cfg > 7) cfg = 4;
-    const char* f = getenv("CTR_EPOCH_SCALAR");
-    force_scalar = f ? atoi(f) : 0;
   }
+  const bool force_scalar = epoch_force_scalar();
   static const int kBlocksPerSm[8] = {3, 4, 2, 6, 3, 2, 6, 4};
   const int grid = sm_count() * 3;
   const int n_partials = sm_count() * 6;     // row length of ss_partials (>= every grid used here)

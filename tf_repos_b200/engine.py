@@ -204,7 +204,9 @@ class SparseUpdater:
 
     # ---- exact-deferred ("epoch") mode: csrc/epoch.cu ------------------------------------------------
     def enable_epochs(self, P: int, tables: Sequence[Table]):
-        """Allocates the per-row `last` bytes and the per-step sum(var^2) accumulators."""
+        """Allocates the per-row `last` bytes and the per-step sum(var^2) accumulators.  An [N,K] table and the [N]
+        table gathered with the same ids always hold the same `last` bytes: where the packed Adam sweep can take both
+        in one pass (ops.epoch_sweep2_supported) they share ONE `last` array and one row list."""
         pmax = ops.epoch_max_steps()
         if not 1 <= P <= pmax:
             raise ValueError(f"epoch_steps={P}: must be in [1, {pmax}] (the `last` bytes and lr table hold {pmax} steps)")
@@ -215,10 +217,13 @@ class SparseUpdater:
         self.ep = {}
         # rows the packed Adam sweep found but could not list (a list smaller than include/ctr_b200.h's bound)
         self.list_overflow = torch.zeros(1, dtype=torch.int32, device=dev)
-        for t in tables:
+        self.shared_last = (len(tables) == 2 and tables[1].K == 1 and tables[0].N == tables[1].N
+                            and tables[0].K in ops.EPOCH_ROWS2_K
+                            and ops.epoch_sweep2_supported(self.opt.opt, tables[0].N, tables[0].K))
+        for i, t in enumerate(tables):
             # rows gathered since the last sweep, collected by the packed Adam sweep for its second pass: at most
-            # n distinct ids per step, P <= pmax steps per epoch
-            cap = max(min(self.n * pmax, t.N), 1)
+            # n distinct ids per step, P <= pmax steps per epoch (shared: the [N,K] table's list serves both)
+            cap = 1 if (self.shared_last and i == 1) else max(min(self.n * pmax, t.N), 1)
             self.ep[t.name] = dict(
                 list=torch.empty(cap, dtype=torch.int32, device=dev),
                 list_count=torch.zeros(1, dtype=torch.int32, device=dev),
@@ -226,6 +231,9 @@ class SparseUpdater:
                 ss=torch.zeros(pmax, dtype=torch.float64, device=dev),
                 partials=torch.zeros(pmax * self.n_epart, dtype=torch.float64, device=dev),
                 reg=torch.zeros(pmax, dtype=torch.float32, device=dev))
+        if self.shared_last:
+            ev = self.ep[tables[0].name]
+            self.ep[tables[1].name].update(last=ev["last"], list=ev["list"], list_count=ev["list_count"])
 
     def epoch_rows(self, tables_g, j: int, apply: bool):
         """tables_g: [(Table, g_uniq or None)].  apply=False: catch the gathered rows up to the start of
@@ -235,8 +243,11 @@ class SparseUpdater:
                 and tables_g[0][0].N == tables_g[1][0].N):
             (V, gv), (W, gw) = tables_g            # fm_v + fm_w: one launch for both tables
             ev, ew = self.ep[V.name], self.ep[W.name]
-            ops.epoch_rows2(o.opt, apply, V, W, ev["last"], ew["last"], uw.uniq, uw.n_uniq, gv if apply else None,
-                            gw if apply else None, self.n, o.record(HYPER_TABLE), o.lr_table, j, ev["ss"], ew["ss"])
+            # the catch-up hands the caught-up rows to the apply of the same step through stage_v / stage_w (free in
+            # this mode; see ctr_epoch_rows2_staged)
+            ops.epoch_rows2_staged(o.opt, apply, V, W, ev["last"], ew["last"], uw.uniq, uw.n_uniq,
+                                   gv if apply else None, gw if apply else None, self.n, o.record(HYPER_TABLE),
+                                   o.lr_table, j, ev["ss"], ew["ss"], self.stage_v, self.stage_w)
             return
         for t, g in tables_g:
             e = self.ep[t.name]
@@ -246,6 +257,9 @@ class SparseUpdater:
     def epoch_sweep(self, upto: int, reset: bool):
         """All rows -> state after `upto` steps of this epoch; per-step l2*l2_loss terms -> ep[.]['reg']."""
         o = self.opt
+        if self.shared_last:
+            self.epoch_sweep2(upto, reset)
+            return
         for t in self.tables:
             e = self.ep[t.name]
             ev = None
@@ -260,6 +274,25 @@ class SparseUpdater:
                 self.sweep_events.append(ev)
                 self.sweep_steps.append(upto - self.flush_pos)   # optimizer steps this pass replayed per element
             # accumulate: a mid-epoch flush and the epoch-end sweep each contribute their share
+            ops.epoch_reg_loss(e["ss"], e["partials"], self.n_epart, upto, 0.5 * self.l2_reg, e["reg"], accumulate=True)
+        self.flush_pos = 0 if reset else upto
+
+    def epoch_sweep2(self, upto: int, reset: bool):
+        """epoch_sweep for an [N,K] + [N] pair that shares `last`: one pass and one row list for both tables."""
+        o = self.opt
+        (V, W), (ev, ew) = self.tables, (self.ep[self.tables[0].name], self.ep[self.tables[1].name])
+        rec = None
+        if self.sweep_events is not None:
+            rec = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+            rec[0].record()
+        ops.epoch_sweep2(o.opt, V, W, ev["last"], o.record(HYPER_TABLE), o.lr_table, self.flush_pos, upto, reset,
+                         ev["partials"], ew["partials"], ev["list"], ev["list_count"], ev["ss"], ew["ss"],
+                         self.list_overflow)
+        if rec is not None:
+            rec[1].record()
+            self.sweep_events.append(rec)
+            self.sweep_steps.append(upto - self.flush_pos)
+        for e in (ev, ew):
             ops.epoch_reg_loss(e["ss"], e["partials"], self.n_epart, upto, 0.5 * self.l2_reg, e["reg"], accumulate=True)
         self.flush_pos = 0 if reset else upto
 

@@ -512,6 +512,22 @@ def epoch_rows2(opt, apply: bool, V, W, last_v, last_w, uniq, n_uniq, g_uniq, gw
         "ctr_epoch_rows2")
 
 
+def epoch_rows2_staged(opt, apply: bool, V, W, last_v, last_w, uniq, n_uniq, g_uniq, gw_uniq, n_max, hyper, lr_table, j,
+                       ss_v, ss_w, stage_v, stage_w):
+    """epoch_rows2 whose catch-up and apply of one step hand the rows over through stage_v [n_max*3K] / stage_w
+    [n_max*3] (ctr_epoch_rows2_staged)."""
+    f = torch.float32
+    check(
+        _L.ctr_epoch_rows2_staged(
+            opt, int(apply), _p(V.var, f, "var"), _p(V.slot(0), f), _p(V.slot(1), f), _p(last_v, torch.uint8, "last"),
+            _p(W.var, f, "w_var"), _p(W.slot(0), f), _p(W.slot(1), f), _p(last_w, torch.uint8, "w_last"),
+            _p(uniq, torch.int32, "uniq"), _p(n_uniq, torch.int32, "n_uniq"), _p(g_uniq, f, "g_uniq"),
+            _p(gw_uniq, f, "gw_uniq"), n_max, V.K, _p(hyper, f, "hyper"), _p(lr_table, f, "lr_table"), j,
+            _p(ss_v, torch.float64, "ss"), _p(ss_w, torch.float64, "ss_w"), _p(stage_v, f, "stage"),
+            _p(stage_w, f, "w_stage"), _stream()),
+        "ctr_epoch_rows2_staged")
+
+
 EPOCH_ROWS2_K = (4, 8, 16, 32, 64, 128, 256)
 
 
@@ -534,6 +550,29 @@ def epoch_sweep(opt, var, slot0, slot1, last, n_rows, K, hyper, lr_table, from_:
             _p(list_count, torch.int32, "list_count"), _p(ss_rows, torch.float64, "ss_rows"),
             _p(list_overflow, torch.int32, "list_overflow"), _stream()),
         "ctr_epoch_sweep_ovf")
+    return n_part.value
+
+
+def epoch_sweep2_supported(opt, n_rows: int, K: int) -> bool:
+    """Whether an [n_rows, K] table and a scalar [n_rows] table can share one `last` array (ctr_epoch_sweep2)."""
+    return bool(_L.ctr_epoch_sweep2_supported(opt, n_rows, K))
+
+
+def epoch_sweep2(opt, V, W, last, hyper, lr_table, from_: int, upto: int, reset: bool, ss_partials, w_ss_partials,
+                 list_buf, list_count, ss_rows, w_ss_rows, list_overflow=None):
+    """ctr_epoch_sweep2: V [N,K] and W [N] (engine.Table) sharing `last`, one pass and one row list for both."""
+    f = torch.float32
+    n_part = ctypes.c_int(0)
+    check(
+        _L.ctr_epoch_sweep2(
+            opt, _p(V.var, f, "var"), _p(V.slot(0), f, "slot0"), _p(V.slot(1), f, "slot1"), _p(W.var, f, "w_var"),
+            _p(W.slot(0), f, "w_slot0"), _p(W.slot(1), f, "w_slot1"), _p(last, torch.uint8, "last"), V.N, V.K,
+            _p(hyper, f, "hyper"), _p(lr_table, f, "lr_table"), from_, upto, int(reset),
+            _p(ss_partials, torch.float64, "ss_partials"), _p(w_ss_partials, torch.float64, "w_ss_partials"),
+            ctypes.byref(n_part), _p(list_buf, torch.int32, "list"), list_buf.numel(),
+            _p(list_count, torch.int32, "list_count"), _p(ss_rows, torch.float64, "ss_rows"),
+            _p(w_ss_rows, torch.float64, "w_ss_rows"), _p(list_overflow, torch.int32, "list_overflow"), _stream()),
+        "ctr_epoch_sweep2")
     return n_part.value
 
 
