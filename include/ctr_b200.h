@@ -452,6 +452,24 @@ int ctr_wd_input_fwd(const int32_t* ids, const float* dense, const float* emb, c
 int ctr_wd_input_bwd(const float* dX, const float* dy, const float* dense, int B, int Fc, int Fd, int K, float* g_rows,
                      float* g_cat, float* g_num, float* g_bias, ctr_stream_t stream);
 
+/* ---- wide_n_deep serving input (wide_n_deep.py:233-242, wide_n_deep_serving_client.cpp:45-62; DESIGN.md §2.8) -----
+ * The export's serving_default parses the request's `inputs` tensor -- n serialized tf.Examples -- with
+ * make_parse_example_spec(columns): I1..I13 FixedLenFeature([1], float32) without default, C14..C39
+ * VarLenFeature(int64), other keys ignored, the last map entry of a key wins.  Example b is data[offsets[b],
+ * offsets[b+1]) (device bytes, offsets int64 [n+1], each Example < 2^31 bytes).  One warp per Example parses it
+ * (packed and unpacked lists) and writes what ctr_wd_input_fwd writes with Fc = 26, Fd = 13:
+ *   x   [n, 26*K + 13] = [mean of the bag's emb rows per column C14..C39 (zero row for an empty or missing bag) |
+ *                         I values in num_perm order]                                            (emb != NULL)
+ *   lin [n] = sum of the bags' wide_cat weights + sum_j I(j+1)*wide_num[j] + wide_bias           (wide_* != NULL)
+ * An int64 value outside [0, NB) (all 64 bits) becomes 0.  With one value per C key, x and lin are bit-identical to
+ * ctr_wd_input_fwd.  err (device uint64, set to ~0 by the caller) is min-folded with (example_base + b) << 16 |
+ * check << 8 | key; check 1 = malformed protobuf (key 0), 2 = I key missing, 3 = several kinds in one Feature or a
+ * wrong kind (not FloatList under I, not Int64List under C), 4 = I key without exactly one value; key 0..12 = I1..I13,
+ * 13..38 = C14..C39.  The rows of a rejected Example are not written. */
+int ctr_wd_serve_input(const void* data, const int64_t* offsets, int64_t n, int64_t example_base, const float* emb,
+                       const float* wide_cat, const float* wide_num, const float* wide_bias, const int32_t* num_perm,
+                       int NB, int K, float* x, float* lin, uint64_t* err, ctr_stream_t stream);
+
 /* ---- libsvm input (HOST buffers) -------------------------------------------------------------------
  * decode_libsvm of input_fn (DeepFM.py:65-81): "<label> <id>:<val> ..." lines -> ids int32 [rows,F],
  * vals f32 [rows,F], labels f32 [rows].  Parses complete lines of buf_host[0,len) up to max_rows;

@@ -111,6 +111,7 @@ SIGNATURES = {
     "ctr_gather_scalar": (c_int, [P, P, c_int64, c_int64, P, P]),
     "ctr_wd_input_fwd": (c_int, [P, P, P, P, P, P, P, c_int, c_int, c_int, c_int, c_int, P, P, P, P]),
     "ctr_wd_input_bwd": (c_int, [P, P, P, c_int, c_int, c_int, c_int, P, P, P, P, P]),
+    "ctr_wd_serve_input": (c_int, [P, P, c_int64, c_int64, P, P, P, P, P, c_int, c_int, P, P, P, P]),
     "ctr_parse_libsvm": (c_int64, [c_char_p, c_size_t, c_int, c_int64, c_int, P, P, P, ctypes.POINTER(c_size_t)]),
     "ctr_libsvm_count_fields": (c_int, [c_char_p, c_size_t]),
     "ctr_parse_libsvm_device_workspace_bytes": (c_size_t, [c_size_t, c_int64]),

@@ -642,6 +642,18 @@ def wd_input_bwd(dX, dy, dense, B, Fc, Fd, K, g_rows, g_cat, g_num, g_bias):
           "ctr_wd_input_bwd")
 
 
+def wd_serve_input(data, offsets, example_base: int, emb, wide_cat, wide_num, wide_bias, num_perm, NB, K, x, lin, err):
+    """Serialized tf.Examples data[offsets[b], offsets[b+1]) (uint8, offsets int64 [n+1]) -> x [n, 26K+13] and lin [n]
+    as wd_input_fwd writes them; err int64 [1] (uint64 bits, ~0 = none) is min-folded."""
+    n = offsets.numel() - 1
+    check(_L.ctr_wd_serve_input(_p(data, torch.uint8, "data"), _p(offsets, torch.int64, "offsets"), n, example_base,
+                                _p(emb, torch.float32, "emb"), _p(wide_cat, torch.float32, "wide_cat"),
+                                _p(wide_num, torch.float32, "wide_num"), _p(wide_bias, torch.float32, "wide_bias"),
+                                _p(num_perm, torch.int32, "num_perm"), NB, K, _p(x, torch.float32, "x"),
+                                _p(lin, torch.float32, "lin"), _p(err, torch.int64, "err"), _stream()),
+          "ctr_wd_serve_input")
+
+
 def parse_libsvm_device(text: torch.Tensor, F: int, max_rows: int, final_chunk: bool = True):
     """decode_libsvm (DeepFM.py:65-81) on a uint8 CUDA tensor of text.  Returns (ids int32 [rows,F], vals f32 [rows,F],
     labels f32 [rows], consumed bytes, needs_host) -- when needs_host is True the chunk holds something only the host

@@ -8,6 +8,13 @@
 
 No training state is created (update_mode='lazy': no `last` bytes, no sweeps); requests larger than the configured
 batch are served in slices.  The gather kernel reads int64 ids directly (ctr_fm_embed_fwd id_bits = 64).
+
+wide_n_deep's export (`--task_type=export_model`, `<servable_model_dir>/saved_model.pt`) answers the other client,
+`Serving_pipeline/wide_n_deep_serving_client.cpp:45-62`: its `inputs` tensor is a batch of serialized tf.Examples
+(export definition wide_n_deep.py:233-242, DESIGN.md §2.8), and the output is the classification signature.
+
+    s = Servable.load("./servable")
+    out = s.classify([example_bytes, ...])       # {"scores": float32 [n,2] = [1-p, p], "classes": [n,2] b"0", b"1"}
 """
 from __future__ import annotations
 
@@ -45,13 +52,94 @@ def _build(model_name: str, p: Dict, batch_size: int, device):
     raise ValueError(f"unknown exported model {model_name!r}")
 
 
+_WD_KEYS = ["I%d" % i for i in range(1, 14)] + ["C%d" % i for i in range(14, 40)]
+_WD_CHECKS = {1: "malformed tf.Example protobuf", 2: "required key {key!r} is missing",
+              3: "key {key!r} holds several kinds or the wrong kind (I*: FloatList, C*: Int64List)",
+              4: "key {key!r} must hold exactly one float"}
+
+
+class WideDeepServable:
+    """serving_default of an exported wide_n_deep: serialized tf.Examples in, the binary head's classification out.
+    Per request: one pinned host->device copy (error word, offsets and bytes), the parse + feature-column kernel and
+    the MLP per slice of at most max_batch Examples, one device->host copy (probabilities and error word)."""
+
+    def __init__(self, model):
+        self.model = model
+        self._host = self._dev = None
+
+    @classmethod
+    def load(cls, export_dir: str, max_batch: int = 4096, device="cuda") -> "WideDeepServable":
+        from .wide_deep import WideDeep
+        st = torch.load(os.path.join(export_dir, "saved_model.pt"), map_location="cpu")
+        v = st["variables"]
+        emb = v.get("dnn/input_from_feature_columns/input_layer/C14_embedding/embedding_weights")
+        layers, i = [], 0
+        while f"dnn/hiddenlayer_{i}/kernel" in v:
+            layers.append(int(v[f"dnn/hiddenlayer_{i}/kernel"].shape[1]))
+            i += 1
+        model = WideDeep(int(emb.shape[1]) if emb is not None else 1, max_batch, layers, st["model_type"], device=device)
+        model.load_variables(v)
+        return cls(model)
+
+    def _buffers(self, nbytes: int):
+        if self._host is None or self._host.numel() < nbytes:
+            cap = max(nbytes, 1 << 16)
+            self._host = torch.empty(cap, dtype=torch.uint8, pin_memory=True)
+            self._dev = torch.empty(cap, dtype=torch.uint8, device=self.model.device)
+        return self._host, self._dev
+
+    def classify(self, examples) -> Dict[str, np.ndarray]:
+        """examples: the string_vals of the request's `inputs` tensor (a sequence of bytes).  Raises ValueError naming
+        the first rejected Example (its index in the whole request) and the key."""
+        n = len(examples)
+        if n == 0:
+            return {"scores": np.zeros((0, 2), dtype=np.float32), "classes": np.zeros((0, 2), dtype="S1")}
+        lens = np.fromiter(map(len, examples), dtype=np.int64, count=n)
+        offsets = np.zeros(n + 1, dtype=np.int64)
+        np.cumsum(lens, out=offsets[1:])
+        if int(lens.max()) >= 1 << 31:
+            raise ValueError(f"example {int(np.argmax(lens >= 1 << 31))}: an Example of 2^31 bytes or more")
+        # device layout: prob f32 [n] (padded to 8 bytes) | err | offsets [n+1] | bytes; the first copy fills
+        # err..bytes, the last reads prob..err back
+        p_bytes = (4 * n + 7) & ~7
+        head = 8 + 8 * (n + 1)
+        total = p_bytes + head + int(offsets[-1])
+        host, dev = self._buffers(total)
+        h = host.numpy()
+        h[p_bytes:p_bytes + 8].view(np.int64)[0] = -1
+        h[p_bytes + 8:p_bytes + head].view(np.int64)[:] = offsets
+        h[p_bytes + head:total] = np.frombuffer(b"".join(examples), dtype=np.uint8)
+        dev[p_bytes:total].copy_(host[p_bytes:total], non_blocking=True)
+        pred = dev[:4 * n].view(torch.float32)
+        err = dev[p_bytes:p_bytes + 8].view(torch.int64)
+        off = dev[p_bytes + 8:p_bytes + head].view(torch.int64)
+        data = dev[p_bytes + head:total]
+        B = self.model.B
+        for lo in range(0, n, B):
+            hi = min(lo + B, n)
+            self.model.predict_examples(data, off[lo:hi + 1], err, pred[lo:hi], example_base=lo)
+        host[:p_bytes + 8].copy_(dev[:p_bytes + 8], non_blocking=True)
+        torch.cuda.current_stream(self.model.device).synchronize()
+        word = int(h[p_bytes:p_bytes + 8].view(np.int64)[0])
+        if word != -1:
+            ex, check, key = word >> 16, (word >> 8) & 0xFF, word & 0xFF
+            raise ValueError(f"example {ex}: " + _WD_CHECKS[check].format(key=_WD_KEYS[key]))
+        p = h[:4 * n].view(np.float32).copy()
+        return {"scores": np.stack([np.float32(1) - p, p], axis=1),
+                "classes": np.tile(np.array([b"0", b"1"], dtype="S1"), (n, 1))}
+
+
 class Servable:
     def __init__(self, model, signature: Dict):
         self.model, self.signature = model, signature
         self.F = int(signature["inputs"]["feat_ids"]["shape"][1])
 
     @classmethod
-    def load(cls, export_dir: str, max_batch: int = 4096, device="cuda") -> "Servable":
+    def load(cls, export_dir: str, max_batch: int = 4096, device="cuda"):
+        """the directory `--task_type=export` writes (DeepFM family) -> Servable; the one wide_n_deep's
+        `--task_type=export_model` writes (saved_model.pt) -> WideDeepServable"""
+        if os.path.exists(os.path.join(export_dir, "saved_model.pt")):
+            return WideDeepServable.load(export_dir, max_batch, device)
         sig = json.load(open(os.path.join(export_dir, "signature.json")))
         model = _build(sig["model"], sig["params"], max_batch, torch.device(device))
         model.load_variables(torch.load(os.path.join(export_dir, "variables.pt"), map_location="cpu"))

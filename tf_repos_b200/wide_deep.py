@@ -103,18 +103,40 @@ class WideDeep:
                          self.dense_lin["linear/linear_model/bias_weights"] if self.has_linear else None,
                          self.num_perm, NUM_BUCKETS, self.K, self.flat_ids[: B * N_CAT],
                          self.x[:B] if self.has_dnn else None, lin)
-        y_d = None
-        if self.has_dnn:
-            self._a = self.mlp.forward_hidden(self.x[:B], self.dense_dnn, train=False)
-            y_d = self.mlp.forward_out(self._a, self.dense_dnn)
-        return lin, y_d
+        return lin, self._dnn(B)
+
+    def _dnn(self, B: int):
+        """the DNN logits of x[:B], or None for the linear model"""
+        if not self.has_dnn:
+            return None
+        self._a = self.mlp.forward_hidden(self.x[:B], self.dense_dnn, train=False)
+        return self.mlp.forward_out(self._a, self.dense_dnn)
+
+    def _probabilities(self, B: int, lin, y_d, pred: torch.Tensor) -> torch.Tensor:
+        ops.logit_loss(self.zero_bias, lin, y_d, None, None, B, y=self.y[:B], pred=pred)
+        return pred
 
     def predict(self, dense: torch.Tensor, cat: torch.Tensor) -> torch.Tensor:
         """probabilities[:, 1] (wide_n_deep.py:228-232)"""
         B = dense.shape[0]
         lin, y_d = self._forward(dense, cat)
-        ops.logit_loss(self.zero_bias, lin, y_d, None, None, B, y=self.y[:B], pred=self.pred[:B])
-        return self.pred[:B]
+        return self._probabilities(B, lin, y_d, self.pred[:B])
+
+    def predict_examples(self, data: torch.Tensor, offsets: torch.Tensor, err: torch.Tensor, pred: torch.Tensor,
+                         example_base: int = 0) -> torch.Tensor:
+        """probabilities[:, 1] of the serialized tf.Examples data[offsets[b], offsets[b+1]) (uint8 / int64 [B+1]
+        device tensors, B <= batch_size) -- the serving input of wide_n_deep.py:233-242, parsed on the device
+        (ops.wd_serve_input).  A rejected Example min-folds (example_base + b) << 16 | check << 8 | key into err
+        (int64 [1], -1 = none) and leaves its pred[b] undefined; nothing here waits for the device."""
+        B = offsets.numel() - 1
+        assert B <= self.B
+        lin = self.lin[:B] if self.has_linear else None
+        ops.wd_serve_input(data, offsets, example_base, self.emb.var if self.has_dnn else None,
+                           self.wide_cat.var if self.has_linear else None,
+                           self.dense_lin["linear/numeric"] if self.has_linear else None,
+                           self.dense_lin["linear/linear_model/bias_weights"] if self.has_linear else None,
+                           self.num_perm, NUM_BUCKETS, self.K, self.x[:B] if self.has_dnn else None, lin, err)
+        return self._probabilities(B, lin, self._dnn(B), pred)
 
     # ---- one optimizer step of each part ----------------------------------------------------------------------
     def train_step(self, dense: torch.Tensor, cat: torch.Tensor, labels: torch.Tensor) -> torch.Tensor:
