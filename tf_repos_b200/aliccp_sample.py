@@ -20,8 +20,8 @@ import torch
 
 from . import _lib
 from ._lib import check
-from .aliccp_tfrecord import _pieces
-from .criteo_feature import _Timer, _stream, _upload, _ws
+from .ops import _stream
+from .text_chunks import Timer, pieces, scratch, upload
 
 _L = _lib.raw()
 
@@ -116,14 +116,14 @@ def _pass_a(files, mode, count_table, cap, md5_table, seed, parts, chunk_bytes, 
     line_base = 0
     for path in files:
         file_line, offset = 0, 0
-        for piece in _pieces(path, chunk_bytes):
+        for piece in pieces(path, chunk_bytes):
             if len(piece) >= MAX_CHUNK:
                 raise AliccpSampleError(f"{path}: a line near line {file_line + 1} is 2^30 bytes or longer "
                                         "(not accepted by this implementation)")
             n_lines = piece.count(b"\n") + (0 if piece.endswith(b"\n") else 1)
-            text = _upload(piece, dev)
+            text = upload(piece, dev)
             ws_bytes = int(_L.ctr_aliccp_sample_chunk_workspace_bytes(len(piece), n_lines))
-            ws = _ws(ws_bytes, dev)
+            ws = scratch(ws_bytes, dev)
             timer.start()
             check(_L.ctr_aliccp_sample_classify(text.data_ptr(), len(piece), n_lines, mode,
                                                 count_table.data_ptr() if mode == 2 else None, cap,
@@ -192,7 +192,7 @@ def _pass_b(S: _Set, mult, vocab, n_vocab, out_dir, seed, parts, budget, dev, ti
             vocab.data_ptr(), n_vocab, r_off.data_ptr())
     timers["render"].start()
     check(_L.ctr_aliccp_sample_render(*args, None, _stream()), "ctr_aliccp_sample_render")
-    rendered = _ws(int(r_off[S.n_rec]), dev)
+    rendered = scratch(int(r_off[S.n_rec]), dev)
     check(_L.ctr_aliccp_sample_render(*args, rendered.data_ptr(), _stream()), "ctr_aliccp_sample_render")
     timers["render"].stop()
 
@@ -204,9 +204,9 @@ def _pass_b(S: _Set, mult, vocab, n_vocab, out_dir, seed, parts, budget, dev, ti
     def emit(out, lo, hi):
         nonlocal empty
         for path, offset, length, n_lines, line_base, sample_base in S.chunks:
-            text = _upload(_read(path, offset, length), dev)
+            text = upload(_read(path, offset, length), dev)
             ws_bytes = int(_L.ctr_aliccp_sample_chunk_workspace_bytes(length, n_lines))
-            ws = _ws(ws_bytes, dev)
+            ws = scratch(ws_bytes, dev)
             timers["pass_b"].start()
             check(_L.ctr_aliccp_sample_emit(text.data_ptr(), length, n_lines, line_base, seed, S.s_rec.data_ptr(),
                                             sample_base, r_off.data_ptr(), rendered.data_ptr(), vocab.data_ptr(),
@@ -220,7 +220,7 @@ def _pass_b(S: _Set, mult, vocab, n_vocab, out_dir, seed, parts, budget, dev, ti
     S.stats["empty_lines"] = empty
     part_bytes = torch.empty(parts, dtype=torch.int64, device=dev)
     ws_bytes = int(_L.ctr_aliccp_sample_order_workspace_bytes(S.n_samples))
-    ws = _ws(ws_bytes, dev)
+    ws = scratch(ws_bytes, dev)
     timers["pass_b"].start()
     check(_L.ctr_aliccp_sample_order(S.s_key.data_ptr(), s_val.data_ptr(), S.n_samples, parts, part_bytes.data_ptr(),
                                      ws.data_ptr(), ws_bytes, _stream()), "ctr_aliccp_sample_order")
@@ -241,7 +241,7 @@ def _pass_b(S: _Set, mult, vocab, n_vocab, out_dir, seed, parts, budget, dev, ti
     groups.append((g0, parts))
     for a, b in groups:
         lo, hi = starts[a], starts[b]
-        out = _ws(hi - lo, dev)
+        out = scratch(hi - lo, dev)
         if hi > lo:
             emit(out.data_ptr(), lo, hi)
         for p in range(a, b):
@@ -285,7 +285,7 @@ def _remove(out_dir, parts, extra=()):
 
 
 def _prepare(input_dir, output_dir, cutoff, parts, seed, chunk_bytes, cap, budget, dev):
-    timers = {k: _Timer() for k in ("pass_a", "vocab", "render", "pass_b")}
+    timers = {k: Timer() for k in ("pass_a", "vocab", "render", "pass_b")}
     count_table = torch.zeros(int(_L.ctr_aliccp_sample_count_table_bytes(cap)), dtype=torch.uint8, device=dev)
     md5_table = torch.empty(int(_L.ctr_aliccp_sample_md5_table_bytes(cap)), dtype=torch.uint8, device=dev)
     feat_cnts = os.path.join(output_dir, "feat_cnts")
@@ -311,12 +311,12 @@ def _prepare(input_dir, output_dir, cutoff, parts, seed, chunk_bytes, cap, budge
                               "about twice the number of distinct field:fid keys of tr")
                 vocab = torch.empty(cap, dtype=torch.int64, device=dev)
                 ws_bytes = int(_L.ctr_aliccp_sample_vocab_workspace_bytes(cap))
-                ws = _ws(ws_bytes, dev)
+                ws = scratch(ws_bytes, dev)
                 check(_L.ctr_aliccp_sample_vocab(count_table.data_ptr(), cap, cutoff, vocab.data_ptr(),
                                                  info.data_ptr(), ws.data_ptr(), ws_bytes, _stream()),
                       "ctr_aliccp_sample_vocab")
                 _, _, n_vocab, _, fc_bytes = info.tolist()
-                text = _ws(fc_bytes, dev)
+                text = scratch(fc_bytes, dev)
                 check(_L.ctr_aliccp_sample_feat_cnts(text.data_ptr(), ws.data_ptr(), ws_bytes, cap, _stream()),
                       "ctr_aliccp_sample_feat_cnts")
                 timers["vocab"].stop()

@@ -21,7 +21,8 @@ import torch
 
 from . import _lib
 from ._lib import check
-from .criteo_feature import _Timer, _chunks, _stream, _upload, _ws
+from .ops import _stream
+from .text_chunks import Timer, pieces, scratch, upload
 
 _L = _lib.raw()
 
@@ -78,21 +79,6 @@ def _raise(path: str, line_no: int, code: int, token: bytes):
     raise AliccpTFRecordError(f"{path}: line {line_no}: {_WHAT[code]}: {shown!r}")
 
 
-def _pieces(path: str, chunk_bytes: int):
-    """The file in pieces of whole lines, at most chunk_bytes each unless one line alone is longer."""
-    for data in _chunks(path, chunk_bytes):
-        if len(data) <= chunk_bytes:
-            yield data
-            continue
-        pos = 0
-        while pos < len(data):
-            end = data.rfind(b"\n", pos, pos + chunk_bytes) + 1
-            if end <= pos:
-                end = data.find(b"\n", pos) + 1 or len(data)
-            yield data[pos:end]
-            pos = end
-
-
 def _long_line(piece: bytes):
     """index of the first line of 2^31 bytes (MAX_LINE) or more, or None"""
     pos, k = 0, 0
@@ -106,14 +92,14 @@ def _long_line(piece: bytes):
 
 
 def convert_file(in_path: str, out_path: str, chunk_bytes: int = 64 << 20, device="cuda",
-                 timers: Dict[str, _Timer] = None) -> Dict:
+                 timers: Dict[str, Timer] = None) -> Dict:
     """gen_tfrecords(in_file) (:38-102) into out_path.  -> lines, input and output bytes, declined numbers."""
     dev = torch.device(device)
     if dev.type != "cuda":
         raise _lib.CtrError("aliccp_tfrecord runs on a CUDA device (there is no CPU path)")
     if not 1 <= chunk_bytes < (1 << 30):
         raise ValueError("chunk_bytes must be in [1, 2^30)")
-    timers = timers if timers is not None else {"plan": _Timer(), "write": _Timer()}
+    timers = timers if timers is not None else {"plan": Timer(), "write": Timer()}
     stats = {"lines": 0, "in_bytes": 0, "out_bytes": 0, "declined": 0}
     try:
         with torch.cuda.device(dev), open(out_path, "wb") as fo:
@@ -128,14 +114,14 @@ def convert_file(in_path: str, out_path: str, chunk_bytes: int = 64 << 20, devic
 def _convert(path, fo, chunk_bytes, dev, timers, stats):
     info = torch.empty(4, dtype=torch.int64, device=dev)
     line_base = 0
-    for piece in _pieces(path, chunk_bytes):
+    for piece in pieces(path, chunk_bytes):
         if len(piece) >= MAX_LINE:
             k = _long_line(piece)
             if k is not None:
                 _raise(path, line_base + k + 1, _LONG, piece[:80])
-        text = _upload(piece, dev)
+        text = upload(piece, dev)
         ws_bytes = int(_L.ctr_aliccp_workspace_bytes(len(piece)))
-        ws = _ws(ws_bytes, dev)
+        ws = scratch(ws_bytes, dev)
         timers["plan"].start()
         check(_L.ctr_aliccp_plan(text.data_ptr(), len(piece), line_base, info.data_ptr(), ws.data_ptr(), ws_bytes,
                                  _stream()), "ctr_aliccp_plan")
@@ -165,7 +151,7 @@ def _convert(path, fo, chunk_bytes, dev, timers, stats):
             if token is None:
                 token = _fault_token(piece.split(b"\n", row + 1)[row], code)
             _raise(path, line_base + row + 1, code, token)
-        out = _ws(out_bytes, dev)
+        out = scratch(out_bytes, dev)
         timers["write"].start()
         check(_L.ctr_aliccp_write(text.data_ptr(), len(piece), decl_vals.data_ptr() if decl_vals is not None else None,
                                   out.data_ptr(), ws.data_ptr(), ws_bytes, _stream()), "ctr_aliccp_write")
@@ -187,7 +173,7 @@ def convert(input_dir: str, output_dir: str, chunk_bytes: int = 64 << 20, device
     if not os.path.exists(output_dir):
         os.mkdir(output_dir)
     files = sorted(glob.glob(os.path.join(input_dir, "*-*")))
-    timers = {"plan": _Timer(), "write": _Timer()}
+    timers = {"plan": Timer(), "write": Timer()}
     per_file: List[Dict] = []
     for f in files:
         out = os.path.join(output_dir, os.path.basename(f) + ".tfrecord")

@@ -9,13 +9,15 @@ column; the restrictions of DESIGN.md §2.4 raise the same way."""
 from __future__ import annotations
 
 import os
-from typing import Dict, Iterator, List
+from typing import Dict, List
 
 import numpy as np
 import torch
 
 from . import _lib
 from ._lib import check
+from .ops import _stream
+from .text_chunks import Timer, chunks, scratch, upload
 
 _L = _lib.raw()
 
@@ -46,25 +48,6 @@ def split_decisions(n: int, state: np.random.RandomState) -> np.ndarray:
     return (np.floor(state.random_sample(n) * 10000).astype(np.int64) % 10) != 0
 
 
-def _chunks(path: str, chunk_bytes: int) -> Iterator[bytes]:
-    """The file in pieces of about chunk_bytes that end at a '\\n' (the last piece: at the end of the file)."""
-    with open(path, "rb") as fh:
-        rest = b""
-        while True:
-            buf = fh.read(chunk_bytes)
-            data = rest + buf
-            if not buf:
-                if data:
-                    yield data
-                return
-            cut = data.rfind(b"\n") + 1
-            if cut == 0:
-                rest = data
-                continue
-            yield data[:cut]
-            rest = data[cut:]
-
-
 def _column(col: int, test: bool) -> str:
     j = col + (1 if test else 0)
     return "label" if j == 0 else (f"I{j}" if j <= N_INT else f"C{j - N_INT}")
@@ -73,39 +56,6 @@ def _column(col: int, test: bool) -> str:
 def _raise(path: str, word: int, test: bool = False):
     line, col, code = (word >> 16) & ((1 << 46) - 1), (word >> 8) & 0xFF, word & 0xFF
     raise CriteoFeatureError(f"{path}: line {line + 1}, column {col} ({_column(col, test)}): {_WHAT[code]}")
-
-
-class _Timer:
-    """Device time of the enqueued work between start() and stop(), summed over calls (CUDA events)."""
-
-    def __init__(self):
-        self.pairs = []
-
-    def start(self):
-        e = torch.cuda.Event(enable_timing=True)
-        e.record()
-        self.pairs.append([e, None])
-
-    def stop(self):
-        e = torch.cuda.Event(enable_timing=True)
-        e.record()
-        self.pairs[-1][1] = e
-
-    def ms(self) -> float:
-        torch.cuda.synchronize()
-        return sum(a.elapsed_time(b) for a, b in self.pairs)
-
-
-def _stream() -> int:
-    return torch.cuda.current_stream().cuda_stream
-
-
-def _ws(nbytes: int, dev) -> torch.Tensor:
-    return torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=dev)
-
-
-def _upload(data: bytes, dev) -> torch.Tensor:
-    return torch.from_numpy(np.frombuffer(data, dtype=np.uint8).copy()).to(dev)
 
 
 def preprocess(input_dir: str, output_dir: str, cutoff: int = 200, device="cuda", chunk_bytes: int = 64 << 20,
@@ -131,15 +81,15 @@ def _preprocess(train, test, output_dir, cutoff, dev, chunk_bytes, cap):
     table = torch.zeros(int(_L.ctr_criteo_table_bytes(cap)), dtype=torch.uint8, device=dev)
     minmax = torch.tensor([MAXSIZE] * N_INT + [-MAXSIZE] * N_INT, dtype=torch.int64, device=dev)
     info = torch.empty(5, dtype=torch.int64, device=dev)
-    timers = {k: _Timer() for k in ("stats", "vocab", "emit_train", "emit_test")}
+    timers = {k: Timer() for k in ("stats", "vocab", "emit_train", "emit_test")}
 
     # ---- pass 1: min/max and categorical counts (:74-85, :39-45) ----
     chunk_lines: List[int] = []
     line_base, n_bytes, first_dict_err, last = 0, 0, _NONE, b""
-    for data in _chunks(train, chunk_bytes):
-        text = _upload(data, dev)
+    for data in chunks(train, chunk_bytes):
+        text = upload(data, dev)
         ws_bytes = int(_L.ctr_criteo_stats_workspace_bytes(len(data)))
-        ws = _ws(ws_bytes, dev)
+        ws = scratch(ws_bytes, dev)
         timers["stats"].start()
         check(_L.ctr_criteo_stats(text.data_ptr(), len(data), line_base, table.data_ptr(), cap, minmax.data_ptr(),
                                   info.data_ptr(), ws.data_ptr(), ws_bytes, _stream()), "ctr_criteo_stats")
@@ -166,7 +116,7 @@ def _preprocess(train, test, output_dir, cutoff, dev, chunk_bytes, cap):
     vocab_keys = torch.empty(cap, dtype=torch.int64, device=dev)
     field_counts = torch.empty(N_CAT, dtype=torch.int64, device=dev)
     ws_bytes = int(_L.ctr_criteo_vocab_workspace_bytes(cap))
-    ws = _ws(ws_bytes, dev)
+    ws = scratch(ws_bytes, dev)
     timers["vocab"].start()
     check(_L.ctr_criteo_vocab(table.data_ptr(), cap, cutoff, vocab_keys.data_ptr(), field_counts.data_ptr(),
                               ws.data_ptr(), ws_bytes, _stream()), "ctr_criteo_vocab")
@@ -201,18 +151,18 @@ def _preprocess(train, test, output_dir, cutoff, dev, chunk_bytes, cap):
     off_dev = torch.tensor(offsets[:N_CAT], dtype=torch.int64, device=dev)
     body = last[:-1] if last.endswith(b"\n") else last
     label = body[body.rfind(b"\n") + 1:].split(b"\t")[0]     # `label` of the last train line, used by te (:147,167)
-    label_dev = _upload(label, dev) if label else None
+    label_dev = upload(label, dev) if label else None
 
     def emit(path, files, test, timer, lines_per_chunk=None):
         rs = np.random.RandomState([0])              # random.seed(0) (:127)
         line_base, n_tr, n_va = 0, 0, 0
-        for k, data in enumerate(_chunks(path, chunk_bytes)):
-            text = _upload(data, dev)
+        for k, data in enumerate(chunks(path, chunk_bytes)):
+            text = upload(data, dev)
             flags = None
             if not test:
                 flags = torch.from_numpy(split_decisions(lines_per_chunk[k], rs).astype(np.uint8)).to(dev)
             ws_bytes = int(_L.ctr_criteo_emit_workspace_bytes(len(data)))
-            ws = _ws(ws_bytes, dev)
+            ws = scratch(ws_bytes, dev)
             common = (table.data_ptr(), cap, num_min.data_ptr(), num_den.data_ptr(), off_dev.data_ptr(),
                       label_dev.data_ptr() if (test and label_dev is not None) else None, len(label) if test else 0)
             flag_ptr = flags.data_ptr() if flags is not None and flags.numel() else None
@@ -224,8 +174,8 @@ def _preprocess(train, test, output_dir, cutoff, dev, chunk_bytes, cap):
             word &= _NONE
             if word != _NONE:
                 _raise(path, word, test)
-            out_tr = _ws(tr_bytes, dev)
-            out_va = _ws(va_bytes, dev)
+            out_tr = scratch(tr_bytes, dev)
+            out_va = scratch(va_bytes, dev)
             timer.start()
             check(_L.ctr_criteo_emit_write(text.data_ptr(), len(data), int(test), flag_ptr, *common, out_tr.data_ptr(),
                                            out_va.data_ptr(), ws.data_ptr(), ws_bytes, _stream()),

@@ -26,7 +26,6 @@ constexpr int AS_THREADS = 256, AS_WARPS = AS_THREADS / 32;
 constexpr int AS_MAX_FIELD = 16, AS_MAX_MD5 = 64, AS_MD5_WORDS = 8;
 constexpr int64_t AS_MAX_PROBE = 1 << 15;   // a key that finds no slot within this many probes overflows the table
 constexpr int64_t AS_FIRST_ID = 20;
-constexpr int AS_TILE = 16 * AS_THREADS;     // items per CTA in the radix passes
 constexpr size_t AS_MAX_LEN = (size_t)1 << 30;
 constexpr int64_t AS_MAX_CAP = (int64_t)1 << 31;
 
@@ -34,32 +33,12 @@ enum { AS_SKIP = 0, AS_COMMON = 1, AS_SAMPLE = 2, AS_FILTERED = 3 };
 // info of ctr_aliccp_sample_classify
 enum { AI_LINES, AI_ERR, AI_FILTERED, AI_MALFORMED, AI_CNT_DROP, AI_MD5_DROP, AI_COMMONS, AI_CBYTES, AI_SAMPLES, AI_N };
 
-__device__ __forceinline__ int as_lane() { return threadIdx.x & 31; }
-__device__ __forceinline__ unsigned as_lt() { return (1u << as_lane()) - 1; }
-__device__ __forceinline__ uint32_t as_byte(const uint8_t* t, int64_t p) { return __ldg(t + p); }
-__device__ __forceinline__ bool as_space(uint32_t c) { return c == ' ' || (c >= '\t' && c <= '\r'); }  // str.strip()
 // bytes that no field, val, sample_id, y, z or md5 may hold (restriction): NUL, \x01-\x03, whitespace, ':'
-__device__ __forceinline__ bool as_bad(uint32_t c) { return c <= 3 || as_space(c) || c == ':'; }
-
-__host__ __device__ __forceinline__ uint64_t as_mix(uint64_t x) {   // splitmix64 finaliser
-  x ^= x >> 30; x *= 0xBF58476D1CE4E5B9ull;
-  x ^= x >> 27; x *= 0x94D049BB133111EBull;
-  return x ^ (x >> 31);
-}
+__device__ __forceinline__ bool as_bad(uint32_t c) { return c <= 3 || is_py_space(c) || c == ':'; }
 
 // r_i: the (i+1)-th output of SplitMix64 seeded with `seed`, top 31 bits
 __device__ __forceinline__ uint32_t as_shuffle_key(uint64_t seed, uint64_t i) {
-  return (uint32_t)(as_mix(seed + (i + 1) * 0x9E3779B97F4A7C15ull) >> 33);
-}
-
-__device__ __forceinline__ int as_digits(uint64_t v) {
-  int n = 1;
-  for (; v >= 10; v /= 10) ++n;
-  return n;
-}
-
-__device__ __forceinline__ void as_put_u64(uint64_t v, char* o, int nd) {
-  for (int i = nd - 1; i >= 0; --i) { o[i] = (char)('0' + v % 10); v /= 10; }
+  return (uint32_t)(splitmix64_finalize(seed + (i + 1) * 0x9E3779B97F4A7C15ull) >> 33);
 }
 
 // ---- tables ----------------------------------------------------------------------------------------------------
@@ -97,14 +76,14 @@ struct AsMd5 {
 __device__ __forceinline__ void as_pack_field(const uint8_t* t, int64_t s, int64_t e, uint64_t& a, uint64_t& b) {
   a = 0; b = 0;
   for (int i = 0; i < (int)(e - s); ++i) {
-    const uint64_t c = as_byte(t, s + i);
+    const uint64_t c = byte_at(t, s + i);
     if (i < 8) a |= c << (56 - 8 * i); else b |= c << (56 - 8 * (i - 8));
   }
   if (e - s <= 8) b = 1;
 }
 
 __device__ bool as_cnt_add(const AsCnt& T, uint64_t k0, uint64_t k1, uint64_t k2, uint64_t add) {
-  uint64_t s = __umul64hi(as_mix(k0 ^ as_mix(k1 ^ as_mix(k2))), (uint64_t)T.cap);
+  uint64_t s = __umul64hi(splitmix64_finalize(k0 ^ splitmix64_finalize(k1 ^ splitmix64_finalize(k2))), (uint64_t)T.cap);
   const int64_t probes = T.cap < AS_MAX_PROBE ? T.cap : AS_MAX_PROBE;
   for (int64_t i = 0; i < probes; ++i) {
     if (as_claim(T.k0 + s, k0) && as_claim(T.k1 + s, k1) && as_claim(T.k2 + s, k2)) {
@@ -121,9 +100,9 @@ __device__ int64_t as_md5_insert(const AsMd5& M, const uint8_t* t, int64_t s, in
   uint64_t w[AS_MD5_WORDS];
   const int n = (int)(e - s), nw = (n + 7) / 8;
   for (int j = 0; j < AS_MD5_WORDS; ++j) w[j] = 0;
-  for (int i = 0; i < n; ++i) w[i >> 3] |= (uint64_t)as_byte(t, s + i) << (8 * (i & 7));
-  uint64_t h = as_mix((uint64_t)n);
-  for (int j = 0; j < nw; ++j) h = as_mix(h ^ w[j]);
+  for (int i = 0; i < n; ++i) w[i >> 3] |= (uint64_t)byte_at(t, s + i) << (8 * (i & 7));
+  uint64_t h = splitmix64_finalize((uint64_t)n);
+  for (int j = 0; j < nw; ++j) h = splitmix64_finalize(h ^ w[j]);
   uint64_t slot = __umul64hi(h, (uint64_t)M.cap);
   const int64_t probes = M.cap < AS_MAX_PROBE ? M.cap : AS_MAX_PROBE;
   for (int64_t i = 0; i < probes; ++i) {
@@ -147,18 +126,18 @@ struct AsLine {
 
 // line.strip() of [p, e) and its first five commas.  Warp-uniform.
 __device__ void as_fields(const uint8_t* t, int64_t p, int64_t e, AsLine& L) {
-  const int lane = as_lane();
+  const int lane = lane_id();
   int64_t s = e, te = e;
   for (int64_t w = p; w < e; w += 32) {
     const int64_t q = w + lane;
-    const unsigned m = __ballot_sync(FULL_MASK, q < e && !as_space(as_byte(t, q)));
+    const unsigned m = __ballot_sync(FULL_MASK, q < e && !is_py_space(byte_at(t, q)));
     if (m) { s = w + __ffs(m) - 1; break; }
   }
   L.s = s; L.te = e; L.nul = false; L.nf = 1;
   if (s == e) return;   // blank: one empty field
   for (int64_t w = e; w > s; w -= 32) {
     const int64_t q = w - 32 + lane;
-    const unsigned m = __ballot_sync(FULL_MASK, q >= s && !as_space(as_byte(t, q)));
+    const unsigned m = __ballot_sync(FULL_MASK, q >= s && !is_py_space(byte_at(t, q)));
     if (m) { te = w - 32 + (31 - __clz(m)) + 1; break; }
   }
   L.te = te;
@@ -166,7 +145,7 @@ __device__ void as_fields(const uint8_t* t, int64_t p, int64_t e, AsLine& L) {
   bool nul = false;
   for (int64_t w = s; w < te && nc <= 5; w += 32) {
     const int64_t q = w + lane;
-    const uint32_t b = q < te ? as_byte(t, q) : 1u;
+    const uint32_t b = q < te ? byte_at(t, q) : 1u;
     unsigned m = __ballot_sync(FULL_MASK, b == ',');
     nul |= __ballot_sync(FULL_MASK, b == 0) != 0;
     while (m && nc <= 5) {
@@ -196,8 +175,8 @@ __device__ __forceinline__ int as_kind(const uint8_t* t, const AsLine& L, AsSpan
   }
   if (L.nf != 6) return AS_SKIP;
   S.md5_s = L.c2 + 1; S.md5_e = L.c3; S.fs = L.c4 + 1; S.fe = L.te;
-  const bool y0 = L.c1 - L.c0 == 2 && as_byte(t, L.c0 + 1) == '0';
-  const bool z1 = L.c2 - L.c1 == 2 && as_byte(t, L.c1 + 1) == '1';
+  const bool y0 = L.c1 - L.c0 == 2 && byte_at(t, L.c0 + 1) == '0';
+  const bool z1 = L.c2 - L.c1 == 2 && byte_at(t, L.c1 + 1) == '1';
   return y0 && z1 ? AS_FILTERED : AS_SAMPLE;
 }
 
@@ -212,25 +191,25 @@ __device__ int as_token(const uint8_t* t, int64_t s, int64_t e, AsTok& k) {
   int n2 = 0, n3 = 0;
   k.p2 = k.p3 = -1;
   for (int64_t p = s; p < e; ++p)
-    if (as_byte(t, p) == 2) { ++n2; k.p2 = p; }
+    if (byte_at(t, p) == 2) { ++n2; k.p2 = p; }
   if (n2 != 1) return 1;
   for (int64_t p = k.p2 + 1; p < e; ++p)
-    if (as_byte(t, p) == 3) { ++n3; k.p3 = p; }
+    if (byte_at(t, p) == 3) { ++n3; k.p3 = p; }
   if (n3 != 1) return 1;
   if (k.p2 - s < 1 || k.p2 - s > AS_MAX_FIELD) return 2;
   for (int64_t p = s; p < k.p2; ++p)
-    if (as_bad(as_byte(t, p))) return 2;
+    if (as_bad(byte_at(t, p))) return 2;
   // fid: 0 or [1-9][0-9]* below 2^63, so that its text and its number are one key
-  if (k.p3 == k.p2 + 1 || (as_byte(t, k.p2 + 1) == '0' && k.p3 > k.p2 + 2)) return 2;
+  if (k.p3 == k.p2 + 1 || (byte_at(t, k.p2 + 1) == '0' && k.p3 > k.p2 + 2)) return 2;
   uint64_t v = 0;
   for (int64_t p = k.p2 + 1; p < k.p3; ++p) {
-    const uint64_t d = as_byte(t, p) - (uint64_t)'0';
+    const uint64_t d = byte_at(t, p) - (uint64_t)'0';
     if (d > 9 || v > (0x7FFFFFFFFFFFFFFFull - d) / 10) return 2;
     v = v * 10 + d;
   }
   k.fid = v;
   for (int64_t p = k.p3 + 1; p < e; ++p)
-    if (as_bad(as_byte(t, p))) return 2;
+    if (as_bad(byte_at(t, p))) return 2;
   return 0;
 }
 
@@ -238,13 +217,13 @@ __device__ int as_token(const uint8_t* t, int64_t s, int64_t e, AsTok& k) {
 // lanes with `end` set end the token [start, q).
 template <class Visit>
 __device__ __forceinline__ void as_tokens(const uint8_t* t, int64_t s, int64_t e, Visit&& visit) {
-  const int lane = as_lane();
+  const int lane = lane_id();
   int64_t carry = s - 1;
   for (int64_t w = s; w <= e; w += 32) {
     const int64_t q = w + lane;
-    const bool end = q <= e && (q == e || as_byte(t, q) == 1);
+    const bool end = q <= e && (q == e || byte_at(t, q) == 1);
     const unsigned m = __ballot_sync(FULL_MASK, end);
-    const unsigned below = m & as_lt();
+    const unsigned below = m & lanemask_lt();
     visit(end, (below ? w + 31 - __clz(below) : carry) + 1, q);
     if (m) carry = w + 31 - __clz(m);
   }
@@ -253,8 +232,8 @@ __device__ __forceinline__ void as_tokens(const uint8_t* t, int64_t s, int64_t e
 __device__ __forceinline__ bool as_any_bad(const uint8_t* t, int64_t s, int64_t e) {
   bool bad = false;
   for (int64_t w = s; w < e; w += 32) {
-    const int64_t q = w + as_lane();
-    bad |= __ballot_sync(FULL_MASK, q < e && as_bad(as_byte(t, q))) != 0;
+    const int64_t q = w + lane_id();
+    bad |= __ballot_sync(FULL_MASK, q < e && as_bad(byte_at(t, q))) != 0;
   }
   return bad;
 }
@@ -276,17 +255,6 @@ __device__ int as_check(const uint8_t* t, const AsLine& L, const AsSpans& S, int
   return kind;
 }
 
-__device__ __forceinline__ void as_bounds(const int64_t* line_start, int64_t nn, int64_t len, int64_t row, int64_t& p,
-                                          int64_t& e) {
-  p = line_start[row];
-  e = row < nn ? line_start[row + 1] - 1 : len;
-}
-
-__device__ __forceinline__ int64_t as_n_lines(const uint8_t* t, int64_t len, int64_t nn, int64_t cap) {
-  const int64_t n = nn + ((len > 0 && t[len - 1] != '\n') ? 1 : 0);
-  return n < cap ? n : cap;
-}
-
 // per-line results of classify, scanned in place: cls | slot | fs (feat_list start) | flen (common records) |
 // coff (scan of flen) | cord (scan of is-common) | sord (scan of is-sample)
 struct AsPerLine {
@@ -299,13 +267,13 @@ __global__ void __launch_bounds__(AS_THREADS) as_classify_kernel(const uint8_t* 
                                                                 const int64_t* __restrict__ nnl, int64_t n_cap,
                                                                 int mode, AsCnt C, AsMd5 M, AsPerLine P,
                                                                 int64_t* __restrict__ info) {
-  const int lane = as_lane();
-  const int64_t nn = nnl[0], n_lines = as_n_lines(t, len, nn, n_cap);
+  const int lane = lane_id();
+  const int64_t nn = nnl[0], n_lines = chunk_lines(t, len, nn, n_cap);
   if (blockIdx.x == 0 && threadIdx.x == 0) info[AI_LINES] = n_lines;
   const int64_t warps = (int64_t)gridDim.x * AS_WARPS;
   for (int64_t row = (int64_t)blockIdx.x * AS_WARPS + (threadIdx.x >> 5); row < n_lines; row += warps) {
     int64_t p, e;
-    as_bounds(line_start, nn, len, row, p, e);
+    line_bounds(line_start, nn, len, row, p, e);
     AsLine L;
     as_fields(t, p, e, L);
     AsSpans S;
@@ -349,43 +317,6 @@ __global__ void __launch_bounds__(AS_THREADS) as_classify_kernel(const uint8_t* 
   }
 }
 
-// exclusive scan of a[0, n) in place (one CTA, tiles of 1024); n = *count when count is given; total -> *total
-template <typename T>
-__global__ void __launch_bounds__(1024) as_scan_kernel(T* __restrict__ a, const int64_t* __restrict__ count, int64_t n_fixed,
-                                                       int64_t* __restrict__ total) {
-  __shared__ int64_t warp_sum_s[32];
-  __shared__ int64_t carry_s;
-  const int64_t n = count ? count[0] : n_fixed;
-  if (threadIdx.x == 0) carry_s = 0;
-  __syncthreads();
-  for (int64_t base = 0; base < n; base += 1024) {
-    const int64_t i = base + threadIdx.x;
-    const int64_t v = i < n ? (int64_t)a[i] : 0;
-    int64_t x = v;
-    for (int o = 1; o < 32; o <<= 1) {
-      const int64_t y = __shfl_up_sync(FULL_MASK, x, o);
-      if ((threadIdx.x & 31) >= o) x += y;
-    }
-    if ((threadIdx.x & 31) == 31) warp_sum_s[threadIdx.x >> 5] = x;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-      int64_t w = warp_sum_s[threadIdx.x];
-      for (int o = 1; o < 32; o <<= 1) {
-        const int64_t y = __shfl_up_sync(FULL_MASK, w, o);
-        if (threadIdx.x >= o) w += y;
-      }
-      warp_sum_s[threadIdx.x] = w;
-    }
-    __syncthreads();
-    const int64_t before = carry_s + (threadIdx.x >= 32 ? warp_sum_s[(threadIdx.x >> 5) - 1] : 0) + (x - v);
-    if (i < n) a[i] = (T)before;
-    __syncthreads();
-    if (threadIdx.x == 1023) carry_s = before + v;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0 && total) total[0] = carry_s;
-}
-
 // common records -> arena + (offset, length, slot), md5 record = the largest id; samples -> (slot, part << 31 | r_i)
 __global__ void __launch_bounds__(AS_THREADS) as_place_kernel(const uint8_t* __restrict__ t, const int64_t* __restrict__ info,
                                                              AsPerLine P, int64_t line_base, uint64_t seed, int64_t parts,
@@ -394,7 +325,7 @@ __global__ void __launch_bounds__(AS_THREADS) as_place_kernel(const uint8_t* __r
                                                              int32_t* __restrict__ rec_slot, int64_t rec_base,
                                                              int32_t* __restrict__ s_rec, uint64_t* __restrict__ s_key,
                                                              int64_t sample_base) {
-  const int lane = as_lane();
+  const int lane = lane_id();
   const int64_t n_lines = info[AI_LINES], warps = (int64_t)gridDim.x * AS_WARPS;
   for (int64_t row = (int64_t)blockIdx.x * AS_WARPS + (threadIdx.x >> 5); row < n_lines; row += warps) {
     const int kind = P.cls[row];
@@ -457,7 +388,7 @@ __global__ void __launch_bounds__(AS_THREADS) as_count_commons_kernel(const uint
 // order depends on the schedule; everything downstream is sorted by the whole key first.
 __global__ void __launch_bounds__(AS_THREADS) as_compact_kernel(AsCnt T, int64_t cutoff, AsCnt E,
                                                                uint64_t* __restrict__ kf, int64_t* __restrict__ counts) {
-  const int lane = as_lane();
+  const int lane = lane_id();
   const int64_t stride = (int64_t)gridDim.x * AS_THREADS, n_iter = (T.cap + stride - 1) / stride;
   for (int64_t it = 0; it < n_iter; ++it) {   // uniform trip count: the warp-aggregated atomics need whole warps
     const int64_t s = (it * gridDim.x + blockIdx.x) * AS_THREADS + threadIdx.x;
@@ -471,81 +402,11 @@ __global__ void __launch_bounds__(AS_THREADS) as_compact_kernel(AsCnt T, int64_t
     eu = __shfl_sync(FULL_MASK, eu, 0);
     ek = __shfl_sync(FULL_MASK, ek, 0);
     if (used) {
-      const int64_t e = (int64_t)eu + __popc(bu & as_lt());
+      const int64_t e = (int64_t)eu + __popc(bu & lanemask_lt());
       E.k0[e] = T.k0[s]; E.k1[e] = T.k1[s]; E.k2[e] = T.k2[s]; E.cnt[e] = c;
     }
-    if (keep) kf[(int64_t)ek + __popc(bk & as_lt())] = T.k0[s];
+    if (keep) kf[(int64_t)ek + __popc(bk & lanemask_lt())] = T.k0[s];
   }
-}
-
-// stable LSD radix sort, 8-bit digits: hist[d * nb + b] = items of CTA b with digit d
-__global__ void __launch_bounds__(AS_THREADS) as_hist_kernel(const uint64_t* __restrict__ keys, const int64_t* __restrict__ n_dev,
-                                                            int pass, int32_t* __restrict__ hist,
-                                                            int64_t* __restrict__ hist_count) {
-  __shared__ int h[256];
-  const int64_t n = n_dev[0], nb = (n + AS_TILE - 1) / AS_TILE;
-  if (blockIdx.x == 0 && threadIdx.x == 0) hist_count[0] = 256 * nb;
-  if (blockIdx.x >= nb) return;
-  h[threadIdx.x] = 0;
-  __syncthreads();
-  for (int r = 0; r < AS_TILE / AS_THREADS; ++r) {
-    const int64_t i = (int64_t)blockIdx.x * AS_TILE + r * AS_THREADS + threadIdx.x;
-    if (i < n) atomicAdd(&h[(keys[i] >> (8 * pass)) & 0xFF], 1);
-  }
-  __syncthreads();
-  hist[(int64_t)threadIdx.x * nb + blockIdx.x] = h[threadIdx.x];
-}
-
-// within a CTA the items go in index order (warp match + per-warp digit counts); vals may be null
-__global__ void __launch_bounds__(AS_THREADS) as_scatter_kernel(const uint64_t* __restrict__ keys,
-                                                               const uint32_t* __restrict__ vals,
-                                                               const int64_t* __restrict__ n_dev, int pass,
-                                                               const int32_t* __restrict__ hist,
-                                                               uint64_t* __restrict__ keys2, uint32_t* __restrict__ vals2) {
-  __shared__ int base[256];
-  __shared__ int wcnt[AS_WARPS][256];
-  const int64_t n = n_dev[0], nb = (n + AS_TILE - 1) / AS_TILE;
-  if (blockIdx.x >= nb) return;
-  const int lane = as_lane(), warp = threadIdx.x >> 5;
-  base[threadIdx.x] = hist[(int64_t)threadIdx.x * nb + blockIdx.x];
-  for (int w = 0; w < AS_WARPS; ++w) wcnt[w][threadIdx.x] = 0;
-  __syncthreads();
-  for (int r = 0; r < AS_TILE / AS_THREADS; ++r) {
-    const int64_t i = (int64_t)blockIdx.x * AS_TILE + r * AS_THREADS + threadIdx.x;
-    const bool live = i < n;
-    uint64_t k = 0;
-    uint32_t v = 0;
-    int d = 256;   // no digit: dead lanes match only each other and are not counted
-    if (live) { k = keys[i]; v = vals ? vals[i] : 0; d = (int)((k >> (8 * pass)) & 0xFF); }
-    const uint32_t peers = __match_any_sync(FULL_MASK, d);
-    const int rank = __popc(peers & as_lt());
-    if (live && rank == 0) wcnt[warp][d] = __popc(peers);
-    __syncthreads();
-    if (live) {
-      int pos = base[d] + rank;
-      for (int w = 0; w < warp; ++w) pos += wcnt[w][d];
-      keys2[pos] = k;
-      if (vals) vals2[pos] = v;
-    }
-    __syncthreads();
-    int add = 0;
-    for (int w = 0; w < AS_WARPS; ++w) { add += wcnt[w][threadIdx.x]; wcnt[w][threadIdx.x] = 0; }
-    base[threadIdx.x] += add;
-    __syncthreads();
-  }
-}
-
-__global__ void as_iota_kernel(uint32_t* __restrict__ perm, const int64_t* __restrict__ n_dev) {
-  const int64_t n = n_dev[0];
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-    perm[i] = (uint32_t)i;
-}
-
-__global__ void as_gather_kernel(const uint64_t* __restrict__ src, const uint32_t* __restrict__ perm,
-                                 const int64_t* __restrict__ n_dev, uint64_t* __restrict__ dst) {
-  const int64_t n = n_dev[0];
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-    dst[i] = src[perm ? perm[i] : i];
 }
 
 // sorted kf: run heads
@@ -580,14 +441,14 @@ __global__ void as_feat_cnts_kernel(AsCnt E, const uint32_t* __restrict__ perm, 
   for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (int64_t)gridDim.x * blockDim.x) {
     const uint32_t e = perm[j];
     const uint64_t a = E.k1[e], b = E.k2[e], fid = E.k0[e] - 1, c = E.cnt[e];
-    const int fl = as_field_len(a, b), nf = as_digits(fid), nc = as_digits(c);
+    const int fl = as_field_len(a, b), nf = dec_digits(fid), nc = dec_digits(c);
     if (!W) { off[j] = fl + 1 + nf + 1 + nc + 1; continue; }
     char* o = out + off[j];
     for (int i = 0; i < fl; ++i) o[i] = (char)(i < 8 ? (a >> (56 - 8 * i)) : (b >> (56 - 8 * (i - 8))));
     o[fl] = ':';
-    as_put_u64(fid, o + fl + 1, nf);
+    put_dec(fid, o + fl + 1, nf);
     o[fl + 1 + nf] = '\t';
-    as_put_u64(c, o + fl + 2 + nf, nc);
+    put_dec(c, o + fl + 2 + nf, nc);
     o[fl + 2 + nf + nc] = '\n';
   }
 }
@@ -609,7 +470,7 @@ __device__ __forceinline__ int64_t as_lookup(const uint64_t* __restrict__ vocab,
 template <bool W>
 __device__ void as_remap(const uint8_t* t, int64_t s, int64_t e, const uint64_t* vocab, int64_t n_vocab, char* o,
                          int64_t& pos, int64_t& kept) {
-  const int lane = as_lane();
+  const int lane = lane_id();
   as_tokens(t, s, e, [&](bool end, int64_t ts, int64_t q) {
     AsTok k;
     int64_t id = -1;
@@ -618,8 +479,8 @@ __device__ void as_remap(const uint8_t* t, int64_t s, int64_t e, const uint64_t*
       id = as_lookup(vocab, n_vocab, k.fid);
     }
     const unsigned km = __ballot_sync(FULL_MASK, id >= 0);
-    const bool sep = kept + __popc(km & as_lt()) > 0;
-    const int nd = id >= 0 ? as_digits((uint64_t)id) : 0;
+    const bool sep = kept + __popc(km & lanemask_lt()) > 0;
+    const int nd = id >= 0 ? dec_digits((uint64_t)id) : 0;
     const int64_t L = id >= 0 ? (sep ? 1 : 0) + (k.p2 - ts) + 1 + nd + 1 + (q - k.p3 - 1) : 0;
     int64_t x = L;
     for (int d = 1; d < 32; d <<= 1) {
@@ -629,12 +490,12 @@ __device__ void as_remap(const uint8_t* t, int64_t s, int64_t e, const uint64_t*
     if (W && id >= 0) {
       char* d = o + pos + x - L;
       if (sep) *d++ = ' ';
-      for (int64_t p = ts; p < k.p2; ++p) *d++ = (char)as_byte(t, p);
+      for (int64_t p = ts; p < k.p2; ++p) *d++ = (char)byte_at(t, p);
       *d++ = ':';
-      as_put_u64((uint64_t)id, d, nd);
+      put_dec((uint64_t)id, d, nd);
       d += nd;
       *d++ = ':';
-      for (int64_t p = k.p3 + 1; p < q; ++p) *d++ = (char)as_byte(t, p);
+      for (int64_t p = k.p3 + 1; p < q; ++p) *d++ = (char)byte_at(t, p);
     }
     pos += __shfl_sync(FULL_MASK, x, 31);
     kept += __popc(km);
@@ -654,7 +515,7 @@ __global__ void __launch_bounds__(AS_THREADS) as_render_kernel(const uint8_t* __
     int64_t pos = 0, kept = 0;
     if (mult[r]) as_remap<W>(arena, rec_off[r], rec_off[r] + rec_len[r], vocab, n_vocab, W ? out + r_off[r] : nullptr,
                              pos, kept);
-    if (!W && as_lane() == 0) r_off[r] = pos;
+    if (!W && lane_id() == 0) r_off[r] = pos;
   }
 }
 
@@ -680,7 +541,7 @@ __global__ void __launch_bounds__(AS_THREADS) as_emit_kernel(const uint8_t* __re
                                                             const int64_t* __restrict__ nnl,
                                                             const int64_t* __restrict__ info_cls, AsPerLine P,
                                                             AsEmitArgs a) {
-  const int lane = as_lane();
+  const int lane = lane_id();
   const int64_t nn = nnl[0], n_lines = info_cls[AI_LINES], warps = (int64_t)gridDim.x * AS_WARPS;
   for (int64_t row = (int64_t)blockIdx.x * AS_WARPS + (threadIdx.x >> 5); row < n_lines; row += warps) {
     if (P.cls[row] != AS_SAMPLE) continue;
@@ -691,11 +552,11 @@ __global__ void __launch_bounds__(AS_THREADS) as_emit_kernel(const uint8_t* __re
       if (base < a.lo || base >= a.hi) continue;
     }
     int64_t p, e;
-    as_bounds(line_start, nn, len, row, p, e);
+    line_bounds(line_start, nn, len, row, p, e);
     AsLine L;
     as_fields(t, p, e, L);
     const uint64_t r = as_shuffle_key(a.seed, (uint64_t)(a.line_base + row));
-    const int nr = as_digits(r);
+    const int nr = dec_digits(r);
     char* o = W ? a.out + (base - a.lo) : nullptr;
     int64_t pos = nr + 1 + (L.c2 - L.s) + 1;
     if (W) {
@@ -703,7 +564,7 @@ __global__ void __launch_bounds__(AS_THREADS) as_emit_kernel(const uint8_t* __re
         char c;
         if (i < nr) { uint64_t v = r; for (int j = nr - 1; j > i; --j) v /= 10; c = (char)('0' + v % 10); }
         else if (i == nr) c = '\t';
-        else if (i < pos - 1) c = (char)as_byte(t, L.s + i - nr - 1);
+        else if (i < pos - 1) c = (char)byte_at(t, L.s + i - nr - 1);
         else c = ',';
         o[i] = c;
       }
@@ -747,28 +608,19 @@ __global__ void as_offsets_kernel(const uint32_t* __restrict__ perm, const int64
 }
 
 // ---- workspace layouts and launch helpers ------------------------------------------------------------------------
-static inline size_t as_align(size_t x) { return (x + 255) & ~(size_t)255; }
-
-// per chunk: block_counts int32[nb] | n_newlines int64[2] | info int64[AI_N] | line_start int64[n_lines + 2] |
-// cls uint8[n_lines] | slot, fs, flen, coff, cord, sord int32[n_lines]
-struct AsChunkWs {
-  int32_t* block_counts;
-  int64_t *n_newlines, *info, *line_start;
+// per chunk: LineStarts (max_rows = n_lines + 1) | info int64[AI_N] | cls uint8[n_lines + 1] |
+// slot, fs, flen, coff, cord, sord int32[n_lines + 1]
+struct AsChunkWs : LineStarts {
+  int64_t* info;
   AsPerLine P;
-  int n_blocks;
-  size_t bytes;
-  AsChunkWs(void* ws, size_t len, int64_t n_lines) {
+  AsChunkWs(void* ws, size_t len, int64_t n_lines) : LineStarts(ws, len, n_lines + 1) {
     uint8_t* b = reinterpret_cast<uint8_t*>(ws);
     const size_t n = (size_t)n_lines + 1;
-    n_blocks = (int)((len + LS_BLOCK_BYTES - 1) / LS_BLOCK_BYTES);
-    size_t o = 0;
-    block_counts = reinterpret_cast<int32_t*>(b + o); o += as_align((size_t)n_blocks * 4 + 4);
-    n_newlines = reinterpret_cast<int64_t*>(b + o); o += as_align(16);
-    info = reinterpret_cast<int64_t*>(b + o); o += as_align(AI_N * 8);
-    line_start = reinterpret_cast<int64_t*>(b + o); o += as_align((n + 1) * 8);
-    P.cls = b + o; o += as_align(n);
+    size_t o = bytes;
+    info = reinterpret_cast<int64_t*>(b + o); o += align256(AI_N * 8);
+    P.cls = b + o; o += align256(n);
     int32_t** arrs[6] = {&P.slot, &P.fs, &P.flen, &P.coff, &P.cord, &P.sord};
-    for (auto a : arrs) { *a = reinterpret_cast<int32_t*>(b + o); o += as_align(n * 4); }
+    for (auto a : arrs) { *a = reinterpret_cast<int32_t*>(b + o); o += align256(n * 4); }
     bytes = o;
   }
 };
@@ -785,19 +637,19 @@ struct AsVocabWs {
   size_t bytes;
   AsVocabWs(void* ws, int64_t cap) {
     uint8_t* b = reinterpret_cast<uint8_t*>(ws);
-    const size_t c = (size_t)cap, nb = (size_t)ceil_div64(cap, AS_TILE);
+    const size_t c = (size_t)cap, nb = (size_t)ceil_div64(cap, LSD_TILE);
     size_t o = 0;
     counts = reinterpret_cast<int64_t*>(b + o); n_vocab = counts + 2; hist_count = counts + 3; fc_bytes = counts + 4;
-    o += as_align(5 * 8);
-    hist = reinterpret_cast<int32_t*>(b + o); o += as_align(256 * nb * 4);
-    E = AsCnt(b + o, cap); o += as_align(4 * c * 8);
-    kf = reinterpret_cast<uint64_t*>(b + o); o += as_align(c * 8);
-    keys = reinterpret_cast<uint64_t*>(b + o); o += as_align(c * 8);
-    keys2 = reinterpret_cast<uint64_t*>(b + o); o += as_align(c * 8);
-    perm = reinterpret_cast<uint32_t*>(b + o); o += as_align(c * 4);
-    perm2 = reinterpret_cast<uint32_t*>(b + o); o += as_align(c * 4);
-    head = reinterpret_cast<int32_t*>(b + o); o += as_align(c * 4);
-    lens = reinterpret_cast<int64_t*>(b + o); o += as_align((c + 1) * 8);
+    o += align256(5 * 8);
+    hist = reinterpret_cast<int32_t*>(b + o); o += align256(256 * nb * 4);
+    E = AsCnt(b + o, cap); o += align256(4 * c * 8);
+    kf = reinterpret_cast<uint64_t*>(b + o); o += align256(c * 8);
+    keys = reinterpret_cast<uint64_t*>(b + o); o += align256(c * 8);
+    keys2 = reinterpret_cast<uint64_t*>(b + o); o += align256(c * 8);
+    perm = reinterpret_cast<uint32_t*>(b + o); o += align256(c * 4);
+    perm2 = reinterpret_cast<uint32_t*>(b + o); o += align256(c * 4);
+    head = reinterpret_cast<int32_t*>(b + o); o += align256(c * 4);
+    lens = reinterpret_cast<int64_t*>(b + o); o += align256((c + 1) * 8);
     bytes = o;
   }
 };
@@ -812,44 +664,17 @@ struct AsOrderWs {
   size_t bytes;
   AsOrderWs(void* ws, int64_t n) {
     uint8_t* b = reinterpret_cast<uint8_t*>(ws);
-    const size_t c = (size_t)(n > 0 ? n : 1), nb = (size_t)ceil_div64((int64_t)c, AS_TILE);
+    const size_t c = (size_t)(n > 0 ? n : 1), nb = (size_t)ceil_div64((int64_t)c, LSD_TILE);
     size_t o = 0;
-    n_dev = reinterpret_cast<int64_t*>(b + o); hist_count = n_dev + 1; o += as_align(16);
-    hist = reinterpret_cast<int32_t*>(b + o); o += as_align(256 * nb * 4);
-    keys2 = reinterpret_cast<uint64_t*>(b + o); o += as_align(c * 8);
-    perm = reinterpret_cast<uint32_t*>(b + o); o += as_align(c * 4);
-    perm2 = reinterpret_cast<uint32_t*>(b + o); o += as_align(c * 4);
-    sz = reinterpret_cast<int64_t*>(b + o); o += as_align((c + 1) * 8);
+    n_dev = reinterpret_cast<int64_t*>(b + o); hist_count = n_dev + 1; o += align256(16);
+    hist = reinterpret_cast<int32_t*>(b + o); o += align256(256 * nb * 4);
+    keys2 = reinterpret_cast<uint64_t*>(b + o); o += align256(c * 8);
+    perm = reinterpret_cast<uint32_t*>(b + o); o += align256(c * 4);
+    perm2 = reinterpret_cast<uint32_t*>(b + o); o += align256(c * 4);
+    sz = reinterpret_cast<int64_t*>(b + o); o += align256((c + 1) * 8);
     bytes = o;
   }
 };
-
-static unsigned as_grid(int64_t items, int per_cta) {
-  const int64_t want = ceil_div64(items, per_cta), cap = (int64_t)sm_count() * 16;
-  return (unsigned)(want < 1 ? 1 : (want < cap ? want : cap));
-}
-
-// (keys, vals) sorted stably by the low 8 * passes bits of keys, n = *n_dev <= cap; the result is in keys / vals
-// (passes even) or keys2 / vals2 (odd): *out_keys / *out_vals
-static int as_sort(uint64_t* keys, uint32_t* vals, uint64_t* keys2, uint32_t* vals2, const int64_t* n_dev, int64_t cap,
-                   int passes, int32_t* hist, int64_t* hist_count, cudaStream_t st, uint64_t** out_keys,
-                   uint32_t** out_vals) {
-  const unsigned nb = (unsigned)ceil_div64(cap > 0 ? cap : 1, AS_TILE);
-  uint64_t* k[2] = {keys, keys2};
-  uint32_t* v[2] = {vals, vals2};
-  int cur = 0;
-  for (int pass = 0; pass < passes; ++pass, cur ^= 1) {
-    as_hist_kernel<<<nb, AS_THREADS, 0, st>>>(k[cur], n_dev, pass, hist, hist_count);
-    CTR_LAUNCHED("aliccp_sample(sort hist)");
-    as_scan_kernel<int32_t><<<1, 1024, 0, st>>>(hist, hist_count, 0, nullptr);
-    CTR_LAUNCHED("aliccp_sample(sort scan)");
-    as_scatter_kernel<<<nb, AS_THREADS, 0, st>>>(k[cur], v[cur], n_dev, pass, hist, k[cur ^ 1], v[cur ^ 1]);
-    CTR_LAUNCHED("aliccp_sample(sort scatter)");
-  }
-  *out_keys = k[cur];
-  if (out_vals) *out_vals = v[cur];
-  return CTR_OK;
-}
 
 static int as_zero(void* p, size_t n, cudaStream_t st, const char* what) {
   CTR_REQUIRE(cudaMemsetAsync(p, 0, n, st) == cudaSuccess, CTR_ERR_CUDA, "%s: memset failed", what);
@@ -890,22 +715,17 @@ int ctr_aliccp_sample_classify(const char* text, size_t len, int64_t n_lines, in
               CTR_ERR_CUDA, "ctr_aliccp_sample_classify: memset failed");
   const uint8_t* t = reinterpret_cast<const uint8_t*>(text);
   if (len > 0) {
-    ls_count_kernel<<<W.n_blocks, LS_THREADS, 0, st>>>(t, (int64_t)len, W.block_counts);
-    CTR_LAUNCHED("ctr_aliccp_sample_classify(lines)");
-    ls_scan_kernel<<<1, 1024, 0, st>>>(W.block_counts, W.n_blocks, W.n_newlines);
-    CTR_LAUNCHED("ctr_aliccp_sample_classify(lines)");
-    ls_emit_kernel<<<W.n_blocks, LS_THREADS, 0, st>>>(t, (int64_t)len, W.block_counts, n_lines + 1, W.line_start);
-    CTR_LAUNCHED("ctr_aliccp_sample_classify(lines)");
-    as_classify_kernel<<<as_grid(n_lines, AS_WARPS), AS_THREADS, 0, st>>>(
+    if (int rc = W.launch(t, len, st, "ctr_aliccp_sample_classify(lines)")) return rc;
+    as_classify_kernel<<<grid_for(n_lines, AS_WARPS, 16), AS_THREADS, 0, st>>>(
         t, (int64_t)len, W.line_start, W.n_newlines, n_lines, mode, AsCnt(count_table, count_capacity),
         AsMd5(md5_table, md5_capacity), W.P, W.info);
     CTR_LAUNCHED("ctr_aliccp_sample_classify");
     const int64_t* cnt = W.info + AI_LINES;
-    as_scan_kernel<int32_t><<<1, 1024, 0, st>>>(W.P.coff, cnt, 0, W.info + AI_CBYTES);
+    cta_scan_kernel<int32_t><<<1, 1024, 0, st>>>(W.P.coff, cnt, 0, W.info + AI_CBYTES);
     CTR_LAUNCHED("ctr_aliccp_sample_classify(scan)");
-    as_scan_kernel<int32_t><<<1, 1024, 0, st>>>(W.P.cord, cnt, 0, W.info + AI_COMMONS);
+    cta_scan_kernel<int32_t><<<1, 1024, 0, st>>>(W.P.cord, cnt, 0, W.info + AI_COMMONS);
     CTR_LAUNCHED("ctr_aliccp_sample_classify(scan)");
-    as_scan_kernel<int32_t><<<1, 1024, 0, st>>>(W.P.sord, cnt, 0, W.info + AI_SAMPLES);
+    cta_scan_kernel<int32_t><<<1, 1024, 0, st>>>(W.P.sord, cnt, 0, W.info + AI_SAMPLES);
     CTR_LAUNCHED("ctr_aliccp_sample_classify(scan)");
   }
   CTR_REQUIRE(cudaMemcpyAsync(info, W.info, AI_N * 8, cudaMemcpyDeviceToDevice, st) == cudaSuccess, CTR_ERR_CUDA,
@@ -925,7 +745,7 @@ int ctr_aliccp_sample_place(const char* text, size_t len, int64_t n_lines, int64
               "ctr_aliccp_sample_place: workspace too small");
   if (len == 0 || n_lines == 0) return CTR_OK;
   AsChunkWs W(const_cast<void*>(ws), len, n_lines);
-  as_place_kernel<<<as_grid(n_lines, AS_WARPS), AS_THREADS, 0, as_stream(stream)>>>(
+  as_place_kernel<<<grid_for(n_lines, AS_WARPS, 16), AS_THREADS, 0, as_stream(stream)>>>(
       reinterpret_cast<const uint8_t*>(text), W.info, W.P, line_base, seed, parts, AsMd5(md5_table, md5_capacity), arena,
       arena_base, rec_off, rec_len, rec_slot, rec_base, s_rec, s_key, sample_base);
   CTR_LAUNCHED("ctr_aliccp_sample_place");
@@ -944,8 +764,8 @@ int ctr_aliccp_sample_resolve(const void* md5_table, int64_t md5_capacity, int32
     if (int rc = as_zero(mult, (size_t)n_records * 4, st, "ctr_aliccp_sample_resolve")) return rc;
   const int64_t n = n_samples > n_records ? n_samples : n_records;
   if (n == 0) return CTR_OK;
-  as_resolve_kernel<<<as_grid(n, AS_THREADS), AS_THREADS, 0, st>>>(AsMd5(const_cast<void*>(md5_table), md5_capacity),
-                                                                   s_rec, n_samples, rec_slot, n_records, mult, info);
+  as_resolve_kernel<<<grid_for(n, AS_THREADS, 16), AS_THREADS, 0, st>>>(
+      AsMd5(const_cast<void*>(md5_table), md5_capacity), s_rec, n_samples, rec_slot, n_records, mult, info);
   CTR_LAUNCHED("ctr_aliccp_sample_resolve");
   return CTR_OK;
 }
@@ -959,7 +779,7 @@ int ctr_aliccp_sample_count_commons(const uint8_t* arena, const int64_t* rec_off
   cudaStream_t st = as_stream(stream);
   if (int rc = as_zero(info, 8, st, "ctr_aliccp_sample_count_commons")) return rc;
   if (n_records == 0) return CTR_OK;
-  as_count_commons_kernel<<<as_grid(n_records, AS_WARPS), AS_THREADS, 0, st>>>(
+  as_count_commons_kernel<<<grid_for(n_records, AS_WARPS, 16), AS_THREADS, 0, st>>>(
       arena, rec_off, rec_len, mult, n_records, AsCnt(count_table, count_capacity), info);
   CTR_LAUNCHED("ctr_aliccp_sample_count_commons");
   return CTR_OK;
@@ -979,29 +799,31 @@ int ctr_aliccp_sample_vocab(const void* count_table, int64_t count_capacity, int
   AsVocabWs V(ws, count_capacity);
   if (int rc = as_zero(V.counts, 5 * 8, st, "ctr_aliccp_sample_vocab")) return rc;
   const int64_t cap = count_capacity;
-  const unsigned g = as_grid(cap, AS_THREADS);
+  const unsigned g = grid_for(cap, AS_THREADS, 16);
   as_compact_kernel<<<g, AS_THREADS, 0, st>>>(AsCnt(const_cast<void*>(count_table), cap), cutoff, V.E, V.kf, V.counts);
   CTR_LAUNCHED("ctr_aliccp_sample_vocab(compact)");
   // kept fids: sorted (8 passes cover k0 < 2^64), unique -> vocab
   uint64_t* sk;
-  if (int rc = as_sort(V.kf, nullptr, V.keys2, nullptr, V.counts + 1, cap, 8, V.hist, V.hist_count, st, &sk, nullptr))
+  if (int rc = lsd_sort(V.kf, nullptr, V.keys2, nullptr, V.counts + 1, cap, 8, V.hist, V.hist_count, st,
+                        "ctr_aliccp_sample_vocab(sort)", &sk, nullptr))
     return rc;
   as_heads_kernel<<<g, AS_THREADS, 0, st>>>(sk, V.counts + 1, V.head);
   CTR_LAUNCHED("ctr_aliccp_sample_vocab(heads)");
-  as_scan_kernel<int32_t><<<1, 1024, 0, st>>>(V.head, V.counts + 1, 0, V.n_vocab);
+  cta_scan_kernel<int32_t><<<1, 1024, 0, st>>>(V.head, V.counts + 1, 0, V.n_vocab);
   CTR_LAUNCHED("ctr_aliccp_sample_vocab(scan)");
   as_unique_kernel<<<g, AS_THREADS, 0, st>>>(sk, V.counts + 1, V.head, vocab);
   CTR_LAUNCHED("ctr_aliccp_sample_vocab(unique)");
   // entries: LSD by fid, then field bytes 8..15, then field bytes 0..7
-  as_iota_kernel<<<g, AS_THREADS, 0, st>>>(V.perm, V.counts);
+  lsd_iota_kernel<<<g, AS_THREADS, 0, st>>>(V.perm, V.counts);
   CTR_LAUNCHED("ctr_aliccp_sample_vocab(iota)");
   const uint64_t* words[3] = {V.E.k0, V.E.k2, V.E.k1};
   uint32_t* p = V.perm;
   for (int w = 0; w < 3; ++w) {
-    as_gather_kernel<<<g, AS_THREADS, 0, st>>>(words[w], p, V.counts, V.keys);
+    lsd_gather_kernel<<<g, AS_THREADS, 0, st>>>(words[w], p, V.counts, V.keys);
     CTR_LAUNCHED("ctr_aliccp_sample_vocab(gather)");
     uint32_t* other = p == V.perm ? V.perm2 : V.perm;
-    if (int rc = as_sort(V.keys, p, V.keys2, other, V.counts, cap, 8, V.hist, V.hist_count, st, &sk, &p)) return rc;
+    if (int rc = lsd_sort(V.keys, p, V.keys2, other, V.counts, cap, 8, V.hist, V.hist_count, st,
+                          "ctr_aliccp_sample_vocab(sort)", &sk, &p)) return rc;
   }
   if (p != V.perm) {
     CTR_REQUIRE(cudaMemcpyAsync(V.perm, p, (size_t)cap * 4, cudaMemcpyDeviceToDevice, st) == cudaSuccess, CTR_ERR_CUDA,
@@ -1009,7 +831,7 @@ int ctr_aliccp_sample_vocab(const void* count_table, int64_t count_capacity, int
   }
   as_feat_cnts_kernel<false><<<g, AS_THREADS, 0, st>>>(V.E, V.perm, V.counts, V.lens, nullptr);
   CTR_LAUNCHED("ctr_aliccp_sample_vocab(feat_cnts)");
-  as_scan_kernel<int64_t><<<1, 1024, 0, st>>>(V.lens, V.counts, 0, V.fc_bytes);
+  cta_scan_kernel<int64_t><<<1, 1024, 0, st>>>(V.lens, V.counts, 0, V.fc_bytes);
   CTR_LAUNCHED("ctr_aliccp_sample_vocab(scan)");
   CTR_REQUIRE(cudaMemcpyAsync(info, V.counts, 5 * 8, cudaMemcpyDeviceToDevice, st) == cudaSuccess, CTR_ERR_CUDA,
               "ctr_aliccp_sample_vocab: copy of info failed");
@@ -1023,7 +845,7 @@ int ctr_aliccp_sample_feat_cnts(char* out, const void* ws, size_t ws_bytes, int6
   CTR_REQUIRE(ws && ws_bytes >= ctr_aliccp_sample_vocab_workspace_bytes(count_capacity), CTR_ERR_WORKSPACE,
               "ctr_aliccp_sample_feat_cnts: workspace too small");
   AsVocabWs V(const_cast<void*>(ws), count_capacity);
-  as_feat_cnts_kernel<true><<<as_grid(count_capacity, AS_THREADS), AS_THREADS, 0, as_stream(stream)>>>(
+  as_feat_cnts_kernel<true><<<grid_for(count_capacity, AS_THREADS, 16), AS_THREADS, 0, as_stream(stream)>>>(
       V.E, V.perm, V.counts, V.lens, out);
   CTR_LAUNCHED("ctr_aliccp_sample_feat_cnts");
   return CTR_OK;
@@ -1036,7 +858,7 @@ int ctr_aliccp_sample_render(const uint8_t* arena, const int64_t* rec_off, const
                   (n_records == 0 || (arena && rec_off && rec_len && mult)),
               CTR_ERR_INVALID_ARG, "ctr_aliccp_sample_render: bad arguments");
   cudaStream_t st = as_stream(stream);
-  const unsigned g = as_grid(n_records, AS_WARPS);
+  const unsigned g = grid_for(n_records, AS_WARPS, 16);
   if (!out) {   // plan: r_off[0, n_records] = the exclusive scan of the rendered lengths
     if (int rc = as_zero(r_off + n_records, 8, st, "ctr_aliccp_sample_render")) return rc;
     if (n_records) {
@@ -1044,7 +866,7 @@ int ctr_aliccp_sample_render(const uint8_t* arena, const int64_t* rec_off, const
                                                         nullptr);
       CTR_LAUNCHED("ctr_aliccp_sample_render(plan)");
     }
-    as_scan_kernel<int64_t><<<1, 1024, 0, st>>>(r_off, nullptr, n_records + 1, nullptr);
+    cta_scan_kernel<int64_t><<<1, 1024, 0, st>>>(r_off, nullptr, n_records + 1, nullptr);
     CTR_LAUNCHED("ctr_aliccp_sample_render(scan)");
     return CTR_OK;
   }
@@ -1074,17 +896,12 @@ int ctr_aliccp_sample_emit(const char* text, size_t len, int64_t n_lines, int64_
                   cudaMemsetAsync(W.info + AI_ERR, 0xFF, 8, st) == cudaSuccess &&
                   cudaMemsetAsync(W.n_newlines, 0, 16, st) == cudaSuccess,
               CTR_ERR_CUDA, "ctr_aliccp_sample_emit: memset failed");
-  ls_count_kernel<<<W.n_blocks, LS_THREADS, 0, st>>>(t, (int64_t)len, W.block_counts);
-  CTR_LAUNCHED("ctr_aliccp_sample_emit(lines)");
-  ls_scan_kernel<<<1, 1024, 0, st>>>(W.block_counts, W.n_blocks, W.n_newlines);
-  CTR_LAUNCHED("ctr_aliccp_sample_emit(lines)");
-  ls_emit_kernel<<<W.n_blocks, LS_THREADS, 0, st>>>(t, (int64_t)len, W.block_counts, n_lines + 1, W.line_start);
-  CTR_LAUNCHED("ctr_aliccp_sample_emit(lines)");
-  const unsigned g = as_grid(n_lines, AS_WARPS);
+  if (int rc = W.launch(t, len, st, "ctr_aliccp_sample_emit(lines)")) return rc;
+  const unsigned g = grid_for(n_lines, AS_WARPS, 16);
   as_classify_kernel<<<g, AS_THREADS, 0, st>>>(t, (int64_t)len, W.line_start, W.n_newlines, n_lines, 0, AsCnt(),
                                                AsMd5(), W.P, W.info);
   CTR_LAUNCHED("ctr_aliccp_sample_emit(classify)");
-  as_scan_kernel<int32_t><<<1, 1024, 0, st>>>(W.P.sord, W.info + AI_LINES, 0, nullptr);
+  cta_scan_kernel<int32_t><<<1, 1024, 0, st>>>(W.P.sord, W.info + AI_LINES, 0, nullptr);
   CTR_LAUNCHED("ctr_aliccp_sample_emit(scan)");
   AsEmitArgs a{seed, line_base, sample_base, s_rec, r_off, rendered, vocab, n_vocab, s_val, lo, hi, out, info};
   if (out)
@@ -1115,16 +932,17 @@ int ctr_aliccp_sample_order(uint64_t* s_key, int64_t* s_val, int64_t n_samples, 
   int bits = 31;
   while (((int64_t)1 << (bits - 31)) < parts) ++bits;
   const int passes = (bits + 7) / 8;
-  const unsigned g = as_grid(n_samples, AS_THREADS);
-  as_iota_kernel<<<g, AS_THREADS, 0, st>>>(O.perm, O.n_dev);
+  const unsigned g = grid_for(n_samples, AS_THREADS, 16);
+  lsd_iota_kernel<<<g, AS_THREADS, 0, st>>>(O.perm, O.n_dev);
   CTR_LAUNCHED("ctr_aliccp_sample_order(iota)");
   uint64_t* sk;
   uint32_t* sp;
-  if (int rc = as_sort(s_key, O.perm, O.keys2, O.perm2, O.n_dev, n_samples, passes, O.hist, O.hist_count, st, &sk, &sp))
+  if (int rc = lsd_sort(s_key, O.perm, O.keys2, O.perm2, O.n_dev, n_samples, passes, O.hist, O.hist_count, st,
+                        "ctr_aliccp_sample_order(sort)", &sk, &sp))
     return rc;
   as_sizes_sorted_kernel<<<g, AS_THREADS, 0, st>>>(sk, sp, s_val, n_samples, O.sz, part_bytes);
   CTR_LAUNCHED("ctr_aliccp_sample_order(sizes)");
-  as_scan_kernel<int64_t><<<1, 1024, 0, st>>>(O.sz, O.n_dev, 0, nullptr);
+  cta_scan_kernel<int64_t><<<1, 1024, 0, st>>>(O.sz, O.n_dev, 0, nullptr);
   CTR_LAUNCHED("ctr_aliccp_sample_order(scan)");
   as_offsets_kernel<<<g, AS_THREADS, 0, st>>>(sp, O.sz, n_samples, s_val);
   CTR_LAUNCHED("ctr_aliccp_sample_order(offsets)");

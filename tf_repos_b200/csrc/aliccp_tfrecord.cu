@@ -55,10 +55,6 @@ __constant__ int kAlValKey[AL_AD - AL_UMH] = {8, 12, 6, 10};                   /
 __constant__ double kAlPow10[23] = {1e0,  1e1,  1e2,  1e3,  1e4,  1e5,  1e6,  1e7,  1e8,  1e9,  1e10, 1e11,
                                     1e12, 1e13, 1e14, 1e15, 1e16, 1e17, 1e18, 1e19, 1e20, 1e21, 1e22};
 
-__device__ __forceinline__ int al_lane() { return threadIdx.x & 31; }
-__device__ __forceinline__ unsigned al_lt() { return (1u << al_lane()) - 1; }
-__device__ __forceinline__ uint32_t al_byte(const uint8_t* t, int64_t p) { return __ldg(t + p); }
-__device__ __forceinline__ bool al_space(uint32_t c) { return c == ' ' || (c >= '\t' && c <= '\r'); }  // str.strip()
 __device__ __forceinline__ int al_vl(uint64_t v) { return v < 128 ? 1 : (70 - __clzll((long long)v)) / 7; }
 
 // per-warp state in shared memory
@@ -77,17 +73,17 @@ struct AlLine {
 
 // line.strip().split(',') of [p, e) -> false unless it has exactly 4 fields.  Warp-uniform.
 __device__ __forceinline__ bool al_fields(const uint8_t* t, int64_t p, int64_t e, AlLine& L) {
-  const int lane = al_lane();
+  const int lane = lane_id();
   int64_t s = e, te = e;
   for (int64_t w = p; w < e; w += 32) {
     const int64_t q = w + lane;
-    const unsigned m = __ballot_sync(FULL_MASK, q < e && !al_space(al_byte(t, q)));
+    const unsigned m = __ballot_sync(FULL_MASK, q < e && !is_py_space(byte_at(t, q)));
     if (m) { s = w + __ffs(m) - 1; break; }
   }
   if (s == e) return false;   // blank
   for (int64_t w = e; w > s; w -= 32) {
     const int64_t q = w - 32 + lane;
-    const unsigned m = __ballot_sync(FULL_MASK, q >= s && !al_space(al_byte(t, q)));
+    const unsigned m = __ballot_sync(FULL_MASK, q >= s && !is_py_space(byte_at(t, q)));
     if (m) { te = w - 32 + (31 - __clz(m)) + 1; break; }
   }
   int nc = 0;
@@ -95,7 +91,7 @@ __device__ __forceinline__ bool al_fields(const uint8_t* t, int64_t p, int64_t e
   bool nul = false;
   for (int64_t w = s; w < te && nc <= 3; w += 32) {
     const int64_t q = w + lane;
-    const uint32_t b = q < te ? al_byte(t, q) : 1u;
+    const uint32_t b = q < te ? byte_at(t, q) : 1u;
     unsigned m = __ballot_sync(FULL_MASK, b == ',');
     nul |= __ballot_sync(FULL_MASK, b == 0) != 0;
     while (m && nc <= 3) {
@@ -120,14 +116,14 @@ __device__ __forceinline__ bool al_fields(const uint8_t* t, int64_t p, int64_t e
 __device__ __forceinline__ bool al_value(const uint8_t* t, int64_t s, int64_t e, float& out) {
   if (e <= s || e - s > 64) return false;
   int64_t p = s;
-  uint32_t c = al_byte(t, p);
+  uint32_t c = byte_at(t, p);
   const bool neg = c == '-';
   if (c == '+' || c == '-') ++p;
   uint64_t M = 0;
   int nd = 0, frac = 0;
   bool dot = false, big = false;
   for (; p < e; ++p) {
-    c = al_byte(t, p);
+    c = byte_at(t, p);
     if (c >= '0' && c <= '9') {
       ++nd;
       frac += dot;
@@ -143,13 +139,13 @@ __device__ __forceinline__ bool al_value(const uint8_t* t, int64_t s, int64_t e,
   }
   if (nd == 0) return false;
   int ex = 0;
-  if (p < e && (al_byte(t, p) | 0x20) == 'e') {
+  if (p < e && (byte_at(t, p) | 0x20) == 'e') {
     ++p;
     bool eneg = false;
-    if (p < e && (al_byte(t, p) == '+' || al_byte(t, p) == '-')) eneg = al_byte(t, p++) == '-';
+    if (p < e && (byte_at(t, p) == '+' || byte_at(t, p) == '-')) eneg = byte_at(t, p++) == '-';
     int ned = 0;
-    for (; p < e && al_byte(t, p) >= '0' && al_byte(t, p) <= '9'; ++p, ++ned) {
-      ex = ex * 10 + (int)(al_byte(t, p) - '0');
+    for (; p < e && byte_at(t, p) >= '0' && byte_at(t, p) <= '9'; ++p, ++ned) {
+      ex = ex * 10 + (int)(byte_at(t, p) - '0');
       ex = ex > 10000 ? 10000 : ex;
     }
     if (ned == 0) return false;
@@ -172,7 +168,7 @@ __device__ __forceinline__ bool al_id(const uint8_t* t, int64_t s, int64_t e, ui
   v = 0;
   if (e <= s) return false;
   for (int64_t p = s; p < e; ++p) {
-    const uint32_t c = al_byte(t, p);
+    const uint32_t c = byte_at(t, p);
     if (c < '0' || c > '9') return false;
     const uint64_t d = c - '0';
     if (v > (0x7FFFFFFFFFFFFFFFull - d) / 10) return false;
@@ -186,7 +182,7 @@ __device__ __forceinline__ int al_class(const uint8_t* t, int64_t s, int64_t e) 
   const int64_t n = e - s;
   if (n != 3 && n != 6) return -1;
   uint64_t v = (uint64_t)n << 56;
-  for (int i = 0; i < n; ++i) v |= (uint64_t)al_byte(t, s + i) << (8 * i);
+  for (int i = 0; i < n; ++i) v |= (uint64_t)byte_at(t, s + i) << (8 * i);
   for (int c = 0; c < AL_CLASSES; ++c)
     if (kAlField[c] == v) return c;
   return -1;
@@ -201,15 +197,15 @@ struct AlTok {
 // lanes with sep set end a token.  -> number of tokens.
 template <class Visit>
 __device__ __forceinline__ int al_tokens(const uint8_t* t, int64_t s, int64_t e, Visit&& visit) {
-  const int lane = al_lane();
+  const int lane = lane_id();
   int count = 0, carry_cls = -1;
   int64_t carry = s - 1;
   for (int64_t w = s; w <= e; w += 32) {
     const int64_t q = w + lane;
-    const uint32_t b = q < e ? al_byte(t, q) : ' ';
+    const uint32_t b = q < e ? byte_at(t, q) : ' ';
     const bool sep = q <= e && (b == ' ' || b == ':');
     const unsigned m = __ballot_sync(FULL_MASK, sep);
-    const unsigned below = m & al_lt();
+    const unsigned below = m & lanemask_lt();
     AlTok k;
     k.end = q;
     k.start = (below ? w + 31 - __clz(below) : carry) + 1;
@@ -217,7 +213,7 @@ __device__ __forceinline__ int al_tokens(const uint8_t* t, int64_t s, int64_t e,
     k.role = k.idx % 3;
     const int cls = sep && k.role == 0 ? al_class(t, k.start, k.end) : -1;
     const unsigned fm = __ballot_sync(FULL_MASK, sep && k.role == 0);
-    const unsigned fb = fm & (al_lt() | (1u << lane));   // field tokens at or before this lane
+    const unsigned fb = fm & (lanemask_lt() | (1u << lane));   // field tokens at or before this lane
     const int from = __shfl_sync(FULL_MASK, cls, fb ? 31 - __clz(fb) : 0);
     k.cls = fb ? from : carry_cls;
     const int last = __shfl_sync(FULL_MASK, cls, fm ? 31 - __clz(fm) : 0);
@@ -250,7 +246,7 @@ struct AlPass1 {
 // in line order; spans != nullptr: their (row, start, end) from spans[3 * span_base] on).
 __device__ __forceinline__ void al_pass1(const uint8_t* t, const AlLine& L, AlWarp& W, AlPass1& R, int64_t row, int64_t* spans,
                          int64_t span_base) {
-  const int lane = al_lane();
+  const int lane = lane_id();
   if (lane < AL_CLASSES) { W.cnt[lane] = 0; W.bytes[lane] = 0; }
   __syncwarp();
   float v = 0.f;
@@ -285,7 +281,7 @@ __device__ __forceinline__ void al_pass1(const uint8_t* t, const AlLine& L, AlWa
     first_bad = min(first_bad, al_first(__ballot_sync(FULL_MASK, bad), k.idx));
     const unsigned dm = __ballot_sync(FULL_MASK, decl);
     if (spans && decl) {
-      const int64_t j = span_base + ndecl + __popc(dm & al_lt());
+      const int64_t j = span_base + ndecl + __popc(dm & lanemask_lt());
       spans[3 * j] = row; spans[3 * j + 1] = k.start; spans[3 * j + 2] = k.end;
     }
     ndecl += __popc(dm);
@@ -323,7 +319,7 @@ __device__ __forceinline__ int64_t al_entry(int k, int64_t P, int64_t& head) {
 
 // size of the framed record from W.cnt / W.bytes (every lane gets it)
 __device__ __forceinline__ int64_t al_record_bytes(const AlWarp& W) {
-  const int lane = al_lane();
+  const int lane = lane_id();
   int64_t x = 0, head;
   if (lane < AL_KEYS) x = al_entry(lane, al_payload(W, lane), head);
   for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(FULL_MASK, x, o);
@@ -341,15 +337,6 @@ __device__ __forceinline__ void al_put_f32(uint8_t* o, float f) {
   o[0] = (uint8_t)b; o[1] = (uint8_t)(b >> 8); o[2] = (uint8_t)(b >> 16); o[3] = (uint8_t)(b >> 24);
 }
 
-__device__ __forceinline__ void al_line(const unsigned char* t, int64_t len, const int64_t* line_start, int64_t nn,
-                                        int64_t row, int64_t& p, int64_t& e) {
-  p = line_start[row];
-  e = row < nn ? line_start[row + 1] - 1 : len;
-}
-__device__ __forceinline__ int64_t al_n_lines(const unsigned char* t, int64_t len, int64_t nn) {
-  return nn + ((len > 0 && t[len - 1] != '\n') ? 1 : 0);
-}
-
 // per line: rec[row] = framed record bytes (0 = skipped), decl[row] = declined numbers; the chunk's error word
 __global__ void __launch_bounds__(AL_THREADS) al_plan_kernel(const uint8_t* __restrict__ t, int64_t len,
                                                             const int64_t* __restrict__ line_start,
@@ -358,8 +345,8 @@ __global__ void __launch_bounds__(AL_THREADS) al_plan_kernel(const uint8_t* __re
                                                             int64_t* __restrict__ info) {
   __shared__ AlWarp warps[AL_WARPS];
   AlWarp& W = warps[threadIdx.x >> 5];
-  const int lane = al_lane();
-  const int64_t nn = n_newlines[0], n_lines = al_n_lines(t, len, nn);
+  const int lane = lane_id();
+  const int64_t nn = n_newlines[0], n_lines = chunk_lines(t, len, nn);
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     info[0] = n_lines;
     rec[n_lines] = 0;
@@ -368,7 +355,7 @@ __global__ void __launch_bounds__(AL_THREADS) al_plan_kernel(const uint8_t* __re
   for (int64_t row = (int64_t)blockIdx.x * AL_WARPS + (threadIdx.x >> 5); row < n_lines;
        row += (int64_t)gridDim.x * AL_WARPS) {
     int64_t p, e;
-    al_line(t, len, line_start, nn, row, p, e);
+    line_bounds(line_start, nn, len, row, p, e);
     AlLine L;
     int64_t size = 0, nd = 0;
     if (al_fields(t, p, e, L)) {
@@ -431,12 +418,12 @@ __global__ void __launch_bounds__(AL_THREADS) al_declines_kernel(const uint8_t* 
                                                                 int64_t* __restrict__ spans) {
   __shared__ AlWarp warps[AL_WARPS];
   AlWarp& W = warps[threadIdx.x >> 5];
-  const int64_t nn = n_newlines[0], n_lines = al_n_lines(t, len, nn);
+  const int64_t nn = n_newlines[0], n_lines = chunk_lines(t, len, nn);
   for (int64_t row = (int64_t)blockIdx.x * AL_WARPS + (threadIdx.x >> 5); row < n_lines;
        row += (int64_t)gridDim.x * AL_WARPS) {
     if (decl[row + 1] == decl[row]) continue;
     int64_t p, e;
-    al_line(t, len, line_start, nn, row, p, e);
+    line_bounds(line_start, nn, len, row, p, e);
     AlLine L;
     al_fields(t, p, e, L);
     AlPass1 R;
@@ -456,13 +443,13 @@ __global__ void __launch_bounds__(AL_THREADS, 2) al_write_kernel(const uint8_t* 
   __shared__ AlWarp warps[AL_WARPS];
   tr_crc_tables(tab, x8);
   AlWarp& W = warps[threadIdx.x >> 5];
-  const int lane = al_lane();
-  const int64_t nn = n_newlines[0], n_lines = al_n_lines(t, len, nn);
+  const int lane = lane_id();
+  const int64_t nn = n_newlines[0], n_lines = chunk_lines(t, len, nn);
   for (int64_t row = (int64_t)blockIdx.x * AL_WARPS + (threadIdx.x >> 5); row < n_lines;
        row += (int64_t)gridDim.x * AL_WARPS) {
     if (rec[row + 1] == rec[row]) continue;
     int64_t p, e;
-    al_line(t, len, line_start, nn, row, p, e);
+    line_bounds(line_start, nn, len, row, p, e);
     AlLine L;
     al_fields(t, p, e, L);
     AlPass1 R;
@@ -530,7 +517,7 @@ __global__ void __launch_bounds__(AL_THREADS, 2) al_write_kernel(const uint8_t* 
       if (id) al_id(t, k.start, k.end, v);
       if (val) simple = al_value(t, k.start, k.end, f);
       const unsigned dm = __ballot_sync(FULL_MASK, val && !simple);
-      if (val && !simple) f = decl_vals[dbase + nd + __popc(dm & al_lt())];
+      if (val && !simple) f = decl_vals[dbase + nd + __popc(dm & lanemask_lt())];
       nd += __popc(dm);
       int64_t at = 0;
       unsigned km = __ballot_sync(FULL_MASK, id || val);
@@ -569,33 +556,20 @@ __global__ void __launch_bounds__(AL_THREADS, 2) al_write_kernel(const uint8_t* 
   }
 }
 
-// workspace: block_counts int32[nb] | n_newlines int64[2] | line_start, rec, decl int64[len + 2]
-struct AlWs {
-  int32_t* block_counts;
-  int64_t *n_newlines, *line_start, *rec, *decl;
-  int n_blocks;
-  size_t bytes;
-  AlWs(void* ws, size_t len) {
-    auto align = [](size_t x) { return (x + 255) & ~(size_t)255; };
+// workspace: LineStarts (max_rows = len + 1) | rec, decl int64[len + 2]
+struct AlWs : LineStarts {
+  int64_t *rec, *decl;
+  AlWs(void* ws, size_t len) : LineStarts(ws, len, (int64_t)len + 1) {
     uint8_t* b = reinterpret_cast<uint8_t*>(ws);
-    n_blocks = (int)((len + LS_BLOCK_BYTES - 1) / LS_BLOCK_BYTES);
-    size_t o = 0;
-    block_counts = reinterpret_cast<int32_t*>(b + o); o += align((size_t)n_blocks * 4);
-    n_newlines = reinterpret_cast<int64_t*>(b + o); o += align(16);
-    line_start = reinterpret_cast<int64_t*>(b + o); o += align((len + 2) * 8);
-    rec = reinterpret_cast<int64_t*>(b + o); o += align((len + 2) * 8);
-    decl = reinterpret_cast<int64_t*>(b + o); o += align((len + 2) * 8);
+    size_t o = bytes;
+    rec = reinterpret_cast<int64_t*>(b + o); o += align256((len + 2) * 8);
+    decl = reinterpret_cast<int64_t*>(b + o); o += align256((len + 2) * 8);
     bytes = o;
   }
 };
 
 // chunks the kernels accept: the line-start pass keeps newline counts in int32
 constexpr size_t AL_MAX_LEN = (size_t)1 << 31;
-
-static unsigned al_grid(int64_t lines) {
-  const int64_t want = ceil_div64(lines, AL_WARPS), cap = (int64_t)sm_count() * 8;
-  return (unsigned)(want < 1 ? 1 : (want < cap ? want : cap));
-}
 
 }  // namespace ctr
 
@@ -618,15 +592,10 @@ int ctr_aliccp_plan(const char* text, size_t len, int64_t line_base, int64_t* in
               CTR_ERR_CUDA, "ctr_aliccp_plan: memset failed");
   if (len == 0) return CTR_OK;
   const uint8_t* t = reinterpret_cast<const uint8_t*>(text);
-  AlWs A(ws, len);
-  ls_count_kernel<<<A.n_blocks, LS_THREADS, 0, st>>>(t, (int64_t)len, A.block_counts);
-  CTR_LAUNCHED("ctr_aliccp_plan(lines)");
-  ls_scan_kernel<<<1, 1024, 0, st>>>(A.block_counts, A.n_blocks, A.n_newlines);
-  CTR_LAUNCHED("ctr_aliccp_plan(lines)");
-  ls_emit_kernel<<<A.n_blocks, LS_THREADS, 0, st>>>(t, (int64_t)len, A.block_counts, (int64_t)len + 1, A.line_start);
-  CTR_LAUNCHED("ctr_aliccp_plan(lines)");
-  al_plan_kernel<<<al_grid((int64_t)len + 1), AL_THREADS, 0, st>>>(t, (int64_t)len, A.line_start, A.n_newlines,
-                                                                  line_base, A.rec, A.decl, info);
+  const AlWs A(ws, len);
+  if (int rc = A.launch(t, len, st, "ctr_aliccp_plan(lines)")) return rc;
+  al_plan_kernel<<<grid_for((int64_t)len + 1, AL_WARPS, 8), AL_THREADS, 0, st>>>(
+      t, (int64_t)len, A.line_start, A.n_newlines, line_base, A.rec, A.decl, info);
   CTR_LAUNCHED("ctr_aliccp_plan");
   al_scan_kernel<<<1, 1024, 0, st>>>(A.rec, A.decl, info);
   CTR_LAUNCHED("ctr_aliccp_plan(scan)");
@@ -641,7 +610,7 @@ int ctr_aliccp_declines(const char* text, size_t len, const void* ws, size_t ws_
               "ctr_aliccp_declines: workspace too small");
   if (len == 0) return CTR_OK;
   AlWs A(const_cast<void*>(ws), len);
-  al_declines_kernel<<<al_grid((int64_t)len + 1), AL_THREADS, 0, as_stream(stream)>>>(
+  al_declines_kernel<<<grid_for((int64_t)len + 1, AL_WARPS, 8), AL_THREADS, 0, as_stream(stream)>>>(
       reinterpret_cast<const uint8_t*>(text), (int64_t)len, A.line_start, A.n_newlines, A.decl, spans);
   CTR_LAUNCHED("ctr_aliccp_declines");
   return CTR_OK;
@@ -655,7 +624,7 @@ int ctr_aliccp_write(const char* text, size_t len, const float* decl_vals, void*
               "ctr_aliccp_write: workspace too small");
   if (len == 0) return CTR_OK;
   AlWs A(const_cast<void*>(ws), len);
-  al_write_kernel<<<al_grid((int64_t)len + 1), AL_THREADS, 0, as_stream(stream)>>>(
+  al_write_kernel<<<grid_for((int64_t)len + 1, AL_WARPS, 8), AL_THREADS, 0, as_stream(stream)>>>(
       reinterpret_cast<const uint8_t*>(text), (int64_t)len, A.line_start, A.n_newlines, A.rec, A.decl, decl_vals,
       static_cast<uint8_t*>(out));
   CTR_LAUNCHED("ctr_aliccp_write");

@@ -71,6 +71,44 @@ __device__ __forceinline__ float4 f4_shfl_xor(float4 a, int o) {
 }
 __device__ __forceinline__ float f4_hsum(float4 a) { return (a.x + a.y) + (a.z + a.w); }
 
+__device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
+__device__ __forceinline__ unsigned lanemask_lt() { return (1u << lane_id()) - 1; }
+
+// text bytes: a read-only byte load, and the whitespace Python's str.strip() removes
+__device__ __forceinline__ uint32_t byte_at(const uint8_t* t, int64_t p) { return __ldg(t + p); }
+__device__ __forceinline__ bool is_py_space(uint32_t c) { return c == ' ' || (c >= '\t' && c <= '\r'); }
+
+__host__ __device__ __forceinline__ uint64_t splitmix64_finalize(uint64_t x) {   // the SplitMix64 finaliser
+  x ^= x >> 30; x *= 0xBF58476D1CE4E5B9ull;
+  x ^= x >> 27; x *= 0x94D049BB133111EBull;
+  return x ^ (x >> 31);
+}
+
+// decimal digits of v, and v written in decimal at o[0, nd) with nd = dec_digits(v)
+__device__ __forceinline__ int dec_digits(uint64_t v) {
+  int n = 1;
+  for (; v >= 10; v /= 10) ++n;
+  return n;
+}
+__device__ __forceinline__ void put_dec(uint64_t v, char* o, int nd) {
+  for (int i = nd - 1; i >= 0; --i) { o[i] = (char)('0' + v % 10); v /= 10; }
+}
+// v in decimal at o when W; -> its length
+template <bool W>
+__device__ __forceinline__ int put_dec(uint64_t v, char* o) {
+  const int nd = dec_digits(v);
+  if (W) put_dec(v, o, nd);
+  return nd;
+}
+
 static inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+static inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// grid of a grid-stride kernel: one CTA per per_cta items, at most ctas_per_sm CTAs per SM, at least one
+static inline unsigned grid_for(int64_t items, int64_t per_cta, int ctas_per_sm) {
+  const int64_t want = ceil_div64(items, per_cta), cap = (int64_t)sm_count() * ctas_per_sm;
+  return (unsigned)(want < 1 ? 1 : (want < cap ? want : cap));
+}
 
 }  // namespace ctr

@@ -53,11 +53,7 @@ struct CfTable {
 };
 
 __device__ __forceinline__ uint64_t cf_home(uint64_t key, int f, int64_t cap) {
-  uint64_t x = key ^ ((uint64_t)(f + 1) * 0x9E3779B97F4A7C15ull);   // splitmix64 finaliser
-  x ^= x >> 30; x *= 0xBF58476D1CE4E5B9ull;
-  x ^= x >> 27; x *= 0x94D049BB133111EBull;
-  x ^= x >> 31;
-  return __umul64hi(x, (uint64_t)cap);
+  return __umul64hi(splitmix64_finalize(key ^ ((uint64_t)(f + 1) * 0x9E3779B97F4A7C15ull)), (uint64_t)cap);
 }
 
 // Linear probing without locks: a slot's key is set once (CAS 0 -> key), then its tag once (CAS 0 -> field + 1).
@@ -133,28 +129,7 @@ __device__ __forceinline__ int64_t cf_col_end(const unsigned char* __restrict__ 
   return q;
 }
 
-// line `row` of the chunk: [p, e), '\n' dropped
-__device__ __forceinline__ void cf_line(const unsigned char* __restrict__ text, int64_t len,
-                                        const int64_t* __restrict__ line_start, int64_t nn, int64_t row, int64_t& p,
-                                        int64_t& e) {
-  p = line_start[row];
-  e = row < nn ? line_start[row + 1] - 1 : len;
-}
-
-__device__ __forceinline__ int64_t cf_n_lines(const unsigned char* __restrict__ text, int64_t len, int64_t nn) {
-  return nn + ((len > 0 && text[len - 1] != '\n') ? 1 : 0);
-}
-
 // ---- formatting ----------------------------------------------------------------------------------------------
-template <bool W>
-__device__ __forceinline__ int cf_put_u64(uint64_t v, char* o) {
-  int nd = 1;
-  for (uint64_t x = v; x >= 10; x /= 10) ++nd;
-  if (W)
-    for (int i = nd - 1; i >= 0; --i) { o[i] = (char)('0' + v % 10); v /= 10; }
-  return nd;
-}
-
 // "{:.6f}".format(q).rstrip('0').rstrip('.'): the exact binary value of q rounded half-to-even at 1e-6.
 // q = m * 2^s; the integer part is m >> -s and the fraction fm / 2^-s is scaled by 10^6 in 128-bit integers.
 // In this pipeline |q| < 2^55 (|v - min| <= 2^54, |max - min| >= 1; min = sys.maxsize gives |q| ~ 0.5).
@@ -181,7 +156,7 @@ __device__ __forceinline__ int cf_put_fixed6(double q, char* o) {
   }
   int n = 0;
   if (bits >> 63) { if (W) o[n] = '-'; ++n; }
-  n += cf_put_u64<W>(ip, o + n);
+  n += put_dec<W>(ip, o + n);
   if (fr) {
     int nd = 6;
     while (fr % 10 == 0) { fr /= 10; --nd; }
@@ -226,7 +201,7 @@ __device__ int64_t cf_emit_line(const unsigned char* __restrict__ t, int64_t p, 
       n += ce - q;
     } else if (j <= CF_NI) {
       if (W) o[n] = ' ';
-      n += 1 + cf_put_u64<W>((uint64_t)j, o + n + 1);
+      n += 1 + put_dec<W>((uint64_t)j, o + n + 1);
       if (W) o[n] = ':';
       ++n;
       double v = 0.0;
@@ -247,7 +222,7 @@ __device__ int64_t cf_emit_line(const unsigned char* __restrict__ t, int64_t p, 
       // values the train dictionary cannot hold (empty, > 8 bytes, NUL, "<unk>") are <unk> = 0, as in the reference
       const uint32_t id = (ce > q && cf_pack_key(t, q, ce, key) == 0) ? cf_lookup(a.table, key, f) : 0u;
       if (W) o[n] = ' ';
-      n += 1 + cf_put_u64<W>((uint64_t)(a.offsets[f] + id), o + n + 1);
+      n += 1 + put_dec<W>((uint64_t)(a.offsets[f] + id), o + n + 1);
       if (W) { o[n] = ':'; o[n + 1] = '1'; }
       n += 2;
     }
@@ -269,12 +244,12 @@ __global__ void __launch_bounds__(CF_THREADS) cf_stats_kernel(const unsigned cha
   __shared__ long long smin[CF_NI], smax[CF_NI];
   if (threadIdx.x < CF_NI) { smin[threadIdx.x] = CF_MAXSIZE; smax[threadIdx.x] = -CF_MAXSIZE; }
   __syncthreads();
-  const int64_t nn = n_newlines[0], n_lines = cf_n_lines(t, len, nn);
+  const int64_t nn = n_newlines[0], n_lines = chunk_lines(t, len, nn);
   if (blockIdx.x == 0 && threadIdx.x == 0) info[0] = n_lines;
   for (int64_t row = (int64_t)blockIdx.x * CF_THREADS + threadIdx.x; row < n_lines;
        row += (int64_t)gridDim.x * CF_THREADS) {
     int64_t p, e;
-    cf_line(t, len, line_start, nn, row, p, e);
+    line_bounds(line_start, nn, len, row, p, e);
     const int64_t line = line_base + row;
     uint64_t err = ~0ull;
     int col = 0;
@@ -313,43 +288,6 @@ __global__ void __launch_bounds__(CF_THREADS) cf_stats_kernel(const unsigned cha
   }
 }
 
-// exclusive scan of a[0, *count) in place (one CTA, tiles of 1024); total -> *total
-template <typename T>
-__global__ void __launch_bounds__(1024) cf_scan_kernel(T* __restrict__ a, const int64_t* __restrict__ count,
-                                                       int64_t* __restrict__ total) {
-  __shared__ int64_t warp_sum_s[32];
-  __shared__ int64_t carry_s;
-  const int64_t n = count[0];
-  if (threadIdx.x == 0) carry_s = 0;
-  __syncthreads();
-  for (int64_t base = 0; base < n; base += 1024) {
-    const int64_t i = base + threadIdx.x;
-    const int64_t v = i < n ? (int64_t)a[i] : 0;
-    int64_t x = v;
-    for (int o = 1; o < 32; o <<= 1) {
-      const int64_t y = __shfl_up_sync(FULL_MASK, x, o);
-      if ((threadIdx.x & 31) >= o) x += y;
-    }
-    if ((threadIdx.x & 31) == 31) warp_sum_s[threadIdx.x >> 5] = x;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-      int64_t w = warp_sum_s[threadIdx.x];
-      for (int o = 1; o < 32; o <<= 1) {
-        const int64_t y = __shfl_up_sync(FULL_MASK, w, o);
-        if (threadIdx.x >= o) w += y;
-      }
-      warp_sum_s[threadIdx.x] = w;
-    }
-    __syncthreads();
-    const int64_t before = carry_s + (threadIdx.x >= 32 ? warp_sum_s[(threadIdx.x >> 5) - 1] : 0) + (x - v);
-    if (i < n) a[i] = (T)before;
-    __syncthreads();
-    if (threadIdx.x == 1023) carry_s = before + v;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0 && total) total[0] = carry_s;
-}
-
 // CTA-wide exclusive scan of two int64 values (CF_THREADS threads); returns the CTA totals through s_a / s_b
 __device__ __forceinline__ void cf_block_scan2(int64_t& a, int64_t& b, int64_t& s_a, int64_t& s_b) {
   __shared__ int64_t wa[CF_THREADS / 32], wb[CF_THREADS / 32];
@@ -380,7 +318,7 @@ __global__ void __launch_bounds__(CF_THREADS) cf_plan_kernel(const unsigned char
                                                             int32_t* __restrict__ line_len, int64_t* __restrict__ tile_tr,
                                                             int64_t* __restrict__ tile_va, int64_t* __restrict__ tile_trn,
                                                             int64_t* __restrict__ n_tiles, int64_t* __restrict__ info) {
-  const int64_t nn = n_newlines[0], n_lines = cf_n_lines(t, len, nn);
+  const int64_t nn = n_newlines[0], n_lines = chunk_lines(t, len, nn);
   if (blockIdx.x == 0 && threadIdx.x == 0) { info[0] = n_lines; n_tiles[0] = (n_lines + CF_THREADS - 1) / CF_THREADS; }
   for (int64_t tile = blockIdx.x; tile * CF_THREADS < n_lines; tile += gridDim.x) {
     const int64_t row = tile * CF_THREADS + threadIdx.x;
@@ -388,7 +326,7 @@ __global__ void __launch_bounds__(CF_THREADS) cf_plan_kernel(const unsigned char
     bool tr = true;
     if (row < n_lines) {
       int64_t p, e;
-      cf_line(t, len, line_start, nn, row, p, e);
+      line_bounds(line_start, nn, len, row, p, e);
       uint64_t err = ~0ull;
       L = cf_emit_line<false>(t, p, e, a, line_base + row, err, nullptr);
       if (err != ~0ull) atomicMin(reinterpret_cast<unsigned long long*>(&info[1]), (unsigned long long)err);
@@ -410,7 +348,7 @@ __global__ void __launch_bounds__(CF_THREADS) cf_write_kernel(const unsigned cha
                                                              const int64_t* __restrict__ tile_tr,
                                                              const int64_t* __restrict__ tile_va, char* __restrict__ out_tr,
                                                              char* __restrict__ out_va) {
-  const int64_t nn = n_newlines[0], n_lines = cf_n_lines(t, len, nn);
+  const int64_t nn = n_newlines[0], n_lines = chunk_lines(t, len, nn);
   for (int64_t tile = blockIdx.x; tile * CF_THREADS < n_lines; tile += gridDim.x) {
     const int64_t row = tile * CF_THREADS + threadIdx.x;
     const bool live = row < n_lines, tr = !live || a.test || to_train[row];
@@ -419,7 +357,7 @@ __global__ void __launch_bounds__(CF_THREADS) cf_write_kernel(const unsigned cha
     cf_block_scan2(x_tr, x_va, s_tr, s_va);
     if (live) {
       int64_t p, e;
-      cf_line(t, len, line_start, nn, row, p, e);
+      line_bounds(line_start, nn, len, row, p, e);
       uint64_t err = ~0ull;
       char* o = tr ? out_tr + tile_tr[tile] + x_tr : out_va + tile_va[tile] + x_va;
       cf_emit_line<true>(t, p, e, a, row, err, o);
@@ -428,9 +366,6 @@ __global__ void __launch_bounds__(CF_THREADS) cf_write_kernel(const unsigned cha
 }
 
 // ---- vocabulary ----------------------------------------------------------------------------------------------
-constexpr int VC_TILE = 16 * CF_THREADS;   // items per CTA in the radix passes
-constexpr int VC_PASSES = 13;              // 8 digits of the key, then 5 of (field << 32 | ~count)
-
 // kept slots -> (lo = key, hi = field << 32 | ~count, slot); vals are cleared to the <unk> id 0
 __global__ void __launch_bounds__(CF_THREADS) vc_compact_kernel(CfTable T, int64_t cutoff, uint64_t* __restrict__ lo,
                                                                uint64_t* __restrict__ hi, uint32_t* __restrict__ sl,
@@ -470,70 +405,14 @@ __global__ void __launch_bounds__(CF_THREADS) vc_compact_kernel(CfTable T, int64
     atomicAdd(reinterpret_cast<unsigned long long*>(&field_counts[threadIdx.x]), (unsigned long long)cnt[threadIdx.x]);
 }
 
-__device__ __forceinline__ int vc_digit(uint64_t lo, uint64_t hi, int pass) {
-  return (int)(((pass < 8 ? lo >> (8 * pass) : hi >> (8 * (pass - 8)))) & 0xFF);
-}
-
-// hist[d * nb + b] = items of CTA b with digit d; nb = ceil(n / VC_TILE)
-__global__ void __launch_bounds__(CF_THREADS) vc_hist_kernel(const uint64_t* __restrict__ lo, const uint64_t* __restrict__ hi,
-                                                            const int64_t* __restrict__ n_kept, int pass,
-                                                            int32_t* __restrict__ hist, int64_t* __restrict__ hist_count) {
-  __shared__ int h[256];
-  const int64_t n = n_kept[0], nb = (n + VC_TILE - 1) / VC_TILE;
-  if (blockIdx.x == 0 && threadIdx.x == 0) hist_count[0] = 256 * nb;
-  if (blockIdx.x >= nb) return;
-  h[threadIdx.x] = 0;
-  __syncthreads();
-  for (int r = 0; r < VC_TILE / CF_THREADS; ++r) {
-    const int64_t i = (int64_t)blockIdx.x * VC_TILE + r * CF_THREADS + threadIdx.x;
-    if (i < n) atomicAdd(&h[vc_digit(lo[i], hi[i], pass)], 1);
-  }
-  __syncthreads();
-  hist[(int64_t)threadIdx.x * nb + blockIdx.x] = h[threadIdx.x];
-}
-
-// stable scatter by digit: within a CTA the items go in index order (warp match + per-warp digit counts)
-__global__ void __launch_bounds__(CF_THREADS) vc_scatter_kernel(const uint64_t* __restrict__ lo, const uint64_t* __restrict__ hi,
-                                                               const uint32_t* __restrict__ sl,
-                                                               const int64_t* __restrict__ n_kept, int pass,
-                                                               const int32_t* __restrict__ hist, uint64_t* __restrict__ lo2,
-                                                               uint64_t* __restrict__ hi2, uint32_t* __restrict__ sl2) {
-  constexpr int NW = CF_THREADS / 32;
-  __shared__ int base[256];
-  __shared__ int wcnt[NW][256];
-  const int64_t n = n_kept[0], nb = (n + VC_TILE - 1) / VC_TILE;
-  if (blockIdx.x >= nb) return;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  base[threadIdx.x] = hist[(int64_t)threadIdx.x * nb + blockIdx.x];
-  for (int w = 0; w < NW; ++w) wcnt[w][threadIdx.x] = 0;
-  __syncthreads();
-  for (int r = 0; r < VC_TILE / CF_THREADS; ++r) {
-    const int64_t i = (int64_t)blockIdx.x * VC_TILE + r * CF_THREADS + threadIdx.x;
-    const bool live = i < n;
-    uint64_t l = 0, h = 0;
-    uint32_t s = 0;
-    int d = 256;   // no digit: dead lanes match only each other and are not counted
-    if (live) { l = lo[i]; h = hi[i]; s = sl[i]; d = vc_digit(l, h, pass); }
-    const uint32_t peers = __match_any_sync(FULL_MASK, d);
-    const int rank = __popc(peers & ((1u << lane) - 1));
-    if (live && rank == 0) wcnt[warp][d] = __popc(peers);
-    __syncthreads();
-    if (live) {
-      int pos = base[d] + rank;
-      for (int w = 0; w < warp; ++w) pos += wcnt[w][d];
-      lo2[pos] = l; hi2[pos] = h; sl2[pos] = s;
-    }
-    __syncthreads();
-    int add = 0;
-    for (int w = 0; w < NW; ++w) { add += wcnt[w][threadIdx.x]; wcnt[w][threadIdx.x] = 0; }
-    base[threadIdx.x] += add;
-    __syncthreads();
-  }
-}
-
-// sorted position p of field f -> id p - start(f) + 1, written into the slot; keys -> vocab_keys
-__global__ void __launch_bounds__(CF_THREADS) vc_assign_kernel(CfTable T, const uint64_t* __restrict__ lo,
-                                                              const uint64_t* __restrict__ hi, const uint32_t* __restrict__ sl,
+// The kept items in (hi, lo) order: hi_s = the sorted hi words, lo_s = the lo words sorted alone, order[p] = the
+// position in lo_s of sorted item p, by_lo[q] = the compaction index of lo_s[q].  Sorted position p of field f ->
+// id p - start(f) + 1, written into the item's slot; its key -> vocab_keys[p]
+__global__ void __launch_bounds__(CF_THREADS) vc_assign_kernel(CfTable T, const uint64_t* __restrict__ lo_s,
+                                                              const uint64_t* __restrict__ hi_s,
+                                                              const uint32_t* __restrict__ sl,
+                                                              const uint32_t* __restrict__ by_lo,
+                                                              const uint32_t* __restrict__ order,
                                                               const int64_t* __restrict__ n_kept,
                                                               const int64_t* __restrict__ field_counts,
                                                               uint64_t* __restrict__ vocab_keys) {
@@ -545,68 +424,51 @@ __global__ void __launch_bounds__(CF_THREADS) vc_assign_kernel(CfTable T, const 
   __syncthreads();
   const int64_t n = n_kept[0];
   for (int64_t p = (int64_t)blockIdx.x * CF_THREADS + threadIdx.x; p < n; p += (int64_t)gridDim.x * CF_THREADS) {
-    const int f = (int)(hi[p] >> 32);
-    T.vals[sl[p]] = (uint32_t)(p - start[f] + 1);
-    vocab_keys[p] = lo[p];
+    const int f = (int)(hi_s[p] >> 32);
+    const uint32_t q = order[p];
+    T.vals[sl[by_lo[q]]] = (uint32_t)(p - start[f] + 1);
+    vocab_keys[p] = lo_s[q];
   }
 }
 
 // ---- workspace layouts -----------------------------------------------------------------------------------------
-static inline size_t cf_align(size_t x) { return (x + 255) & ~(size_t)255; }
-
-// line starts of a chunk: block_counts int32[nb] | n_newlines int64[2] | line_start int64[len + 2]
-struct CfLines {
-  int32_t* block_counts;
-  int64_t* n_newlines;
-  int64_t* line_start;
-  int n_blocks;
-  size_t bytes;
-  CfLines(void* ws, size_t len) {
-    uint8_t* b = reinterpret_cast<uint8_t*>(ws);
-    n_blocks = (int)((len + LS_BLOCK_BYTES - 1) / LS_BLOCK_BYTES);
-    size_t o = 0;
-    block_counts = reinterpret_cast<int32_t*>(b + o); o += cf_align((size_t)n_blocks * 4);
-    n_newlines = reinterpret_cast<int64_t*>(b + o); o += cf_align(16);
-    line_start = reinterpret_cast<int64_t*>(b + o); o += cf_align((len + 2) * 8);
-    bytes = o;
-  }
-};
-
-// emit: CfLines | line_len int32[len + 1] | tile_tr, tile_va, tile_trn int64[nt] | n_tiles int64[2]
-struct CfEmitWs {
-  CfLines lines;
+// emit: LineStarts (max_rows = len + 1) | line_len int32[len + 1] | tile_tr, tile_va, tile_trn int64[nt] |
+// n_tiles int64[2]
+struct CfEmitWs : LineStarts {
   int32_t* line_len;
   int64_t *tile_tr, *tile_va, *tile_trn, *n_tiles;
-  size_t bytes;
-  CfEmitWs(void* ws, size_t len) : lines(ws, len) {
+  CfEmitWs(void* ws, size_t len) : LineStarts(ws, len, (int64_t)len + 1) {
     uint8_t* b = reinterpret_cast<uint8_t*>(ws);
     const size_t nt = (len + 1 + CF_THREADS - 1) / CF_THREADS;
-    size_t o = lines.bytes;
-    line_len = reinterpret_cast<int32_t*>(b + o); o += cf_align((len + 1) * 4);
-    tile_tr = reinterpret_cast<int64_t*>(b + o); o += cf_align(nt * 8);
-    tile_va = reinterpret_cast<int64_t*>(b + o); o += cf_align(nt * 8);
-    tile_trn = reinterpret_cast<int64_t*>(b + o); o += cf_align(nt * 8);
-    n_tiles = reinterpret_cast<int64_t*>(b + o); o += cf_align(16);
+    size_t o = bytes;
+    line_len = reinterpret_cast<int32_t*>(b + o); o += align256((len + 1) * 4);
+    tile_tr = reinterpret_cast<int64_t*>(b + o); o += align256(nt * 8);
+    tile_va = reinterpret_cast<int64_t*>(b + o); o += align256(nt * 8);
+    tile_trn = reinterpret_cast<int64_t*>(b + o); o += align256(nt * 8);
+    n_tiles = reinterpret_cast<int64_t*>(b + o); o += align256(16);
     bytes = o;
   }
 };
 
-// vocab: n_kept, hist_count int64 | hist int32[256 * nb] | lo, hi uint64[2][cap] | sl uint32[2][cap]
+// vocab: n_kept, hist_count int64 | hist int32[256 * nb] | lo, hi, keys2 uint64[cap] | sl, by_lo, order, perm2
+// uint32[cap] (one aligned block, so that the whole stays within 40 B per slot)
 struct CfVocabWs {
   int64_t *n_kept, *hist_count;
   int32_t* hist;
-  uint64_t *lo[2], *hi[2];
-  uint32_t* sl[2];
+  uint64_t *lo, *hi, *keys2;
+  uint32_t *sl, *by_lo, *order, *perm2;
   size_t bytes;
   CfVocabWs(void* ws, int64_t cap) {
     uint8_t* b = reinterpret_cast<uint8_t*>(ws);
-    const size_t nb = (size_t)ceil_div64(cap, VC_TILE), c = (size_t)cap;
+    const size_t nb = (size_t)ceil_div64(cap, LSD_TILE), c = (size_t)cap;
     size_t o = 0;
-    n_kept = reinterpret_cast<int64_t*>(b + o); hist_count = n_kept + 1; o += cf_align(16);
-    hist = reinterpret_cast<int32_t*>(b + o); o += cf_align(256 * nb * 4);
-    for (int k = 0; k < 2; ++k) { lo[k] = reinterpret_cast<uint64_t*>(b + o); o += cf_align(c * 8); }
-    for (int k = 0; k < 2; ++k) { hi[k] = reinterpret_cast<uint64_t*>(b + o); o += cf_align(c * 8); }
-    for (int k = 0; k < 2; ++k) { sl[k] = reinterpret_cast<uint32_t*>(b + o); o += cf_align(c * 4); }
+    n_kept = reinterpret_cast<int64_t*>(b + o); hist_count = n_kept + 1; o += align256(16);
+    hist = reinterpret_cast<int32_t*>(b + o); o += align256(256 * nb * 4);
+    lo = reinterpret_cast<uint64_t*>(b + o); o += align256(c * 8);
+    hi = reinterpret_cast<uint64_t*>(b + o); o += align256(c * 8);
+    keys2 = reinterpret_cast<uint64_t*>(b + o); o += align256(c * 8);
+    sl = reinterpret_cast<uint32_t*>(b + o); by_lo = sl + c; order = by_lo + c; perm2 = order + c;
+    o += align256(c * 16);
     bytes = o;
   }
 };
@@ -614,21 +476,6 @@ struct CfVocabWs {
 // chunk buffers the per-line kernels accept: len < 2^30 keeps block offsets and line lengths in int32
 constexpr size_t CF_MAX_LEN = (size_t)1 << 30;
 constexpr int64_t CF_MAX_CAP = (int64_t)1 << 31;   // slot numbers are uint32, sort positions int32
-
-static int cf_line_starts(const unsigned char* t, size_t len, const CfLines& L, cudaStream_t st, const char* what) {
-  ls_count_kernel<<<L.n_blocks, LS_THREADS, 0, st>>>(t, (int64_t)len, L.block_counts);
-  CTR_LAUNCHED(what);
-  ls_scan_kernel<<<1, 1024, 0, st>>>(L.block_counts, L.n_blocks, L.n_newlines);
-  CTR_LAUNCHED(what);
-  ls_emit_kernel<<<L.n_blocks, LS_THREADS, 0, st>>>(t, (int64_t)len, L.block_counts, (int64_t)len + 1, L.line_start);
-  CTR_LAUNCHED(what);
-  return CTR_OK;
-}
-
-static unsigned cf_grid(int64_t items) {
-  const int64_t want = ceil_div64(items, CF_THREADS), cap = (int64_t)sm_count() * 16;
-  return (unsigned)(want < 1 ? 1 : (want < cap ? want : cap));
-}
 
 }  // namespace ctr
 
@@ -638,7 +485,7 @@ extern "C" {
 
 size_t ctr_criteo_table_bytes(int64_t capacity) { return capacity > 0 ? (size_t)capacity * 16 : 0; }
 
-size_t ctr_criteo_stats_workspace_bytes(size_t len) { return CfLines(nullptr, len).bytes; }
+size_t ctr_criteo_stats_workspace_bytes(size_t len) { return LineStarts(nullptr, len, (int64_t)len + 1).bytes; }
 
 int ctr_criteo_stats(const char* text, size_t len, int64_t line_base, void* table, int64_t capacity, int64_t* minmax,
                      int64_t* info, void* ws, size_t ws_bytes, ctr_stream_t stream) {
@@ -654,10 +501,10 @@ int ctr_criteo_stats(const char* text, size_t len, int64_t line_base, void* tabl
               CTR_ERR_CUDA, "ctr_criteo_stats: memset failed");
   if (len == 0) return CTR_OK;
   const unsigned char* t = reinterpret_cast<const unsigned char*>(text);
-  CfLines L(ws, len);
-  if (int rc = cf_line_starts(t, len, L, st, "ctr_criteo_stats(lines)")) return rc;
-  cf_stats_kernel<<<cf_grid((int64_t)len + 1), CF_THREADS, 0, st>>>(t, (int64_t)len, L.line_start, L.n_newlines,
-                                                                    line_base, CfTable(table, capacity), minmax, info);
+  const LineStarts L(ws, len, (int64_t)len + 1);
+  if (int rc = L.launch(t, len, st, "ctr_criteo_stats(lines)")) return rc;
+  cf_stats_kernel<<<grid_for((int64_t)len + 1, CF_THREADS, 16), CF_THREADS, 0, st>>>(
+      t, (int64_t)len, L.line_start, L.n_newlines, line_base, CfTable(table, capacity), minmax, info);
   CTR_LAUNCHED("ctr_criteo_stats");
   return CTR_OK;
 }
@@ -678,22 +525,27 @@ int ctr_criteo_vocab(void* table, int64_t capacity, int64_t cutoff, uint64_t* vo
   CTR_REQUIRE(cudaMemsetAsync(V.n_kept, 0, 16, st) == cudaSuccess &&
                   cudaMemsetAsync(field_counts, 0, CF_NC * sizeof(int64_t), st) == cudaSuccess,
               CTR_ERR_CUDA, "ctr_criteo_vocab: memset failed");
-  vc_compact_kernel<<<cf_grid(capacity), CF_THREADS, 0, st>>>(T, cutoff, V.lo[0], V.hi[0], V.sl[0], V.n_kept,
-                                                             field_counts);
+  const unsigned g = grid_for(capacity, CF_THREADS, 16);
+  vc_compact_kernel<<<g, CF_THREADS, 0, st>>>(T, cutoff, V.lo, V.hi, V.sl, V.n_kept, field_counts);
   CTR_LAUNCHED("ctr_criteo_vocab(compact)");
-  const unsigned nb = (unsigned)ceil_div64(capacity, VC_TILE);
-  int cur = 0;
-  for (int pass = 0; pass < VC_PASSES; ++pass, cur ^= 1) {
-    vc_hist_kernel<<<nb, CF_THREADS, 0, st>>>(V.lo[cur], V.hi[cur], V.n_kept, pass, V.hist, V.hist_count);
-    CTR_LAUNCHED("ctr_criteo_vocab(hist)");
-    cf_scan_kernel<int32_t><<<1, 1024, 0, st>>>(V.hist, V.hist_count, nullptr);
-    CTR_LAUNCHED("ctr_criteo_vocab(scan)");
-    vc_scatter_kernel<<<nb, CF_THREADS, 0, st>>>(V.lo[cur], V.hi[cur], V.sl[cur], V.n_kept, pass, V.hist,
-                                                 V.lo[cur ^ 1], V.hi[cur ^ 1], V.sl[cur ^ 1]);
-    CTR_LAUNCHED("ctr_criteo_vocab(scatter)");
-  }
-  vc_assign_kernel<<<cf_grid(capacity), CF_THREADS, 0, st>>>(T, V.lo[cur], V.hi[cur], V.sl[cur], V.n_kept, field_counts,
-                                                            vocab_keys);
+  // (hi, lo) order from two stable sorts over the 13 digits of the 104 key bits: lo in place (8 passes, so the result
+  // is back in lo / by_lo) carrying the compaction index, then hi gathered into that order and sorted (5 passes, hi's
+  // own buffer as scratch) carrying the lo-sorted position
+  lsd_iota_kernel<<<g, CF_THREADS, 0, st>>>(V.by_lo, V.n_kept);
+  CTR_LAUNCHED("ctr_criteo_vocab(iota)");
+  uint64_t *lo_s, *hi_s;
+  uint32_t *by_lo, *order;
+  if (int rc = lsd_sort(V.lo, V.by_lo, V.keys2, V.perm2, V.n_kept, capacity, 8, V.hist, V.hist_count, st,
+                        "ctr_criteo_vocab(sort)", &lo_s, &by_lo))
+    return rc;
+  lsd_gather_kernel<<<g, CF_THREADS, 0, st>>>(V.hi, by_lo, V.n_kept, V.keys2);
+  CTR_LAUNCHED("ctr_criteo_vocab(gather)");
+  lsd_iota_kernel<<<g, CF_THREADS, 0, st>>>(V.order, V.n_kept);
+  CTR_LAUNCHED("ctr_criteo_vocab(iota)");
+  if (int rc = lsd_sort(V.keys2, V.order, V.hi, V.perm2, V.n_kept, capacity, 5, V.hist, V.hist_count, st,
+                        "ctr_criteo_vocab(sort)", &hi_s, &order))
+    return rc;
+  vc_assign_kernel<<<g, CF_THREADS, 0, st>>>(T, lo_s, hi_s, V.sl, by_lo, order, V.n_kept, field_counts, vocab_keys);
   CTR_LAUNCHED("ctr_criteo_vocab(assign)");
   return CTR_OK;
 }
@@ -726,17 +578,17 @@ int ctr_criteo_emit_plan(const char* text, size_t len, int test, int64_t line_ba
               CTR_ERR_CUDA, "ctr_criteo_emit_plan: memset failed");
   if (len == 0) return CTR_OK;
   const unsigned char* t = reinterpret_cast<const unsigned char*>(text);
-  CfEmitWs E(ws, len);
-  if (int rc = cf_line_starts(t, len, E.lines, st, "ctr_criteo_emit_plan(lines)")) return rc;
-  cf_plan_kernel<<<cf_grid((int64_t)len + 1), CF_THREADS, 0, st>>>(t, (int64_t)len, E.lines.line_start,
-                                                                   E.lines.n_newlines, line_base, to_train, a, E.line_len,
-                                                                   E.tile_tr, E.tile_va, E.tile_trn, E.n_tiles, info);
+  const CfEmitWs E(ws, len);
+  if (int rc = E.launch(t, len, st, "ctr_criteo_emit_plan(lines)")) return rc;
+  cf_plan_kernel<<<grid_for((int64_t)len + 1, CF_THREADS, 16), CF_THREADS, 0, st>>>(
+      t, (int64_t)len, E.line_start, E.n_newlines, line_base, to_train, a, E.line_len, E.tile_tr, E.tile_va, E.tile_trn,
+      E.n_tiles, info);
   CTR_LAUNCHED("ctr_criteo_emit_plan");
-  cf_scan_kernel<int64_t><<<1, 1024, 0, st>>>(E.tile_tr, E.n_tiles, info + 3);
+  cta_scan_kernel<int64_t><<<1, 1024, 0, st>>>(E.tile_tr, E.n_tiles, 0, info + 3);
   CTR_LAUNCHED("ctr_criteo_emit_plan(scan)");
-  cf_scan_kernel<int64_t><<<1, 1024, 0, st>>>(E.tile_va, E.n_tiles, info + 4);
+  cta_scan_kernel<int64_t><<<1, 1024, 0, st>>>(E.tile_va, E.n_tiles, 0, info + 4);
   CTR_LAUNCHED("ctr_criteo_emit_plan(scan)");
-  cf_scan_kernel<int64_t><<<1, 1024, 0, st>>>(E.tile_trn, E.n_tiles, info + 2);
+  cta_scan_kernel<int64_t><<<1, 1024, 0, st>>>(E.tile_trn, E.n_tiles, 0, info + 2);
   CTR_LAUNCHED("ctr_criteo_emit_plan(scan)");
   return CTR_OK;
 }
@@ -753,8 +605,8 @@ int ctr_criteo_emit_write(const char* text, size_t len, int test, const uint8_t*
   if (int rc = cf_emit_args(table, capacity, num_min, num_den, offsets, label, label_len, test, a)) return rc;
   if (len == 0) return CTR_OK;
   CfEmitWs E(const_cast<void*>(ws), len);
-  cf_write_kernel<<<cf_grid((int64_t)len + 1), CF_THREADS, 0, as_stream(stream)>>>(
-      reinterpret_cast<const unsigned char*>(text), (int64_t)len, E.lines.line_start, E.lines.n_newlines, to_train, a,
+  cf_write_kernel<<<grid_for((int64_t)len + 1, CF_THREADS, 16), CF_THREADS, 0, as_stream(stream)>>>(
+      reinterpret_cast<const unsigned char*>(text), (int64_t)len, E.line_start, E.n_newlines, to_train, a,
       E.line_len, E.tile_tr, E.tile_va, out_tr, out_va);
   CTR_LAUNCHED("ctr_criteo_emit_write");
   return CTR_OK;

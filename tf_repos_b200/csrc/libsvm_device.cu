@@ -141,8 +141,7 @@ using namespace ctr;
 extern "C" {
 
 size_t ctr_parse_libsvm_device_workspace_bytes(size_t len, int64_t max_rows) {
-  const size_t n_blocks = (len + LS_BLOCK_BYTES - 1) / LS_BLOCK_BYTES;
-  return n_blocks * sizeof(int32_t) + 16 + (size_t)(max_rows + 1) * sizeof(int64_t) + 16;
+  return LineStarts(nullptr, len, max_rows).bytes;
 }
 
 int ctr_parse_libsvm_device(const char* text, size_t len, int F, int64_t max_rows, int final_chunk, int32_t* ids,
@@ -157,19 +156,11 @@ int ctr_parse_libsvm_device(const char* text, size_t len, int F, int64_t max_row
   CTR_REQUIRE(cudaMemsetAsync(info, 0, 5 * sizeof(int64_t), st) == cudaSuccess, CTR_ERR_CUDA,
               "ctr_parse_libsvm_device: memset failed");
   if (len == 0 || max_rows == 0) return CTR_OK;
-  const int n_blocks = (int)((len + LS_BLOCK_BYTES - 1) / LS_BLOCK_BYTES);
-  int32_t* block_counts = reinterpret_cast<int32_t*>(ws);
-  int64_t* n_newlines = reinterpret_cast<int64_t*>(reinterpret_cast<uint8_t*>(ws) + (((size_t)n_blocks * 4 + 15) & ~(size_t)15));
-  int64_t* line_start = n_newlines + 2;
   const unsigned char* t = reinterpret_cast<const unsigned char*>(text);
-  ls_count_kernel<<<n_blocks, LS_THREADS, 0, st>>>(t, (int64_t)len, block_counts);
-  CTR_LAUNCHED("ctr_parse_libsvm_device(count)");
-  ls_scan_kernel<<<1, 1024, 0, st>>>(block_counts, n_blocks, n_newlines);
-  CTR_LAUNCHED("ctr_parse_libsvm_device(scan)");
-  ls_emit_kernel<<<n_blocks, LS_THREADS, 0, st>>>(t, (int64_t)len, block_counts, max_rows, line_start);
-  CTR_LAUNCHED("ctr_parse_libsvm_device(emit)");
-  ls_parse_kernel<<<(unsigned)ceil_div64(max_rows, 128), 128, 0, st>>>(t, (int64_t)len, line_start, n_newlines, max_rows, F,
-                                                                       final_chunk, ids, vals, labels, info);
+  const LineStarts L(ws, len, max_rows);
+  if (int rc = L.launch(t, len, st, "ctr_parse_libsvm_device(lines)")) return rc;
+  ls_parse_kernel<<<(unsigned)ceil_div64(max_rows, 128), 128, 0, st>>>(
+      t, (int64_t)len, L.line_start, L.n_newlines, max_rows, F, final_chunk, ids, vals, labels, info);
   CTR_LAUNCHED("ctr_parse_libsvm_device(parse)");
   return CTR_OK;
 }

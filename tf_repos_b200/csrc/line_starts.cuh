@@ -1,10 +1,12 @@
 // line_starts.cuh -- line starts of a text buffer in device memory, shared by the tokenizers
-// (libsvm_device.cu, criteo_feature.cu).
+// (libsvm_device.cu, criteo_feature.cu, aliccp_tfrecord.cu, aliccp_sample.cu).
 //
-// Kernels: (1) count '\n' per 4 KB block; (2) scan the block counts; (3) emit line starts.
+// Kernels: (1) count '\n' per 4 KB block; (2) scan the block counts (cta_scan_kernel); (3) emit line starts.
+// LineStarts is their workspace and launches them; line_bounds / chunk_lines read the result in the per-line kernels.
 // They live in an anonymous namespace so that every translation unit that includes this header owns its copy.
 #pragma once
 #include "common.cuh"
+#include "scan_sort.cuh"
 
 namespace ctr {
 namespace {
@@ -45,42 +47,6 @@ __global__ void __launch_bounds__(LS_THREADS) ls_count_kernel(const unsigned cha
   }
 }
 
-// exclusive scan of block_counts (one CTA, sequential over tiles of 1024); total -> info_lines[0]
-__global__ void __launch_bounds__(1024) ls_scan_kernel(int32_t* __restrict__ block_counts, int n_blocks,
-                                                       int64_t* __restrict__ n_newlines) {
-  __shared__ int64_t warp_sum_s[32];
-  __shared__ int64_t carry_s;
-  if (threadIdx.x == 0) carry_s = 0;
-  __syncthreads();
-  for (int base = 0; base < n_blocks; base += 1024) {
-    const int i = base + threadIdx.x;
-    const int64_t v = i < n_blocks ? block_counts[i] : 0;
-    int64_t x = v;
-    for (int o = 1; o < 32; o <<= 1) {
-      const int64_t y = __shfl_up_sync(FULL_MASK, x, o);
-      if ((threadIdx.x & 31) >= o) x += y;
-    }
-    if ((threadIdx.x & 31) == 31) warp_sum_s[threadIdx.x >> 5] = x;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-      int64_t w = warp_sum_s[threadIdx.x];
-      for (int o = 1; o < 32; o <<= 1) {
-        const int64_t y = __shfl_up_sync(FULL_MASK, w, o);
-        if (threadIdx.x >= o) w += y;
-      }
-      warp_sum_s[threadIdx.x] = w;   // inclusive over warps
-    }
-    __syncthreads();
-    const int64_t before = carry_s + (threadIdx.x >= 32 ? warp_sum_s[(threadIdx.x >> 5) - 1] : 0) + (x - v);
-    // block counts are < 2^31 in total for any buffer this API accepts (len < 2^31 * 1 byte per newline)
-    if (i < n_blocks) block_counts[i] = (int32_t)before;
-    __syncthreads();
-    if (threadIdx.x == 1023) carry_s = before + v;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) n_newlines[0] = carry_s;
-}
-
 // line_start[k+1] = position just after the k-th '\n' (k < max_rows); line_start[0] = 0
 __global__ void __launch_bounds__(LS_THREADS) ls_emit_kernel(const unsigned char* __restrict__ text, int64_t len,
                                                             const int32_t* __restrict__ block_offsets, int64_t max_rows,
@@ -107,6 +73,51 @@ __global__ void __launch_bounds__(LS_THREADS) ls_emit_kernel(const unsigned char
     ++k;
   }
 }
+
+// line `row` of the chunk: [p, e), '\n' dropped (the last line of the chunk may have none)
+__device__ __forceinline__ void line_bounds(const int64_t* line_start, int64_t nn, int64_t len, int64_t row,
+                                            int64_t& p, int64_t& e) {
+  p = line_start[row];
+  e = row < nn ? line_start[row + 1] - 1 : len;
+}
+
+// lines of the chunk, nn = its '\n' count: an unterminated last line counts; at most cap
+__device__ __forceinline__ int64_t chunk_lines(const uint8_t* __restrict__ t, int64_t len, int64_t nn,
+                                               int64_t cap = INT64_MAX) {
+  const int64_t n = nn + ((len > 0 && t[len - 1] != '\n') ? 1 : 0);
+  return n < cap ? n : cap;
+}
+
+// Workspace of a chunk of len bytes: block_counts int32[nb] | n_newlines int64[2] | line_start int64[max_rows + 1],
+// each 256-B aligned; bytes = its end, where a caller's own arrays may follow.
+struct LineStarts {
+  int32_t* block_counts;
+  int64_t *n_newlines, *line_start;
+  int64_t max_rows;
+  int n_blocks;
+  size_t bytes;
+  LineStarts(void* ws, size_t len, int64_t rows) : max_rows(rows) {
+    uint8_t* b = reinterpret_cast<uint8_t*>(ws);
+    n_blocks = (int)((len + LS_BLOCK_BYTES - 1) / LS_BLOCK_BYTES);
+    size_t o = 0;
+    block_counts = reinterpret_cast<int32_t*>(b + o); o += align256((size_t)n_blocks * 4);
+    n_newlines = reinterpret_cast<int64_t*>(b + o); o += align256(16);
+    line_start = reinterpret_cast<int64_t*>(b + o); o += align256((size_t)(max_rows + 1) * 8);
+    bytes = o;
+  }
+
+  // n_newlines[0] = the '\n' count of text[0, len); line_start[0] = 0 and line_start[k + 1] = the position after the
+  // k-th '\n' for k < max_rows
+  int launch(const uint8_t* t, size_t len, cudaStream_t st, const char* what) const {
+    ls_count_kernel<<<n_blocks, LS_THREADS, 0, st>>>(t, (int64_t)len, block_counts);
+    CTR_LAUNCHED(what);
+    cta_scan_kernel<int32_t><<<1, 1024, 0, st>>>(block_counts, nullptr, n_blocks, n_newlines);
+    CTR_LAUNCHED(what);
+    ls_emit_kernel<<<n_blocks, LS_THREADS, 0, st>>>(t, (int64_t)len, block_counts, max_rows, line_start);
+    CTR_LAUNCHED(what);
+    return CTR_OK;
+  }
+};
 
 }  // namespace
 }  // namespace ctr

@@ -327,11 +327,6 @@ __global__ void __launch_bounds__(TR_THREADS) tr_emit_esmm_kernel(
   }
 }
 
-static unsigned tr_grid(int64_t items) {
-  const int64_t want = (items + TR_WARPS - 1) / TR_WARPS, cap = (int64_t)sm_count() * 16;
-  return (unsigned)(want < 1 ? 1 : (want < cap ? want : cap));
-}
-
 }  // namespace ctr
 
 using namespace ctr;
@@ -346,7 +341,7 @@ int ctr_tfrecord_scan(const void* chunk, size_t len, const int64_t* rec_off, int
   CTR_REQUIRE(record_base + n_rec < ((int64_t)1 << 47), CTR_ERR_INVALID_ARG, "ctr_tfrecord_scan: record index >= 2^47");
   (void)len;
   if (n_rec == 0) return CTR_OK;
-  tr_scan_kernel<<<tr_grid(n_rec), TR_THREADS, 0, as_stream(stream)>>>(
+  tr_scan_kernel<<<grid_for(n_rec, TR_WARPS, 16), TR_THREADS, 0, as_stream(stream)>>>(
       static_cast<const uint8_t*>(chunk), rec_off, n_rec, record_base, F, labels_mask, lens,
       reinterpret_cast<unsigned long long*>(err));
   CTR_LAUNCHED("ctr_tfrecord_scan");
@@ -359,7 +354,7 @@ int ctr_tfrecord_emit_din(const void* stage, const int64_t* slot_off, const int3
   CTR_REQUIRE(stage && slot_off && slot_len && B > 0 && F > 0 && P > 0 && a_int_off && feat_ids && a_ids && u_ids &&
                   u_wgt && y,
               CTR_ERR_INVALID_ARG, "ctr_tfrecord_emit_din: bad arguments");
-  tr_emit_din_kernel<<<tr_grid(B), TR_THREADS, 0, as_stream(stream)>>>(
+  tr_emit_din_kernel<<<grid_for(B, TR_WARPS, 16), TR_THREADS, 0, as_stream(stream)>>>(
       static_cast<const uint8_t*>(stage), slot_off, slot_len, B, F, P, a_int_off, feat_ids, a_ids, a_int_ids, u_ids,
       u_wgt, y);
   CTR_LAUNCHED("ctr_tfrecord_emit_din");
@@ -371,7 +366,7 @@ int ctr_tfrecord_emit_esmm(const void* stage, const int64_t* slot_off, const int
                            float* y, float* z, ctr_stream_t stream) {
   CTR_REQUIRE(stage && slot_off && slot_len && B > 0 && F > 0 && bag_off && feat_ids && a_ids && y && z,
               CTR_ERR_INVALID_ARG, "ctr_tfrecord_emit_esmm: bad arguments");
-  tr_emit_esmm_kernel<<<tr_grid(B), TR_THREADS, 0, as_stream(stream)>>>(
+  tr_emit_esmm_kernel<<<grid_for(B, TR_WARPS, 16), TR_THREADS, 0, as_stream(stream)>>>(
       static_cast<const uint8_t*>(stage), slot_off, slot_len, B, F, bag_off, feat_ids, a_ids, bag_ids, bag_wgt, y, z);
   CTR_LAUNCHED("ctr_tfrecord_emit_esmm");
   return CTR_OK;
