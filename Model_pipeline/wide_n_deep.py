@@ -29,6 +29,8 @@ flags.DEFINE_string("servable_model_dir", "", "export servable model for TensorF
 flags.DEFINE_string("task_type", "train", "task type {train, predict, export}")
 flags.DEFINE_string("model_type", "wide_n_deep", "model type {'wide', 'deep', 'wide_n_deep'}")
 flags.DEFINE_boolean("clear_existing_model", False, "clear existing model or not")
+# engine-only flag (not in the reference)
+flags.DEFINE_string("input_parse", "device", "{device, host}: where the CSV text is tokenised (same values)")
 
 
 def main():

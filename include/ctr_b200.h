@@ -491,6 +491,25 @@ size_t ctr_parse_libsvm_device_workspace_bytes(size_t len, int64_t max_rows);
 int ctr_parse_libsvm_device(const char* text, size_t len, int F, int64_t max_rows, int final_chunk, int32_t* ids,
                             float* vals, float* labels, int64_t* info, void* ws, size_t ws_bytes, ctr_stream_t stream);
 
+/* ---- wide_n_deep CSV input (DEVICE buffers; DESIGN.md §2.9) ------------------------------------------------
+ * The tf.decode_csv of input_fn (wide_n_deep.py:55-73; record_defaults [[0.0]] + 13*[[0.0]] + 26*[[0]]) for text that
+ * is already in device memory: the first max_rows complete lines of text[0,len) (plus an unterminated last line when
+ * final_chunk != 0) are split on ',' by one thread each into n_float float columns then n_int int columns; an empty
+ * field takes its default (0.0 / 0).  Column 0 = label, then n_float-1 dense, then n_int:
+ *   labels f32 [rows], dense f32 [rows, n_float-1], cat int32 [rows, n_int], row-major; ids are not clamped.
+ * Every value this path emits has exactly the bits wide_deep_main.decode_csv_file (Python float() / int(), NumPy cast)
+ * gives; whatever it cannot guarantee is only COUNTED and the caller re-parses the piece with the host decoder:
+ *   info (device int64[5]) = { rows, bytes consumed, blank lines, malformed lines (field count != n_float + n_int, or
+ *                             a '"', blank or tab in the line), lines holding a number for the host (a float outside
+ *                             the fast decimal path of ctr_parse_libsvm_device or not ending at its field's end; an
+ *                             int that is not [+-]?[0-9]{1,9}) }
+ * labels/dense/cat rows are valid iff info[2] == info[3] == info[4] == 0.  len < 2^32.  No allocation and no
+ * synchronisation inside. */
+size_t ctr_parse_csv_device_workspace_bytes(size_t len, int64_t max_rows);
+int ctr_parse_csv_device(const char* text, size_t len, int n_float, int n_int, int64_t max_rows, int final_chunk,
+                         float* labels, float* dense, int32_t* cat, int64_t* info, void* ws, size_t ws_bytes,
+                         ctr_stream_t stream);
+
 /* ---- Criteo feature pipeline (deep_ctr/Feature_pipeline/get_criteo_feature.py; DESIGN.md §2.4) ----------------
  * Raw Criteo TSV -> tr/va/te.libsvm + feature_map, byte for byte.  `text` is a chunk of whole lines (a last line
  * without '\n' counts), len < 2^30; line_base = index of its first line in the file (error positions are file lines).

@@ -116,6 +116,8 @@ SIGNATURES = {
     "ctr_libsvm_count_fields": (c_int, [c_char_p, c_size_t]),
     "ctr_parse_libsvm_device_workspace_bytes": (c_size_t, [c_size_t, c_int64]),
     "ctr_parse_libsvm_device": (c_int, [P, c_size_t, c_int, c_int64, c_int, P, P, P, P, P, c_size_t, P]),
+    "ctr_parse_csv_device_workspace_bytes": (c_size_t, [c_size_t, c_int64]),
+    "ctr_parse_csv_device": (c_int, [P, c_size_t, c_int, c_int, c_int64, c_int, P, P, P, P, P, c_size_t, P]),
     "ctr_criteo_table_bytes": (c_size_t, [c_int64]),
     "ctr_criteo_stats_workspace_bytes": (c_size_t, [c_size_t]),
     "ctr_criteo_stats": (c_int, [P, c_size_t, c_int64, P, c_int64, P, P, P, c_size_t, P]),

@@ -673,6 +673,30 @@ def parse_libsvm_device(text: torch.Tensor, F: int, max_rows: int, final_chunk: 
     return ids[:rows], vals[:rows], labels[:rows], consumed, bool(blank or bad or host)
 
 
+def parse_csv_device_workspace_bytes(n_bytes: int, max_rows: int) -> int:
+    return int(_L.ctr_parse_csv_device_workspace_bytes(n_bytes, max_rows))
+
+
+def parse_csv_device(text: torch.Tensor, n_bytes: int, n_float: int, n_int: int, max_rows: int, ws: torch.Tensor,
+                     final_chunk: bool = True):
+    """tf.decode_csv (wide_n_deep.py:55-73) of text[:n_bytes], a uint8 CUDA tensor; ws holds at least
+    parse_csv_device_workspace_bytes(n_bytes, max_rows) device bytes.  Returns (labels f32 [max_rows], dense f32
+    [max_rows, n_float-1], cat int32 [max_rows, n_int], info int64 [5] on the device) without waiting for the device:
+    info = (rows, bytes consumed, blank lines, malformed lines, lines with a number for the host), and when any of the
+    last three is non-zero the piece holds something only the host decoder may decide and the outputs must be
+    discarded."""
+    assert text.is_cuda and text.dtype == torch.uint8 and text.is_contiguous() and 0 <= n_bytes <= text.numel()
+    dev = text.device
+    labels = torch.empty(max_rows, dtype=torch.float32, device=dev)
+    dense = torch.empty(max_rows, n_float - 1, dtype=torch.float32, device=dev)
+    cat = torch.empty(max_rows, n_int, dtype=torch.int32, device=dev)
+    info = torch.empty(5, dtype=torch.int64, device=dev)
+    check(_L.ctr_parse_csv_device(text.data_ptr(), n_bytes, n_float, n_int, max_rows, int(final_chunk),
+                                  labels.data_ptr(), dense.data_ptr(), cat.data_ptr(), info.data_ptr(),
+                                  _p(ws, torch.uint8, "ws"), ws.numel(), _stream()), "ctr_parse_csv_device")
+    return labels, dense, cat, info
+
+
 def tfrecord_frame(buf, final_chunk: bool, max_records: int):
     """Frames the TFRecords of a host uint8 numpy buffer (ctr_tfrecord_frame).  Returns (rec_off int64 [records],
     consumed, error class, error offset, bytes the next record needs)."""

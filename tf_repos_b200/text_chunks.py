@@ -1,5 +1,6 @@
-"""Host side of the GPU text pipelines (criteo_feature, aliccp_tfrecord, aliccp_sample): input files read in pieces cut
-at line ends, the upload of a piece, device scratch buffers and the CUDA-event timer of each pass."""
+"""Host side of the GPU text pipelines (criteo_feature, aliccp_tfrecord, aliccp_sample, wide_n_deep's CSV input):
+input files read in pieces cut at line ends, the upload of a piece, device scratch buffers and the CUDA-event timer of
+each pass."""
 from __future__ import annotations
 
 from typing import Iterator

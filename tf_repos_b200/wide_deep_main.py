@@ -8,6 +8,7 @@ files and epochs, the last partial batch is kept); no shuffle.  Task types `trai
 from __future__ import annotations
 
 import glob
+import io
 import json
 import os
 import random
@@ -25,31 +26,143 @@ from .flags import FLAGS
 N_NUM, N_CAT = 13, 26
 
 
-def decode_csv_file(path: str) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
-    """-> labels f32 [n], dense f32 [n,13], cat int32 [n,26].  Empty fields take the record defaults; a line
-    without exactly 40 fields is an error (tf.decode_csv raises InvalidArgument)."""
+def _decode_csv_lines(fh, path: str, line_base: int = 0):
+    """The lines of text stream fh -> (labels, dense, cat) as decode_csv_file returns them, and how many lines were
+    read; line_base = lines of `path` before fh's first one (error positions are file lines)."""
     labels: List[float] = []
     dense: List[List[float]] = []
     cat: List[List[int]] = []
-    with open(path, "r") as fh:
-        for ln, line in enumerate(fh):
-            line = line.rstrip("\r\n")
-            if line == "":
-                continue
-            cols = line.split(",")
-            if len(cols) != 1 + N_NUM + N_CAT:
-                raise ValueError("%s:%d: Expect %d fields but have %d in record" % (path, ln + 1, 1 + N_NUM + N_CAT, len(cols)))
-            labels.append(float(cols[0]) if cols[0].strip() else 0.0)
-            dense.append([float(c) if c.strip() else 0.0 for c in cols[1:1 + N_NUM]])
-            cat.append([int(c) if c.strip() else 0 for c in cols[1 + N_NUM:]])
+    n_lines = 0
+    for ln, line in enumerate(fh, line_base + 1):
+        n_lines += 1
+        line = line.rstrip("\r\n")
+        if line == "":
+            continue
+        cols = line.split(",")
+        if len(cols) != 1 + N_NUM + N_CAT:
+            raise ValueError("%s:%d: Expect %d fields but have %d in record" % (path, ln, 1 + N_NUM + N_CAT, len(cols)))
+        labels.append(float(cols[0]) if cols[0].strip() else 0.0)
+        dense.append([float(c) if c.strip() else 0.0 for c in cols[1:1 + N_NUM]])
+        cat.append([int(c) if c.strip() else 0 for c in cols[1 + N_NUM:]])
     return (np.asarray(labels, dtype=np.float32), np.asarray(dense, dtype=np.float32).reshape(-1, N_NUM),
-            np.asarray(cat, dtype=np.int64).astype(np.int32).reshape(-1, N_CAT))
+            np.asarray(cat, dtype=np.int64).astype(np.int32).reshape(-1, N_CAT)), n_lines
 
 
-def input_fn(filenames: Sequence[str], num_epochs: int, batch_size: int = 1) -> Iterator[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]]:
-    """yields (dense f32 [B,13], cat int32 [B,26], labels f32 [B]) host tensors"""
+def decode_csv_file(path: str) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """-> labels f32 [n], dense f32 [n,13], cat int32 [n,26].  Empty fields take the record defaults; a line
+    without exactly 40 fields is an error (tf.decode_csv raises InvalidArgument)."""
+    with open(path, "r") as fh:
+        return _decode_csv_lines(fh, path)[0]
+
+
+def decode_csv_bytes(data: bytes, path: str, line_base: int = 0):
+    """decode_csv_file of a piece of `path` (whole lines, line_base lines of the file before it):
+    -> (labels, dense, cat, lines in the piece), with the file's own line numbers in the error messages."""
+    with io.TextIOWrapper(io.BytesIO(data)) as fh:      # the decoding and line ends of open(path, "r")
+        arrays, n_lines = _decode_csv_lines(fh, path, line_base)
+    return arrays + (n_lines,)
+
+
+def _csv_device_parts(files: Sequence[str], num_epochs: int, dev: torch.device, chunk_bytes: int):
+    """(labels, dense, cat) CUDA tensors of every piece of every file, num_epochs times: the file is read in pieces of
+    whole lines (text_chunks.pieces), a piece is staged in pinned memory, copied on a side stream and tokenised by
+    ctr_parse_csv_device; a piece the kernel declines is decoded by decode_csv_bytes, which owns the error messages.
+    Piece i+1 is read and its copy queued before piece i's counters are read back, so the copy runs under piece i's
+    kernel and under whatever the consumer queues for piece i's batches; that read-back is the only synchronise."""
+    from . import ops, text_chunks
+    main, side = torch.cuda.current_stream(dev), torch.cuda.Stream(dev)
+    copied = [torch.cuda.Event(), torch.cuda.Event()]
+    host = [torch.empty(max(chunk_bytes, 1), dtype=torch.uint8, pin_memory=True) for _ in range(2)]
+    text = [text_chunks.scratch(chunk_bytes, dev) for _ in range(2)]
+    ws = text_chunks.scratch(0, dev)
+
+    def stream():
+        for _ in range(num_epochs):
+            for path in files:
+                line_base = [0]                               # advanced by the consumer of each piece
+                for data in text_chunks.pieces(path, chunk_bytes):
+                    yield path, line_base, data
+
+    def upload(i: int, data: bytes):
+        """stage piece i and queue its copy.  Piece i-2's counters have been read back by now, so its copy and its
+        kernel, the last users of host[s] and text[s], are done."""
+        s, n = i % 2, len(data)
+        if host[s].numel() < n:                               # one line longer than chunk_bytes
+            host[s] = torch.empty(n, dtype=torch.uint8, pin_memory=True)
+            text[s] = text_chunks.scratch(n, dev)
+            side.wait_stream(main)                            # the new block may be memory main's queue still reads
+        host[s].numpy()[:n] = np.frombuffer(data, dtype=np.uint8)
+        with torch.cuda.stream(side):
+            text[s][:n].copy_(host[s][:n], non_blocking=True)
+            copied[s].record(side)
+
+    it = stream()
+    nxt = next(it, None)
+    if nxt is not None:
+        upload(0, nxt[2])
+    i = 0
+    try:
+        while nxt is not None:
+            path, line_base, data = nxt
+            s, n = i % 2, len(data)
+            max_rows = data.count(b"\n") + 1
+            need = ops.parse_csv_device_workspace_bytes(n, max_rows)
+            if ws.numel() < need:
+                ws = text_chunks.scratch(need, dev)
+            main.wait_event(copied[s])
+            labels, dense, cat, info = ops.parse_csv_device(text[s], n, 1 + N_NUM, N_CAT, max_rows, ws)
+            nxt = next(it, None)
+            if nxt is not None:
+                upload(i + 1, nxt[2])
+            rows, consumed, blank, bad, number = info.tolist()
+            if blank or bad or number or consumed != n:
+                labels, dense, cat, n_lines = decode_csv_bytes(data, path, line_base[0])
+                labels, dense, cat = (torch.from_numpy(a).to(dev) for a in (labels, dense, cat))
+                line_base[0] += n_lines
+            else:
+                labels, dense, cat = labels[:rows], dense[:rows], cat[:rows]
+                line_base[0] += rows
+            yield labels, dense, cat
+            i += 1
+    finally:
+        side.synchronize()                                    # no copy out of the pinned buffers is left in flight
+
+
+def _input_fn_device(files, num_epochs, batch_size, dev, chunk_bytes):
+    """The host generator's batching over device pieces: repeat before batch, batches straddle pieces, files and
+    epochs, the last partial batch is kept."""
+    carry = None                                              # fewer than batch_size rows waiting for the next piece
+    for part in _csv_device_parts(files, num_epochs, dev, chunk_bytes):
+        lo, n = 0, part[0].shape[0]
+        if carry is not None:
+            lo = min(batch_size - carry[0].shape[0], n)
+            carry = tuple(torch.cat([c, p[:lo]]) for c, p in zip(carry, part))
+            if carry[0].shape[0] < batch_size:
+                continue
+            yield carry[1], carry[2], carry[0]
+            carry = None
+        n_full = lo + ((n - lo) // batch_size) * batch_size
+        for b in range(lo, n_full, batch_size):
+            yield part[1][b:b + batch_size], part[2][b:b + batch_size], part[0][b:b + batch_size]
+        if n_full < n:
+            carry = tuple(p[n_full:] for p in part)
+    if carry is not None:
+        yield carry[1], carry[2], carry[0]
+
+
+CSV_CHUNK = 16 << 20  # bytes of text per piece of the device path
+
+
+def input_fn(filenames: Sequence[str], num_epochs: int, batch_size: int = 1, device=None,
+             chunk_bytes: int = CSV_CHUNK) -> Iterator[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]]:
+    """yields (dense f32 [B,13], cat int32 [B,26], labels f32 [B]).  device=None: host decoder, host tensors.
+    device="cuda[:i]": the text is streamed to the GPU in pieces of chunk_bytes and tokenised there
+    (ctr_parse_csv_device); batches are CUDA tensors.  Identical values either way."""
     print("Parsing", filenames)
     files = [filenames] if isinstance(filenames, str) else list(filenames)
+    if device is not None:
+        yield from _input_fn_device(files, num_epochs, batch_size, torch.device(device), chunk_bytes)
+        return
     carry = None
     for _ in range(num_epochs):
         for path in files:
@@ -129,9 +242,13 @@ def run():
     restore_checkpoint(model, FLAGS.model_dir)
     dev = model.device
 
+    if FLAGS.input_parse not in ("device", "host"):
+        raise SystemExit("input_parse must be one of {device, host}")
+    parse_dev = dev if FLAGS.input_parse == "device" else None
+
     def batches(files, epochs):
-        for dense, cat, labels in input_fn(files, epochs, FLAGS.batch_size):
-            yield dense.to(dev), cat.to(dev), labels.to(dev)
+        for batch in input_fn(files, epochs, FLAGS.batch_size, device=parse_dev):
+            yield batch if parse_dev is not None else tuple(t.to(dev) for t in batch)
 
     def evaluate(files):
         preds, labs = [], []
