@@ -258,7 +258,7 @@ int ctr_logit_loss(const float* bias, const float* y_a, const float* y_b, const 
                    const float* labels, int B, int B_total, float* y, float* pred, float* loss_ce,
                    float* dy, float* dbias, ctr_stream_t stream);
 
-/* ---- dense layers: fp32 SIMT GEMMs with fused epilogues -------------------------------------------
+/* ---- dense layers: wgmma 3xTF32 GEMMs with fused epilogues -----------------------------------------
  * tf.contrib.layers.fully_connected (DeepFM.py:156,165) + tf.nn.dropout (:162) and their autodiff.
  *   fwd: out[M,Nd] = dropout(act(in[M,Kd] @ Wt[Kd,Nd] + b)),  act 0 = identity, 1 = relu;
  *        drop_mask = binary keep mask [M,Nd] (NULL = no dropout): out = x / keep_prob * mask.

@@ -11,13 +11,9 @@ Error bounds used below (each comparison states which one and why):
   gemm_rel(R, adds): a product over a reduction of length R, then `adds` rounded fp32 additions (split-R partial sums,
              bias, group bias, C += acc), relative to |A|@|B| + |addends|.  One wgmma k8 step aligns its 8 products and the
              accumulator and truncates each: <= 9 truncations per 8 reduction indices, 9/8*R*TRUNC; the cross-term accumulator
-             (2^-10 of the main one) adds at most 2^-9 of that; acc + acc2 is one more rounding.  The SIMT tiles (fmaf chain,
-             R roundings of U) stay inside the same bound.
+             (2^-10 of the main one) adds at most 2^-9 of that; acc + acc2 is one more rounding.
 """
 import math
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -25,12 +21,10 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 U = 2.0 ** -24
 TRUNC = 2.0 ** -23
 SPLIT = 3 * 2.0 ** -21
 DIN_K = (4, 8, 16, 32, 64, 128, 256)
-SIMT = os.environ.get("CTR_GEMM") == "simt"
 
 
 def gemm_rel(R, adds=0):
@@ -73,7 +67,7 @@ def _sm_count():
 
 def _pick_split(M, N, R):
     """fc.cu pick_split: the number of split-R chunks of a dW product (needed for its error bound)."""
-    t = 64 if SIMT else 128
+    t = 128
     tiles = ((M + t - 1) // t) * ((N + t - 1) // t)
     s = max((2 * _sm_count() + tiles - 1) // tiles, 1)
     return max(min(s, (R + 255) // 256, 64), 1)
@@ -146,24 +140,13 @@ def test_fc_bwd_act2_accumulate(M, K, H):
     _within(dE, dE_old.double() + dZ64 @ W64.T, gemm_rel(H, adds=1) * (dZ64.abs() @ W64.abs().T + dE_old.double().abs()),
             f"dE += dZ Wc^T (M={M} K={K} H={H})")
     # dW: S split-R chunks of ceil(M/S) rows each on the GEMM, then S - 1 fixed-order fp32 adds
-    transposed = (not SIMT) and K <= 64 and H >= 128
+    transposed = K <= 64 and H >= 128
     S = _pick_split(H, K, M) if transposed else _pick_split(K, H, M)
     _within(dW, E64.T @ dZ64, gemm_rel(-(-M // S), adds=S) * (E64.abs().T @ dZ64.abs()),
             f"dW (M={M} K={K} H={H} S={S} transposed={transposed})")
     dE2, dW2 = run()
     _bits_equal(dE2, dE, "dE on a second call")
     _bits_equal(dW2, dW, "dW on a second call")
-
-
-def test_simt_twins_of_the_grouped_and_accumulate_epilogues():
-    """CTR_GEMM=simt routes the same products through gemm_tile_kernel's EPI 1 (group bias) and EPI 2 (C += acc)
-    epilogues.  The switch is read once per process, so the two tests above run again in a child process."""
-    env = dict(os.environ, CTR_GEMM="simt")
-    r = subprocess.run([sys.executable, "-m", "pytest", "-q", "-x", "-p", "no:cacheprovider", os.path.abspath(__file__),
-                        "-k", "(fc_fwd_grouped or fc_bwd_act2) and not simt"],
-                       cwd=ROOT, capture_output=True, text=True, timeout=900, env=env)
-    assert r.returncode == 0, r.stdout[-4000:] + r.stderr[-2000:]
-    assert " passed" in r.stdout and " skipped" not in r.stdout, r.stdout[-2000:]
 
 
 # ---------------------------------------------------------------------------------------------------------------------

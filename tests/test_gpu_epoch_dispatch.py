@@ -35,7 +35,8 @@ ctr_epoch_max_steps(): `last` bytes reach 32 and the sweeps' per-step shared arr
 mid-epoch flushes and with a flush directly followed by the epoch end; one step that gathers nothing; ids re-gathered
 in later steps; ids never gathered.  The "big" cases hold >= 2e6 floats, so every sweep family runs its grid-stride
 loop more than once per thread; the "extreme" cases start from zero, denormal and near-FLT_MIN states.
-The process-wide switches CTR_EPOCH_SCALAR and CTR_EPOCH_CFG run in child processes (they are read once per process).
+The process-wide switch CTR_EPOCH_SCALAR (Adam through the scalar sweep kernels instead of the packed ones) runs in a
+child process (it is read once per process).
 """
 import json
 import math
@@ -464,55 +465,47 @@ def test_model_check_ids_raises_on_list_overflow():
 # ---------------------------------------------------------------------------------------------------------------
 # process-wide switches (read once per process): same bits as this process
 # ---------------------------------------------------------------------------------------------------------------
-_SWITCH_CASES = {
-    "scalar": [dict(opt="Adam", K=1, N=4000, P=7, flush=((3,),)), dict(opt="Adam", K=16, N=2000, P=7, flush=((3,),))],
-    "cfg": [dict(opt=o, K=16, N=2000, P=7, flush=((3,),)) for o in NON_ADAM],
-}
+_SWITCH_CASES = [dict(opt="Adam", K=1, N=4000, P=7, flush=((3,),)), dict(opt="Adam", K=16, N=2000, P=7, flush=((3,),))]
 
 CHILD = r"""
 import json, sys
 sys.path.insert(0, %(root)r)
 from tests.test_gpu_epoch_dispatch import _run_case, _SWITCH_CASES
-print("RESULT " + json.dumps([_run_case(c) for c in _SWITCH_CASES[%(which)r]]))
+print("RESULT " + json.dumps([_run_case(c) for c in _SWITCH_CASES]))
 """
 
 
-_SWITCH_ENVS = [{"CTR_EPOCH_SCALAR": "1"}] + [{"CTR_EPOCH_CFG": str(c)} for c in range(8)]
+_SWITCH_ENVS = [{"CTR_EPOCH_SCALAR": "1"}]
 
 
 def _env_id(env):
     return ",".join(f"{k}={v}" for k, v in env.items()) or "default"
 
 
-def _which(env):
-    return "scalar" if "CTR_EPOCH_SCALAR" in env else "cfg"
-
-
 @pytest.fixture(scope="module")
 def switch_runs():
     """Every switch setting and the default, each in its own child process, all started at once."""
-    runs = [({}, "scalar"), ({}, "cfg")] + [(e, _which(e)) for e in _SWITCH_ENVS]
+    runs = [{}] + _SWITCH_ENVS
     procs = []
-    for env_extra, which in runs:
-        env = {k: v for k, v in os.environ.items() if k not in ("CTR_EPOCH_CFG", "CTR_EPOCH_SCALAR")}
+    for env_extra in runs:
+        env = {k: v for k, v in os.environ.items() if k != "CTR_EPOCH_SCALAR"}
         env.update(env_extra)
-        procs.append(subprocess.Popen([sys.executable, "-c", CHILD % {"root": ROOT, "which": which}], cwd=ROOT, env=env,
+        procs.append(subprocess.Popen([sys.executable, "-c", CHILD % {"root": ROOT}], cwd=ROOT, env=env,
                                       stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True))
     out = {}
-    for (env_extra, which), p in zip(runs, procs):
+    for env_extra, p in zip(runs, procs):
         so, se = p.communicate(timeout=600)
         res = None
         if p.returncode == 0:
             res = json.loads([l for l in so.splitlines() if l.startswith("RESULT ")][-1][len("RESULT "):])
-        out[(_env_id(env_extra), which)] = (res, so[-2000:] + se[-3000:])
+        out[_env_id(env_extra)] = (res, so[-2000:] + se[-3000:])
     return out
 
 
 @pytest.mark.parametrize("env", _SWITCH_ENVS, ids=_env_id)
 def test_epoch_switch_leaves_every_bit_unchanged(switch_runs, env):
-    which = _which(env)
-    base, log0 = switch_runs[("default", which)]
-    got, log = switch_runs[(_env_id(env), which)]
+    base, log0 = switch_runs["default"]
+    got, log = switch_runs[_env_id(env)]
     assert base is not None, log0
     # the child checks every call against the oracle itself; its digests must also match the default process
     assert got is not None, log

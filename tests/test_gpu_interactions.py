@@ -34,13 +34,10 @@ Error bounds (each comparison states which one and why):
              slab and then n_warps partials in order -> gam(m + n_warps); dx0 = L fmafs + 2 adds -> gam(L + 2).
   fc1        y: ceil(Ka/32) + ceil(Kb/32) fmafs, 5 shuffle adds, + b -> gam(n + 6); dw/db: a chain of <= 64 rows per
              chunk, then colsum_rows (ceil(chunks/8) adds per row group, 8 more) -> gam(64 + ceil(chunks/8) + 8).
-  gemm_rel   as in test_gpu_din_attention.py: a 3xTF32 (or SIMT fmaf) product over a reduction of length R, then
+  gemm_rel   as in test_gpu_din_attention.py: a 3xTF32 product over a reduction of length R, then
              `adds` rounded fp32 additions, relative to |A|@|B| + |addends|.
 """
 import math
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -48,13 +45,11 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 U = 2.0 ** -24
 TRUNC = 2.0 ** -23
 SPLIT = 3 * 2.0 ** -21
 TINY = 2.0 ** -126
 SUB = 2.0 ** -149    # the subnormal spacing: a rounding whose result is below 2^-126 errs by up to SUB/2
-SIMT = os.environ.get("CTR_GEMM") == "simt"
 
 
 def gam(n):
@@ -590,7 +585,7 @@ NAMES = list(MODELS)
 
 def _pick_split(M, N, R):
     """fc.cu pick_split: the number of split-R chunks of a dW product"""
-    t = 64 if SIMT else 128
+    t = 128
     tiles = ((M + t - 1) // t) * ((N + t - 1) // t)
     s = max((2 * _sm_count() + tiles - 1) // tiles, 1)
     return max(min(s, (R + 255) // 256, 64), 1)
@@ -713,17 +708,6 @@ def test_dcn_default_config_one_step_with_several_samples_per_cross_warp():
     """B = 4 n_warps + 3: the model path gives every cross_bwd warp four or five samples"""
     n_warps = _sm_count() * _wpc(1248, 3)
     _one_step("DCN", 4 * n_warps + 3)
-
-
-def test_simt_twins_of_the_default_config_gradients():
-    """CTR_GEMM=simt routes the models' GEMMs through the SIMT tiles.  The switch is read once per process, so the
-    one-step tests above run again in a child process."""
-    env = dict(os.environ, CTR_GEMM="simt")
-    r = subprocess.run([sys.executable, "-m", "pytest", "-q", "-x", "-p", "no:cacheprovider", os.path.abspath(__file__),
-                        "-k", "default_config_one_step and not simt"],
-                       cwd=ROOT, capture_output=True, text=True, timeout=1200, env=env)
-    assert r.returncode == 0, r.stdout[-4000:] + r.stderr[-2000:]
-    assert "4 passed" in r.stdout and " skipped" not in r.stdout, r.stdout[-2000:]
 
 
 def _gpu_state_views(gpu, name):

@@ -13,18 +13,15 @@ Error bounds (each comparison states which one and why):
   U = 2^-24 is the unit roundoff of one round-to-nearest fp32 operation.  A value computed with n rounded operations
   chained along any one path of a fixed summation tree is within gamma(n) = n*U/(1 - n*U) of the exact result,
   relative to the sum of the absolute values of its terms (Higham, Accuracy and Stability, 4.2).  A fused
-  multiply-add rounds once.  gemm_rel is the 3xTF32 / SIMT product bound derived in test_gpu_din_attention.py.
+  multiply-add rounds once.  gemm_rel is the 3xTF32 product bound derived in test_gpu_din_attention.py.
 """
 import math
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 import torch
 
-from tests.test_gpu_din_attention import ROOT, U, _bits_equal, _np, _pick_split, _within, gemm_rel
+from tests.test_gpu_din_attention import U, _bits_equal, _np, _pick_split, _within, gemm_rel
 
 pytestmark = pytest.mark.gpu
 
@@ -518,17 +515,6 @@ def test_fc_wide_deep_layers(M, Kd, Nd, act):
     _bits_equal(dIn2, dIn, "dIn on a second call")
     _bits_equal(dW2, dW, "dW on a second call")
     _bits_equal(db2, db, "db on a second call")
-
-
-def test_simt_twin_of_the_wide_deep_layers():
-    """CTR_GEMM=simt routes the same layers through the SIMT tiles; the switch is read once per process, so the layer
-    test runs again in a child process."""
-    env = dict(os.environ, CTR_GEMM="simt")
-    r = subprocess.run([sys.executable, "-m", "pytest", "-q", "-x", "-p", "no:cacheprovider", os.path.abspath(__file__),
-                        "-k", "fc_wide_deep_layers and not simt"],
-                       cwd=ROOT, capture_output=True, text=True, timeout=900, env=env)
-    assert r.returncode == 0, r.stdout[-4000:] + r.stderr[-2000:]
-    assert " passed" in r.stdout and " skipped" not in r.stdout, r.stdout[-2000:]
 
 
 # ---------------------------------------------------------------------------------------------------------------------

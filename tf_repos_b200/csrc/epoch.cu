@@ -21,14 +21,12 @@
 
 namespace ctr {
 
-constexpr int EPOCH_MAX = 32;  // max steps per epoch (lr table / ss table size)
-
 // epoch_adam.cu: Adam sweep on the packed fp32 pipe (rows nothing gathered since `from`; the others go to `list`)
 // w_*: an optional scalar table [n_rows] that shares `last` and is swept in the same launch
 bool launch_epoch_sweep_adam(float* var, float* slot0, float* slot1, const uint8_t* last, int64_t n_rows, int K,
                              const float* hyper, const float* lr_table, int from, int upto, double* ss_partials,
                              int n_partials, int32_t* list, int32_t* list_count, int64_t list_cap,
-                             int32_t* list_overflow, int grid, cudaStream_t st, float* w_var = nullptr,
+                             int32_t* list_overflow, cudaStream_t st, float* w_var = nullptr,
                              float* w_slot0 = nullptr, float* w_slot1 = nullptr, double* w_ss_partials = nullptr);
 
 __device__ __forceinline__ float sq4(const float4& x) {
@@ -268,13 +266,14 @@ __device__ __forceinline__ void sweep_ss_flush(float (*ss_thr)[256], int upto, d
   }
 }
 
-template <int OPT, int UNROLL, int MINB>
-__global__ void __launch_bounds__(256, MINB)
+template <int OPT>
+__global__ void __launch_bounds__(256, 3)
 epoch_sweep_kernel(float* __restrict__ var, float* __restrict__ slot0, float* __restrict__ slot1,
                    uint8_t* __restrict__ last, int64_t n4, int K, const float* __restrict__ hyper,
                    const float* __restrict__ lr_table, int upto, int reset,
                    double* __restrict__ ss_partials, int n_partials) {
   constexpr bool two = OptTraits<OPT>::slots == 2;
+  constexpr int UNROLL = 2;
   __shared__ float lr_s[EPOCH_MAX];
   // sum(var^2) seen at step s: one fp32 accumulator per thread and step (each takes a few thousand terms of
   // similar size), reduced once at the end; the cross-CTA sum is double (ctr_epoch_reg_loss)
@@ -631,7 +630,7 @@ static bool epoch_rows2_supported(int K) {
 }
 
 static bool epoch_rows_supported(int K) {
-  return K == 4 || K == 8 || K == 16 || K == 32 || K == 64 || K == 128 || K == 256 || (K >= 1 && K <= 256);
+  return K >= 1 && K <= 256;
 }
 
 int ctr_epoch_rows(int opt, int apply, float* var, float* slot0, float* slot1, uint8_t* last,
@@ -767,7 +766,7 @@ int ctr_epoch_sweep2(int opt, float* var, float* slot0, float* slot1, float* w_v
   CTR_REQUIRE(cudaMemsetAsync(list_count, 0, sizeof(int32_t), st) == cudaSuccess, CTR_ERR_CUDA,
               "ctr_epoch_sweep2: memset failed");
   const bool ok = launch_epoch_sweep_adam(var, slot0, slot1, last, n_rows, K, hyper, lr_table, from, upto, ss_partials,
-                                          n_partials, list, list_count, list_cap, list_overflow, 0, st, w_var, w_slot0,
+                                          n_partials, list, list_count, list_cap, list_overflow, st, w_var, w_slot0,
                                           w_slot1, w_ss_partials);
   CTR_REQUIRE(ok, CTR_ERR_UNSUPPORTED, "ctr_epoch_sweep2: packed path refused K=%d", K);
   CTR_LAUNCHED("ctr_epoch_sweep2(adam)");
@@ -790,19 +789,10 @@ int ctr_epoch_sweep_ovf(int opt, float* var, float* slot0, float* slot1, uint8_t
                         int32_t* list_overflow, ctr_stream_t stream) {
   CTR_REQUIRE(n_rows >= 0 && K > 0 && from >= 0 && from <= upto && upto <= EPOCH_MAX, CTR_ERR_INVALID_ARG,
               "ctr_epoch_sweep: bad n_rows/K/from/upto");
-  // tuning hook (tools/tune_epoch.py): CTR_EPOCH_CFG selects (unroll, CTAs/SM) of the scalar K%4==0 kernel;
-  // CTR_EPOCH_SCALAR=1 routes Adam through the scalar kernels as well (A/B against the packed sweep)
-  static int cfg = -1;
-  if (cfg < 0) {
-    const char* e = getenv("CTR_EPOCH_CFG");
-    cfg = e ? atoi(e) : 4;
-    if (cfg < 0 || cfg > 7) cfg = 4;
-  }
+  // CTR_EPOCH_SCALAR=1 routes Adam through the scalar kernels below (A/B against the packed sweep)
   const bool force_scalar = epoch_force_scalar();
-  static const int kBlocksPerSm[8] = {3, 4, 2, 6, 3, 2, 6, 4};
   const int grid = sm_count() * 3;
   const int n_partials = sm_count() * 6;     // row length of ss_partials (>= every grid used here)
-  const int grid_v = sm_count() * kBlocksPerSm[cfg];
   if (n_partials_host) *n_partials_host = n_partials;
   if (n_rows == 0 || upto == 0) return CTR_OK;
   CTR_REQUIRE(var && slot0 && last && hyper && lr_table && ss_partials, CTR_ERR_INVALID_ARG,
@@ -819,8 +809,7 @@ int ctr_epoch_sweep_ovf(int opt, float* var, float* slot0, float* slot1, uint8_t
     CTR_REQUIRE(cudaMemsetAsync(list_count, 0, sizeof(int32_t), st) == cudaSuccess, CTR_ERR_CUDA,
                 "ctr_epoch_sweep: memset failed");
     const bool ok = launch_epoch_sweep_adam(var, slot0, slot1, last, n_rows, K, hyper, lr_table, from, upto,
-                                            ss_partials, n_partials, list, list_count, list_cap, list_overflow, grid,
-                                            st);
+                                            ss_partials, n_partials, list, list_count, list_cap, list_overflow, st);
     CTR_REQUIRE(ok, CTR_ERR_UNSUPPORTED, "ctr_epoch_sweep: packed path refused K=%d", K);
     CTR_LAUNCHED("ctr_epoch_sweep(adam)");
     // rows gathered since `from`: catch up from their own `last` to upto; they get their final `last` here
@@ -835,23 +824,11 @@ int ctr_epoch_sweep_ovf(int opt, float* var, float* slot0, float* slot1, uint8_t
   }
 
   if (row_in_warp) {   // a row's float4s sit in one warp: `last` can be rewritten in place
-#define ES_LAUNCH(OPT, U, MB)                                                                         \
-  epoch_sweep_kernel<OPT, U, MB><<<grid_v, 256, 0, st>>>(var, slot0, slot1, last, n_elem / 4, K, hyper, \
-                                                         lr_table, upto, reset, ss_partials, n_partials)
-#define ES_CALL(OPT)                                   \
-  switch (cfg) {                                       \
-    case 1: ES_LAUNCH(OPT, 2, 4); break;               \
-    case 2: ES_LAUNCH(OPT, 4, 2); break;               \
-    case 3: ES_LAUNCH(OPT, 2, 6); break;               \
-    case 4: ES_LAUNCH(OPT, 2, 3); break;               \
-    case 5: ES_LAUNCH(OPT, 2, 2); break;               \
-    case 6: ES_LAUNCH(OPT, 1, 6); break;               \
-    case 7: ES_LAUNCH(OPT, 1, 4); break;               \
-    default: ES_LAUNCH(OPT, 4, 3); break;              \
-  }
+#define ES_CALL(OPT)                                                                           \
+  epoch_sweep_kernel<OPT><<<grid, 256, 0, st>>>(var, slot0, slot1, last, n_elem / 4, K, hyper, \
+                                                lr_table, upto, reset, ss_partials, n_partials);
     CTR_OPT_SWITCH(opt, ES_CALL)
 #undef ES_CALL
-#undef ES_LAUNCH
     CTR_LAUNCHED("ctr_epoch_sweep");
   } else if (K == 1 && n_rows % 4 == 0 && ((uintptr_t)last & 3) == 0) {
 #define ES1_CALL(OPT)                                                                                \

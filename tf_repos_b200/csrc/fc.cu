@@ -1,118 +1,13 @@
 // fc.cu -- the dense 'Deep-part': fully_connected layers (DeepFM.py:152-167), forward and backward,
-// with fused epilogues (bias + relu + dropout; dZ + bias-gradient).  The products run on the tensor cores
-// (tc_gemm.cu, 3xTF32); the fp32 SIMT tiles below are the CTR_GEMM=simt alternative.
-//
-// One templated tile kernel serves the three products of a layer:
-//   forward   out[M,N]  = act(in[M,K] @ W[K,N] + b)          (A reduce-contiguous, B row-contiguous)
-//   backward  dIn[M,K]  = dZ[M,N] @ W[K,N]^T                 (A reduce-contiguous, B reduce-contiguous)
+// with fused epilogues (bias + relu + dropout; dZ + bias-gradient).  The three products of a layer run on the
+// tensor cores (tc_gemm.cu, wgmma 3xTF32); this file holds their launches and the passes around them:
+//   forward   out[M,N]  = act(in[M,K] @ W[K,N] + b)
+//   backward  dIn[M,K]  = dZ[M,N] @ W[K,N]^T
 //             dW[K,N]   = in[M,K]^T @ dZ[M,N]  (split over M, deterministic two-pass reduction)
 // Accumulation order over the reduction dimension is fixed => bit-reproducible run to run.
-#include <stdlib.h>
-#include <string.h>
-
 #include "common.cuh"
 
 namespace ctr {
-
-constexpr int GEMM_BK = 16;
-
-// C[i][j] = sum_r A(i,r) * B(r,j),  i < M, j < N, r < R.
-//   A_RC (reduce-contiguous): A(i,r) = A[i*lda + r]   else  A(i,r) = A[r*lda + i]
-//   B_RC (reduce-contiguous): B(r,j) = B[j*ldb + r]   else  B(r,j) = B[r*ldb + j]
-// blockIdx.z splits R into gridDim.z chunks; chunk z writes C + z*M*N (EPI 0) .
-// EPI 1: C = act(acc + bias[j] + gbias[i / gP][j]) (/keep * mask[i][j])   (act: 0 identity, 1 relu)
-//        gbias: optional per-row-group bias (DIN: one row per sample, shared by its P positions)
-// EPI 2: C += acc
-template <int BM, int BN, int TM, int TN, bool A_RC, bool B_RC, int EPI>
-__global__ void __launch_bounds__((BM / TM) * (BN / TN))
-gemm_tile_kernel(const float* __restrict__ A, int lda, const float* __restrict__ B, int ldb,
-                 float* __restrict__ C, int ldc, int M, int N, int R, const float* __restrict__ bias,
-                 int act, const float* __restrict__ mask, float keep, const float* __restrict__ gbias,
-                 int gP) {
-  constexpr int NT = (BM / TM) * (BN / TN);
-  __shared__ __align__(16) float As[2][GEMM_BK][BM + 4];
-  __shared__ __align__(16) float Bs[2][GEMM_BK][BN + 4];
-  const int tid = threadIdx.x;
-  const int tx = tid % (BN / TN), ty = tid / (BN / TN);
-  const int i0 = blockIdx.y * BM, j0 = blockIdx.x * BN;
-  const int r_chunk = (R + gridDim.z - 1) / gridDim.z;
-  const int r_begin = blockIdx.z * r_chunk;
-  const int r_end = min(R, r_begin + r_chunk);
-
-  float acc[TM][TN];
-#pragma unroll
-  for (int a = 0; a < TM; ++a)
-#pragma unroll
-    for (int b = 0; b < TN; ++b) acc[a][b] = 0.f;
-
-  // cooperative tile loads (scalar, bounds-checked; the tiles are small and L2-resident)
-  auto load_tiles = [&](int buf, int r0) {
-    for (int e = tid; e < BM * GEMM_BK; e += NT) {
-      int i, r;
-      if (A_RC) { r = e % GEMM_BK; i = e / GEMM_BK; } else { i = e % BM; r = e / BM; }
-      const int gi = i0 + i, gr = r0 + r;
-      float v = 0.f;
-      if (gi < M && gr < r_end) v = A_RC ? A[(int64_t)gi * lda + gr] : A[(int64_t)gr * lda + gi];
-      As[buf][r][i] = v;
-    }
-    for (int e = tid; e < BN * GEMM_BK; e += NT) {
-      int j, r;
-      if (B_RC) { r = e % GEMM_BK; j = e / GEMM_BK; } else { j = e % BN; r = e / BN; }
-      const int gj = j0 + j, gr = r0 + r;
-      float v = 0.f;
-      if (gj < N && gr < r_end) v = B_RC ? B[(int64_t)gj * ldb + gr] : B[(int64_t)gr * ldb + gj];
-      Bs[buf][r][j] = v;
-    }
-  };
-
-  int buf = 0;
-  if (r_begin < r_end) load_tiles(0, r_begin);
-  __syncthreads();
-  for (int r0 = r_begin; r0 < r_end; r0 += GEMM_BK) {
-    if (r0 + GEMM_BK < r_end) load_tiles(buf ^ 1, r0 + GEMM_BK);
-#pragma unroll
-    for (int r = 0; r < GEMM_BK; ++r) {
-      float a[TM], b[TN];
-#pragma unroll
-      for (int u = 0; u < TM; u += 4) {
-        const float4 t = *reinterpret_cast<const float4*>(&As[buf][r][ty * TM + u]);
-        a[u] = t.x; a[u + 1] = t.y; a[u + 2] = t.z; a[u + 3] = t.w;
-      }
-#pragma unroll
-      for (int u = 0; u < TN; u += 4) {
-        const float4 t = *reinterpret_cast<const float4*>(&Bs[buf][r][tx * TN + u]);
-        b[u] = t.x; b[u + 1] = t.y; b[u + 2] = t.z; b[u + 3] = t.w;
-      }
-#pragma unroll
-      for (int u = 0; u < TM; ++u)
-#pragma unroll
-        for (int w = 0; w < TN; ++w) acc[u][w] = fmaf(a[u], b[w], acc[u][w]);
-    }
-    __syncthreads();
-    buf ^= 1;
-  }
-
-  float* Cz = C + (EPI == 0 ? (int64_t)blockIdx.z * M * ldc : 0);
-#pragma unroll
-  for (int u = 0; u < TM; ++u) {
-    const int gi = i0 + ty * TM + u;
-    if (gi >= M) continue;
-#pragma unroll
-    for (int w = 0; w < TN; ++w) {
-      const int gj = j0 + tx * TN + w;
-      if (gj >= N) continue;
-      float v = acc[u][w];
-      if (EPI == 2) v += Cz[(int64_t)gi * ldc + gj];
-      if (EPI == 1) {
-        if (bias) v += bias[gj];
-        if (gbias) v += gbias[(int64_t)(gi / gP) * N + gj];
-        if (act == 1) v = fmaxf(v, 0.f);
-        if (mask) v = __fdiv_rn(v, keep) * mask[(int64_t)gi * ldc + gj];  // tf.nn.dropout: x/keep*binary
-      }
-      Cz[(int64_t)gi * ldc + gj] = v;
-    }
-  }
-}
 
 // out[k][n] = sum_z partial[z][k][n]  (fixed order)
 __global__ void splitk_reduce_kernel(const float* __restrict__ partial, int S, int64_t n, float* __restrict__ out) {
@@ -246,23 +141,14 @@ __global__ void dropout_mask_kernel(float* __restrict__ mask, int64_t n, float k
   }
 }
 
-// tc_gemm.cu: the same products on wgmma tensor cores (3xTF32).  CTR_GEMM=simt selects the SIMT tiles.
+// tc_gemm.cu: the products on wgmma tensor cores (3xTF32)
 int tc_gemm_dispatch(int kind, int epi, const float* A, int lda, const float* B, int ldb, float* C, int ldc, int M, int N,
                      int R, int S, const float* bias, int act, const float* mask, float keep, const float* gbias, int gP,
                      cudaStream_t st);
 
-static bool use_tc() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("CTR_GEMM");
-    v = (e && strcmp(e, "simt") == 0) ? 0 : 1;
-  }
-  return v == 1;
-}
-
 static int pick_split(int M, int N, int R) {
   // dW-style product: few output tiles, long reduction => split R so that >= ~2 waves of CTAs exist
-  const int t = use_tc() ? 128 : 64;
+  const int t = 128;   // tc_gemm.cu's output tile rows (TC_BM)
   const int tiles = ((M + t - 1) / t) * ((N + t - 1) / t);
   int s = (2 * sm_count() + tiles - 1) / tiles;
   if (s < 1) s = 1;
@@ -296,17 +182,7 @@ int ctr_fc_fwd_grouped(const float* in, const float* Wt, const float* b, const f
   CTR_REQUIRE(in && Wt && out, CTR_ERR_INVALID_ARG, "ctr_fc_fwd: null buffer");
   CTR_REQUIRE(!drop_mask || keep_prob > 0.f, CTR_ERR_INVALID_ARG, "ctr_fc_fwd: keep_prob must be > 0");
   cudaStream_t st = as_stream(stream);
-  if (use_tc()) {
-    tc_gemm_dispatch(0, 1, in, Kd, Wt, Nd, out, Nd, M, Nd, Kd, 1, b, act, drop_mask, keep_prob, group_bias, group_P, st);
-  } else if (Nd >= 128) {
-    dim3 grid((Nd + 127) / 128, (M + 63) / 64, 1);
-    gemm_tile_kernel<64, 128, 4, 8, true, false, 1><<<grid, 256, 0, st>>>(in, Kd, Wt, Nd, out, Nd, M, Nd, Kd, b, act,
-                                                                          drop_mask, keep_prob, group_bias, group_P);
-  } else {
-    dim3 grid((Nd + 63) / 64, (M + 63) / 64, 1);
-    gemm_tile_kernel<64, 64, 4, 4, true, false, 1><<<grid, 256, 0, st>>>(in, Kd, Wt, Nd, out, Nd, M, Nd, Kd, b, act,
-                                                                         drop_mask, keep_prob, group_bias, group_P);
-  }
+  tc_gemm_dispatch(0, 1, in, Kd, Wt, Nd, out, Nd, M, Nd, Kd, 1, b, act, drop_mask, keep_prob, group_bias, group_P, st);
   CTR_LAUNCHED("ctr_fc_fwd");
   return CTR_OK;
 }
@@ -341,7 +217,7 @@ int ctr_fc_bwd(const float* in, const float* Wt, const float* out, const float* 
   // 2. dW[Kd,Nd] = in^T @ dZ, split over M
   // narrow layer input (DIN attention: Kd = 32, Nd = 256, M = B*P = 409600): as in^T @ dZ the 128-row MMA tile
   // would be 3/4 padding; the transposed product dW^T[Nd,Kd] = dZ^T @ in fills it (and its N = Kd MMAs are 4x smaller)
-  const bool dw_transposed = use_tc() && Kd <= 64 && Nd >= 128;
+  const bool dw_transposed = Kd <= 64 && Nd >= 128;
   const int S = dw_transposed ? pick_split(Nd, Kd, M) : pick_split(Kd, Nd, M);
   if (dw_transposed) {
     tc_gemm_dispatch(2, 0, dOut, Nd, in, Kd, dw_part, Kd, Nd, Kd, M, S, nullptr, 0, nullptr, 1.f, nullptr, 1, st);
@@ -350,13 +226,7 @@ int ctr_fc_bwd(const float* in, const float* Wt, const float* out, const float* 
     splitk_reduce_t_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(dw_part, S, Kd, Nd, dW);
     CTR_LAUNCHED("fc_dw_reduce(t)");
   } else {
-    if (use_tc()) {
-      tc_gemm_dispatch(2, 0, in, Kd, dOut, Nd, S == 1 ? dW : dw_part, Nd, Kd, Nd, M, S, nullptr, 0, nullptr, 1.f, nullptr, 1, st);
-    } else {
-      dim3 grid((Nd + 63) / 64, (Kd + 63) / 64, S);
-      gemm_tile_kernel<64, 64, 4, 4, false, false, 0><<<grid, 256, 0, st>>>(in, Kd, dOut, Nd, S == 1 ? dW : dw_part, Nd,
-                                                                            Kd, Nd, M, nullptr, 0, nullptr, 1.f, nullptr, 1);
-    }
+    tc_gemm_dispatch(2, 0, in, Kd, dOut, Nd, S == 1 ? dW : dw_part, Nd, Kd, Nd, M, S, nullptr, 0, nullptr, 1.f, nullptr, 1, st);
     CTR_LAUNCHED("fc_dw");
     if (S > 1) {
       const int64_t n = (int64_t)Kd * Nd;
@@ -365,17 +235,8 @@ int ctr_fc_bwd(const float* in, const float* Wt, const float* out, const float* 
     }
   }
   // 3. dIn[M,Kd] = dZ @ W^T
-  if (dIn && use_tc()) {
+  if (dIn) {
     tc_gemm_dispatch(1, accumulate_din ? 2 : 0, dOut, Nd, Wt, Nd, dIn, Kd, M, Kd, Nd, 1, nullptr, 0, nullptr, 1.f, nullptr, 1, st);
-    CTR_LAUNCHED("fc_din");
-  } else if (dIn) {
-    dim3 grid((Kd + 127) / 128, (M + 63) / 64, 1);
-    if (accumulate_din)
-      gemm_tile_kernel<64, 128, 4, 8, true, true, 2><<<grid, 256, 0, st>>>(dOut, Nd, Wt, Nd, dIn, Kd, M, Kd, Nd, nullptr,
-                                                                           0, nullptr, 1.f, nullptr, 1);
-    else
-      gemm_tile_kernel<64, 128, 4, 8, true, true, 0><<<grid, 256, 0, st>>>(dOut, Nd, Wt, Nd, dIn, Kd, M, Kd, Nd, nullptr,
-                                                                           0, nullptr, 1.f, nullptr, 1);
     CTR_LAUNCHED("fc_din");
   }
   return CTR_OK;

@@ -10,8 +10,6 @@
 // updates EVERY row each step: rows gathered this step get g = segment_sum + l2*var, all others
 // g = l2*var.  `ctr_opt_dense_sweep` is that full-table pass: a pure HBM stream
 // (read var,slot0,slot1; write var,slot0,slot1) -- 24 B/element for Adam.
-#include <stdlib.h>
-
 #include "optim_steps.cuh"
 
 namespace ctr {
@@ -99,15 +97,15 @@ opt_patch_rows_kernel(float* __restrict__ var, float* __restrict__ slot0, float*
 // ---- dense sweep (the dominant kernel of an exact-TF step: pure HBM stream) -----------------------
 constexpr int SWEEP_THREADS = 256;
 
-// UNROLL float4 triples in flight per thread; MINB = resident CTAs per SM the register budget is
-// squeezed for: the kernel is a pure stream, so what matters is bytes
-// in flight per SM = MINB * 256 threads * UNROLL * 48 B.
-template <int OPT, int SWEEP_UNROLL, int MINB>
-__global__ void __launch_bounds__(SWEEP_THREADS, MINB)
+// SWEEP_UNROLL float4 triples in flight per thread, register budget squeezed for 2 resident CTAs per SM: the kernel
+// is a pure stream, so what matters is bytes in flight per SM = 2 CTAs * 256 threads * SWEEP_UNROLL * 48 B.
+template <int OPT>
+__global__ void __launch_bounds__(SWEEP_THREADS, 2)
 opt_dense_sweep_kernel(float* __restrict__ var, float* __restrict__ slot0, float* __restrict__ slot1,
                        int64_t n4, int64_t n_elem, const float* __restrict__ hyper,
                        float* __restrict__ sumsq_partials) {
   constexpr bool two = OptTraits<OPT>::slots == 2;
+  constexpr int SWEEP_UNROLL = 4;
   const Hyper h = load_hyper(hyper);
   float4* v4 = reinterpret_cast<float4*>(var);
   float4* a4 = reinterpret_cast<float4*>(slot0);
@@ -281,15 +279,7 @@ int ctr_opt_dense_sweep(int opt, float* var, float* slot0, float* slot1, int64_t
                         const float* hyper, float* sumsq_partials, int* n_partials_host,
                         ctr_stream_t stream) {
   CTR_REQUIRE(n_elem >= 0, CTR_ERR_INVALID_ARG, "ctr_opt_dense_sweep: n_elem < 0");
-  // tuning hook (tools/tune_sweep.py): CTR_SWEEP_CFG = 0..3 selects (unroll, CTAs/SM)
-  static int cfg = -1;
-  if (cfg < 0) {
-    const char* e = getenv("CTR_SWEEP_CFG");
-    cfg = e ? atoi(e) : 0;
-    if (cfg < 0 || cfg > 3) cfg = 0;
-  }
-  static const int kBlocksPerSm[4] = {2, 4, 3, 6};
-  const int grid = sm_count() * kBlocksPerSm[cfg];
+  const int grid = sm_count() * 2;
   if (n_partials_host) *n_partials_host = sm_count() * 8;
   if (n_elem == 0) return CTR_OK;
   CTR_REQUIRE(var && slot0 && hyper, CTR_ERR_INVALID_ARG, "ctr_opt_dense_sweep: null buffer");
@@ -298,19 +288,10 @@ int ctr_opt_dense_sweep(int opt, float* var, float* slot0, float* slot1, int64_t
               CTR_ERR_INVALID_ARG, "ctr_opt_dense_sweep: tensors must be 16-byte aligned");
   cudaStream_t st = as_stream(stream);
   const int64_t n4 = n_elem / 4;
-#define SWEEP_LAUNCH(OPT, U, MB)                                                                   \
-  opt_dense_sweep_kernel<OPT, U, MB><<<grid, SWEEP_THREADS, 0, st>>>(var, slot0, slot1, n4, n_elem, \
-                                                                     hyper, sumsq_partials)
-#define SWEEP_CALL(OPT)                                   \
-  switch (cfg) {                                          \
-    case 1: SWEEP_LAUNCH(OPT, 2, 4); break;               \
-    case 2: SWEEP_LAUNCH(OPT, 4, 3); break;               \
-    case 3: SWEEP_LAUNCH(OPT, 1, 6); break;               \
-    default: SWEEP_LAUNCH(OPT, 4, 2); break;              \
-  }
+#define SWEEP_CALL(OPT)                                                                                     \
+  opt_dense_sweep_kernel<OPT><<<grid, SWEEP_THREADS, 0, st>>>(var, slot0, slot1, n4, n_elem, hyper, sumsq_partials);
   CTR_OPT_SWITCH(opt, SWEEP_CALL)
 #undef SWEEP_CALL
-#undef SWEEP_LAUNCH
   CTR_LAUNCHED("ctr_opt_dense_sweep");
   return CTR_OK;
 }

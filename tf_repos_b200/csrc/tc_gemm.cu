@@ -1,5 +1,6 @@
 // tc_gemm.cu -- the dense GEMMs of the MLP / attention layers on the Hopper tensor cores (wgmma, fp32
-// accumulators in registers), at fp32-class accuracy through a 3xTF32 split.
+// accumulators in registers), at fp32-class accuracy through a 3xTF32 split.  This is the only GEMM path:
+// fc.cu launches every layer product, at every shape, through tc_gemm_dispatch.
 //
 // Why 3xTF32: the parity target is 1e-5 relative on the logits; a plain TF32 (10-bit mantissa) or
 // BF16 product loses 1e-3.  Each fp32 operand is split on the fly into hi = rn_tf32(a) and

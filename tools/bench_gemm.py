@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Times ctr_fc_fwd / ctr_fc_bwd for the MLP and DIN-attention shapes; run with CTR_GEMM=simt to compare the
-fp32 SIMT tiles against the default wgmma 3xTF32 path; prints TFLOP/s (2*M*K*N per product) and max error."""
+"""Times ctr_fc_fwd / ctr_fc_bwd (the wgmma 3xTF32 path) for the MLP and DIN-attention shapes; prints TFLOP/s
+(2*M*K*N per product) and max error."""
 import os
 import sys
 
@@ -11,7 +11,6 @@ sys.path.insert(0, ROOT)
 from tf_repos_b200 import ops  # noqa: E402
 
 d = torch.device("cuda:0")
-print("CTR_GEMM =", os.environ.get("CTR_GEMM", "tc (default)"))
 for (M, Kd, Nd) in [(8192, 624, 256), (8192, 256, 128), (8192, 128, 64), (409600, 32, 256), (4096, 608, 256)]:
     x = torch.randn(M, Kd, device=d); W = torch.randn(Kd, Nd, device=d) / Kd ** 0.5; b = torch.zeros(Nd, device=d)
     out = torch.empty(M, Nd, device=d); dO = torch.randn(M, Nd, device=d)
