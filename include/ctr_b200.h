@@ -580,6 +580,24 @@ int ctr_tfrecord_emit_esmm(const void* stage, const int64_t* slot_off, const int
                            const int32_t* bag_off, int32_t* feat_ids, int32_t* a_ids, int32_t* bag_ids, float* bag_wgt,
                            float* y, float* z, ctr_stream_t stream);
 
+/* ---- DIN serving input (DIN.py:60-77 without labels, DIN.py:385-397; DESIGN.md §2.10) ----------------------------
+ * One slice of a serving request: n serialized tf.Examples, Example b = data[offsets[b], offsets[b+1]) (device bytes,
+ * offsets int64 [n+1], each Example < 2^31 bytes), 1 <= n <= B.  One warp per batch slot b < B walks its Example (slot
+ * b >= n repeats Example 0, as din_main.make_batch pads) with the scan's walk and checks, minus the CRC and the labels:
+ * y and z must be well formed but are neither required nor kind-checked.  Writes
+ *   slot_off int64 [B], slot_len int32 [B]   the slot's bytes, for ctr_tfrecord_emit_din(data, slot_off, slot_len, ...)
+ *   a_int_off int32 [B+1]                    exclusive scan (one CTA, on the device) of the a_intids bag lengths, each
+ *                                            clamped to max_a_int, so the emit writes at most B * max_a_int ids
+ *   maxima int32 [2]                         atomicMax-folded (set to 0 by the caller): the longest u_*ids list and the
+ *                                            longest a_intids bag of the n Examples, unclamped; a longer value than the
+ *                                            emit's P / max_a_int means the slice must be run again with larger buffers
+ *   err                                      min-folded as ctr_tfrecord_scan's with (example_base + b) << 16, b < n;
+ *                                            checks 1-6 (no CRC), arg as there (check 2: keys 2-5 only)
+ * A rejected Example's lengths are 0.  No allocation and no synchronisation inside. */
+int ctr_din_serve_scan(const void* data, const int64_t* offsets, int64_t n, int64_t example_base, int F, int B,
+                       int max_a_int, int64_t* slot_off, int32_t* slot_len, int32_t* a_int_off, int32_t* maxima,
+                       uint64_t* err, ctr_stream_t stream);
+
 /* ---- Ali-CCP TFRecord writer (deep_ctr/Feature_pipeline/get_aliccp_tfrecord.py; DESIGN.md §2.6) ----------------
  * Joined Ali-CCP lines `id,y,z,field:fid:val ...` -> framed tf.Example records, byte-identical to
  * tfrecord.write_records(path, [tfrecord.encode_example(features) ...]) of the features gen_tfrecords builds.  `text` is

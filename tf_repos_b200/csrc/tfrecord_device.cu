@@ -23,6 +23,7 @@
 #include "common.cuh"
 #include "crc32c.cuh"
 #include "example_wire.cuh"   // tr_byte, tr_u32, tr_float, tr_varint, tr_field, tr_utf8
+#include "scan_sort.cuh"      // cta_scan_kernel
 
 namespace ctr {
 
@@ -299,6 +300,51 @@ __global__ void __launch_bounds__(TR_THREADS) tr_emit_din_kernel(
   }
 }
 
+// DIN serving (DESIGN.md §2.10): one warp per batch slot b of a request slice; slot b >= n repeats Example 0, as
+// make_batch pads.  The walk and checks of tr_scan_kernel without framing, CRC or labels: y and z are parsed (they must be
+// well formed) and then dropped, so neither is required nor kind-checked.  Writes the slot's bytes for the emit, its
+// a_int bag length clamped to max_a_int (so the emit stays inside B * max_a_int ids) into a_int_off[b] for the scan,
+// and folds the unclamped longest behaviour list / a_int bag of the real Examples into maxima[0] / maxima[1].
+__global__ void __launch_bounds__(TR_THREADS) tr_din_serve_scan_kernel(
+    const uint8_t* __restrict__ data, const int64_t* __restrict__ offsets, int n, int B, int64_t example_base, int F,
+    int max_a_int, int64_t* __restrict__ slot_off, int32_t* __restrict__ slot_len, int32_t* __restrict__ a_int_off,
+    int32_t* __restrict__ maxima, unsigned long long* __restrict__ err) {
+  __shared__ TrSlot slots[TR_WARPS][TR_KEYS];
+  const int lane = tr_lane(), wib = threadIdx.x >> 5;
+  TrSlot* slot = slots[wib];
+  for (int b = blockIdx.x * TR_WARPS + wib; b < B; b += gridDim.x * TR_WARPS) {
+    const int e = b < n ? b : 0;
+    const int64_t s = offsets[e];
+    const int L = (int)(offsets[e + 1] - s);
+    int word;
+    if (!tr_walk(data + s, L, slot, false, true)) {
+      word = TE_MALFORMED << 8;
+    } else {
+      if (lane == 0) slot[TK_Y].fs = -1;
+      __syncwarp();
+      word = tr_checks(slot, F, 0);
+    }
+    int len = 0;
+    if (word < 0 && lane < 5) {
+      const int k = lane < 4 ? TK_UIDS + lane : TK_AINT;
+      len = slot[k].fs < 0 ? 0 : slot[k].r.count;
+    }
+    const int u_max = __reduce_max_sync(FULL_MASK, lane < 4 ? len : 0);
+    const int a_len = __shfl_sync(FULL_MASK, len, 4);
+    if (lane == 0) {
+      slot_off[b] = s;
+      slot_len[b] = L;
+      a_int_off[b] = a_len < max_a_int ? a_len : max_a_int;
+      if (b < n) {
+        if (u_max) atomicMax(&maxima[0], u_max);
+        if (a_len) atomicMax(&maxima[1], a_len);
+        if (word >= 0) atomicMin(err, (unsigned long long)(example_base + b) << 16 | (unsigned)word);
+      }
+    }
+    __syncwarp();
+  }
+}
+
 // make_batch of esmm_main (DeepCvrMTL.py:63-105): bags u_cat, u_shop, u_brand, u_int, a_int field-major, a_int's
 // weights 1.0
 __global__ void __launch_bounds__(TR_THREADS) tr_emit_esmm_kernel(
@@ -358,6 +404,23 @@ int ctr_tfrecord_emit_din(const void* stage, const int64_t* slot_off, const int3
       static_cast<const uint8_t*>(stage), slot_off, slot_len, B, F, P, a_int_off, feat_ids, a_ids, a_int_ids, u_ids,
       u_wgt, y);
   CTR_LAUNCHED("ctr_tfrecord_emit_din");
+  return CTR_OK;
+}
+
+int ctr_din_serve_scan(const void* data, const int64_t* offsets, int64_t n, int64_t example_base, int F, int B,
+                       int max_a_int, int64_t* slot_off, int32_t* slot_len, int32_t* a_int_off, int32_t* maxima,
+                       uint64_t* err, ctr_stream_t stream) {
+  CTR_REQUIRE(data && offsets && n > 0 && n <= B && example_base >= 0 && F > 0 && max_a_int > 0 && slot_off &&
+                  slot_len && a_int_off && maxima && err,
+              CTR_ERR_INVALID_ARG, "ctr_din_serve_scan: bad arguments");
+  CTR_REQUIRE(example_base + n < ((int64_t)1 << 47) && (int64_t)B * max_a_int < ((int64_t)1 << 31),
+              CTR_ERR_INVALID_ARG, "ctr_din_serve_scan: example index >= 2^47 or B * max_a_int >= 2^31");
+  cudaStream_t st = as_stream(stream);
+  tr_din_serve_scan_kernel<<<grid_for(B, TR_WARPS, 16), TR_THREADS, 0, st>>>(
+      static_cast<const uint8_t*>(data), offsets, (int)n, B, example_base, F, max_a_int, slot_off, slot_len, a_int_off,
+      maxima, reinterpret_cast<unsigned long long*>(err));
+  cta_scan_kernel<int32_t><<<1, 1024, 0, st>>>(a_int_off, nullptr, (int64_t)B + 1, nullptr);
+  CTR_LAUNCHED("ctr_din_serve_scan");
   return CTR_OK;
 }
 

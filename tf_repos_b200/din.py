@@ -119,6 +119,30 @@ class DIN(SparseModel):
         self.d_aint = torch.empty(B, K, **f32)
         self.global_step = 0
 
+    def grow(self, max_len: int, max_a_int: int):
+        """For inference: let predict() take batches whose behaviour lists reach max_len and whose a_int bags reach
+        max_a_int (sizes never shrink).  Only the forward's length-sized buffers are reallocated, all of them before
+        any is replaced, so a failed allocation leaves the model as it was.  The training buffers are released: a grown
+        model predicts but no longer trains.  Variables, optimizer slots and batch-norm statistics stay."""
+        P, A = max(self.P, int(max_len)), max(self.max_a_int, int(max_a_int))
+        if (P, A) == (self.P, self.max_a_int):
+            return
+        B, K, H, dev = self.B, self.K, self.H, self.device
+        f32 = dict(dtype=torch.float32, device=dev)
+        new = {"_poff": (torch.arange(B + 1, device=dev, dtype=torch.int32) * P).contiguous()}
+        if self.attention_pooling:
+            new.update(E=[torch.empty(B * P, K, **f32) for _ in range(4)],
+                       Hh=[torch.empty(B * P, H, **f32) for _ in range(4)],
+                       att=[torch.empty(B * P, **f32) for _ in range(4)], z=torch.empty(B * P, **f32))
+        # every allocation succeeded: commit (nothing below allocates)
+        for name, t in new.items():
+            setattr(self, name, t)
+        self.P, self.max_a_int = P, A
+        self.seg = self.ids_all = self.g_all = None
+        if self.attention_pooling:
+            self.att_mask = [None] * 4
+            self.dE = self.dz = self.dHh = self.dz_b = self.att_ws = None
+
     # ---- plumbing -------------------------------------------------------------------------------------
     def variables(self) -> Dict[str, torch.Tensor]:
         self.flush()
@@ -252,6 +276,8 @@ class DIN(SparseModel):
         step on the n_valid-sample batch (a padded id that enters the de-duplicated update with a zero summed gradient
         takes g = 0 + l2*var, which is the untouched-row update it would have taken anyway).  Not with --batch_norm
         (the padded rows would enter the batch moments)."""
+        if self.ids_all is None:
+            raise RuntimeError("this DIN grew its buffers for inference (DIN.grow) and no longer trains")
         upd = self.updater
         self._stage_ids(batch)
         upd.begin_step()

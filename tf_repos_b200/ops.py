@@ -726,6 +726,19 @@ def tfrecord_emit_din(stage, slot_off, slot_len, B, F, P, a_int_off, feat_ids, a
           "ctr_tfrecord_emit_din")
 
 
+def din_serve_scan(data, offsets, example_base: int, F: int, B: int, max_a_int: int, slot_off, slot_len, a_int_off,
+                   maxima, err):
+    """One serving slice of serialized tf.Examples data[offsets[b], offsets[b+1]) (uint8, offsets int64 [n+1], n <= B)
+    -> slot_off int64 [B], slot_len int32 [B] and a_int_off int32 [B+1] for tfrecord_emit_din; maxima int32 [2]
+    (longest behaviour list, longest a_int bag; zeroed by the caller) and err int64 [1] (uint64 bits, ~0 = none) are
+    folded into."""
+    n = offsets.numel() - 1
+    check(_L.ctr_din_serve_scan(_p(data, torch.uint8, "data"), _p(offsets, torch.int64, "offsets"), n, example_base, F, B,
+                                max_a_int, _p(slot_off, torch.int64, "slot_off"), _p(slot_len, torch.int32, "slot_len"),
+                                _p(a_int_off, torch.int32, "a_int_off"), _p(maxima, torch.int32, "maxima"),
+                                _p(err, torch.int64, "err"), _stream()), "ctr_din_serve_scan")
+
+
 def tfrecord_emit_esmm(stage, slot_off, slot_len, B, F, bag_off, feat_ids, a_ids, bag_ids, bag_wgt, y, z):
     check(_L.ctr_tfrecord_emit_esmm(_p(stage, torch.uint8, "stage"), _p(slot_off, torch.int64, "slot_off"),
                                     _p(slot_len, torch.int32, "slot_len"), B, F, _p(bag_off, torch.int32, "bag_off"),

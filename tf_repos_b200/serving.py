@@ -15,6 +15,13 @@ wide_n_deep's export (`--task_type=export_model`, `<servable_model_dir>/saved_mo
 
     s = Servable.load("./servable")
     out = s.classify([example_bytes, ...])       # {"scores": float32 [n,2] = [1-p, p], "classes": [n,2] b"0", b"1"}
+
+DIN's export (`DIN.py --task_type=export`, `<servable_model_dir>/<timestamp>/`) is a parsing receiver too (DIN.py:385-397);
+its request is serialized tf.Examples with the training schema of DIN.py:60-77 (DESIGN.md §2.10: the feat_ids /
+feat_vals spec its signature.json declares cannot feed DIN, quirk Q6).
+
+    s = Servable.load("./servable/1700000000")
+    prob = s.predict([example_bytes, ...])       # float32 [n]
 """
 from __future__ import annotations
 
@@ -24,6 +31,8 @@ from typing import Dict
 
 import numpy as np
 import torch
+
+from . import ops
 
 
 def _build(model_name: str, p: Dict, batch_size: int, device):
@@ -129,6 +138,168 @@ class WideDeepServable:
                 "classes": np.tile(np.array([b"0", b"1"], dtype="S1"), (n, 1))}
 
 
+_DIN_KEYS = ("y", "z", "feat_ids", "a_catids", "a_shopids", "a_brandids", "a_intids", "u_catids", "u_shopids",
+             "u_brandids", "u_intids", "u_catvals", "u_shopvals", "u_brandvals", "u_intvals")
+_DIN_U = ("cat", "shop", "brand", "int")
+_DIN_CHECKS = {1: "malformed tf.Example protobuf", 2: "required key {key!r} is missing or empty",
+               3: "feat_ids must hold exactly field_size={F} values",
+               4: "u_{u}ids and u_{u}vals differ in length",
+               5: "key {key!r} holds several kinds or the wrong kind ({kind})",
+               6: "key {key!r} holds an id outside [0, 2^31)"}
+# the ids DIN reads, in check order: all of feat_ids, the first value of a_*ids, all of a_intids and u_*ids
+_DIN_ID_KEYS = (("feat_ids", None), ("a_catids", 1), ("a_shopids", 1), ("a_brandids", 1), ("a_intids", None)) + \
+    tuple(("u_%sids" % u, None) for u in _DIN_U)
+
+
+def din_error_message(index: int, check: int, arg: int, F: int) -> str:
+    """ValueError text of the DIN serving check `check` (ctr_din_serve_scan's numbering) on Example `index`"""
+    key = _DIN_KEYS[arg]
+    kind = "float_list" if key.endswith("vals") else "int64_list"
+    return f"example {index}: " + _DIN_CHECKS[check].format(key=key, F=F, u=_DIN_U[arg % 4], kind=kind)
+
+
+def din_id_range_error(examples, upto: int, N: int):
+    """the message for the first of examples[:upto] (all passing the parse checks) whose read ids reach feature_size N,
+    or None"""
+    from .tfrecord import parse_example
+    for i in range(upto):
+        ex = parse_example(examples[i])
+        for key, first in _DIN_ID_KEYS:
+            v = np.asarray(ex.get(key, []), dtype=np.int64)[:first]
+            if len(v) and int(v.max()) >= N:
+                return f"example {i}: key {key!r} holds an id outside [0, feature_size={N})"
+    return None
+
+
+class DINServable:
+    """serving_default of an exported DIN (DIN.py:385-397, DESIGN.md §2.10): serialized tf.Examples with the training
+    schema of DIN.py:60-77 (labels not read) in, prob out.  Per request: one pinned host->device copy (error word,
+    maxima, offsets and bytes); per slice of at most max_batch Examples ctr_din_serve_scan, ctr_tfrecord_emit_din and
+    DIN.predict; one device->host copy (probabilities, error word, out-of-range id counter, maxima) after the only
+    synchronisation.  A slice whose behaviour lists or a_int bags outgrow the model's buffers is run again after
+    DIN.grow, which costs a second round trip.  Growth is permanent: later requests run the forward at the larger P.
+    A failed growth (out of memory) raises and leaves the servable as it was."""
+
+    def __init__(self, model):
+        self.model = model
+        self._host = self._dev = None
+        self._commit_batch(self._alloc_batch(model.P, model.max_a_int))
+
+    @classmethod
+    def load(cls, export_dir: str, max_batch: int = 4096, device="cuda", max_len: int = 64,
+             max_a_int: int = 8) -> "DINServable":
+        """export_dir as `DIN.py --task_type=export` writes it; max_len / max_a_int: the starting buffer lengths"""
+        from .din import DIN
+        p = json.load(open(os.path.join(export_dir, "signature.json")))["params"]
+        model = DIN(int(p["field_size"]), int(p["feature_size"]), int(p["embedding_size"]), max_batch, max_len,
+                    max_a_int=max_a_int, deep_layers=p.get("deep_layers", "256,128,64"),
+                    dropout=p.get("dropout", "0.5,0.5,0.5"), attention_layers=p.get("attention_layers", "256"),
+                    attention_pooling=bool(p.get("attention_pooling", True)), l2_reg=p.get("l2_reg", 1e-4),
+                    learning_rate=p.get("learning_rate", 5e-4), optimizer=p.get("optimizer", "Adam"),
+                    update_mode="lazy", device=device, batch_norm=bool(p.get("batch_norm", False)),
+                    batch_norm_decay=p.get("batch_norm_decay", 0.9))
+        model.load_variables(torch.load(os.path.join(export_dir, "variables.pt"), map_location="cpu"))
+        return cls(model)
+
+    def _alloc_batch(self, P: int, A: int) -> dict:
+        """the emit's buffers for behaviour lists up to P and a_int bags up to A; committed by the caller"""
+        m = self.model
+        B, F, dev = m.B, m.Fp, m.device
+        i32 = dict(dtype=torch.int32, device=dev)
+        return {"slot_off": torch.empty(B, dtype=torch.int64, device=dev), "slot_len": torch.empty(B, **i32),
+                "y": torch.empty(B, dtype=torch.float32, device=dev),          # absorbs the emit's label
+                "batch": {"feat_ids": torch.empty(B, F, **i32), "a_ids": torch.empty(3, B, **i32),
+                          "a_int_ids": torch.empty(B * A, **i32), "a_int_off": torch.empty(B + 1, **i32),
+                          "u_ids": torch.empty(4, B, P, **i32),
+                          "u_wgt": torch.empty(4, B, P, dtype=torch.float32, device=dev)}}
+
+    def _commit_batch(self, bufs: dict):
+        self._slot_off, self._slot_len, self._y, self._batch = bufs["slot_off"], bufs["slot_len"], bufs["y"], bufs["batch"]
+
+    def _grow(self, P: int, A: int):
+        """model and emit buffers for (P, A), or neither: the emit buffers are allocated first, and DIN.grow only
+        changes the model once all of its own allocations succeeded"""
+        bufs = self._alloc_batch(max(P, self.model.P), max(A, self.model.max_a_int))
+        self.model.grow(P, A)
+        self._commit_batch(bufs)
+
+    def _buffers(self, nbytes: int):
+        if self._host is None or self._host.numel() < nbytes:
+            cap = max(nbytes, 1 << 16)
+            self._host = torch.empty(cap, dtype=torch.uint8, pin_memory=True)
+            self._dev = torch.empty(cap, dtype=torch.uint8, device=self.model.device)
+        return self._host, self._dev
+
+    def _run(self, data, off, lo: int, hi: int, err, maxima, pred):
+        m, bt = self.model, self._batch
+        # the emit writes u_ids / u_wgt at stride P and up to B * max_a_int a_int ids: never past these tensors
+        if bt["u_ids"].shape[2] != m.P or bt["a_int_ids"].numel() != m.B * m.max_a_int:
+            raise RuntimeError(f"DINServable: batch buffers {tuple(bt['u_ids'].shape)} / {bt['a_int_ids'].numel()} do "
+                               f"not match the model's P={m.P}, max_a_int={m.max_a_int}")
+        ops.din_serve_scan(data, off[lo:hi + 1], lo, m.Fp, m.B, m.max_a_int, self._slot_off, self._slot_len,
+                           bt["a_int_off"], maxima, err)
+        ops.tfrecord_emit_din(data, self._slot_off, self._slot_len, m.B, m.Fp, m.P, bt["a_int_off"], bt["feat_ids"],
+                              bt["a_ids"], bt["a_int_ids"], bt["u_ids"], bt["u_wgt"], self._y)
+        pred[lo:hi].copy_(m.predict(bt)[:hi - lo])
+
+    def predict(self, examples) -> np.ndarray:
+        """examples: the serialized tf.Examples of the request (a sequence of bytes) -> prob float32 [n].  Raises
+        ValueError naming the first rejected Example (its index in the whole request) and the check."""
+        n = len(examples)
+        if n == 0:
+            return np.zeros(0, dtype=np.float32)
+        m = self.model
+        lens = np.fromiter(map(len, examples), dtype=np.int64, count=n)
+        if int(lens.max()) >= 1 << 31:
+            raise ValueError(f"example {int(np.argmax(lens >= 1 << 31))}: an Example of 2^31 bytes or more")
+        offsets = np.zeros(n + 1, dtype=np.int64)
+        np.cumsum(lens, out=offsets[1:])
+        slices = [(lo, min(lo + m.B, n)) for lo in range(0, n, m.B)]
+        S = len(slices)
+        # device layout: prob f32 [n] (padded to 8 bytes) | err | oob int32 [2] | maxima int32 [S, 2] (padded to 8) |
+        # offsets [n+1] | bytes; the first copy fills err..bytes, the last reads prob..maxima back
+        p_bytes = (4 * n + 7) & ~7
+        m_bytes = (8 * S + 7) & ~7
+        back = p_bytes + 16 + m_bytes
+        head = back + 8 * (n + 1)
+        total = head + int(offsets[-1])
+        host, dev = self._buffers(total)
+        h = host.numpy()
+        h[p_bytes:p_bytes + 8].view(np.int64)[0] = -1
+        h[p_bytes + 8:back] = 0
+        h[back:head].view(np.int64)[:] = offsets
+        h[head:total] = np.frombuffer(b"".join(examples), dtype=np.uint8)
+        dev[p_bytes:total].copy_(host[p_bytes:total], non_blocking=True)
+        pred = dev[:4 * n].view(torch.float32)
+        err = dev[p_bytes:p_bytes + 8].view(torch.int64)
+        oob = dev[p_bytes + 8:p_bytes + 16].view(torch.int32)
+        maxima = dev[p_bytes + 16:p_bytes + 16 + 8 * S].view(torch.int32).view(S, 2)
+        off = dev[back:head].view(torch.int64)
+        data = dev[head:total]
+        todo = list(range(S))
+        while True:
+            P, A = m.P, m.max_a_int
+            for s in todo:
+                self._run(data, off, *slices[s], err, maxima[s], pred)
+            oob.copy_(m.oob)
+            host[:back].copy_(dev[:back], non_blocking=True)
+            torch.cuda.current_stream(m.device).synchronize()
+            word = int(h[p_bytes:p_bytes + 8].view(np.int64)[0])
+            n_oob = int(h[p_bytes + 8:p_bytes + 12].view(np.int32)[0])
+            if word != -1 or n_oob:
+                m.oob.zero_()
+                ex = word >> 16 if word != -1 else n
+                msg = din_id_range_error(examples, ex, m.N)
+                if msg is None and word != -1:
+                    msg = din_error_message(ex, (word >> 8) & 0xFF, word & 0xFF, m.Fp)
+                raise ValueError(msg or f"an id outside [0, feature_size={m.N})")
+            mx = h[p_bytes + 16:p_bytes + 16 + 8 * S].view(np.int32).reshape(S, 2)
+            todo = [s for s in todo if mx[s, 0] > P or mx[s, 1] > A]
+            if not todo:
+                return h[:4 * n].view(np.float32).copy()
+            self._grow(int(mx[todo, 0].max()), int(mx[todo, 1].max()))
+
+
 class Servable:
     def __init__(self, model, signature: Dict):
         self.model, self.signature = model, signature
@@ -136,11 +307,13 @@ class Servable:
 
     @classmethod
     def load(cls, export_dir: str, max_batch: int = 4096, device="cuda"):
-        """the directory `--task_type=export` writes (DeepFM family) -> Servable; the one wide_n_deep's
-        `--task_type=export_model` writes (saved_model.pt) -> WideDeepServable"""
+        """the directory `--task_type=export` writes (DeepFM family) -> Servable, (DIN) -> DINServable; the one
+        wide_n_deep's `--task_type=export_model` writes (saved_model.pt) -> WideDeepServable"""
         if os.path.exists(os.path.join(export_dir, "saved_model.pt")):
             return WideDeepServable.load(export_dir, max_batch, device)
         sig = json.load(open(os.path.join(export_dir, "signature.json")))
+        if sig["model"] == "DIN":
+            return DINServable.load(export_dir, max_batch, device)
         model = _build(sig["model"], sig["params"], max_batch, torch.device(device))
         model.load_variables(torch.load(os.path.join(export_dir, "variables.pt"), map_location="cpu"))
         return cls(model, sig)

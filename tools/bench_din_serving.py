@@ -1,0 +1,126 @@
+#!/usr/bin/env python
+"""Latency and throughput of DIN's serving entry (serving.DINServable.predict) on one GPU.
+
+The model has the shapes of DESIGN.md's config 4 (DIN, F'=11, feature_size 1e8, embedding_size 32, deep_layers
+256,128,64, attention pooling, max_batch 4096) with its constructor's random variables.  Every Example of a request has
+the training schema of DIN.py:60-77: four behaviour lists of U{1..100} seeded ids each, with weights, and an a_intids bag
+of U{1..8} ids.  The servable's buffers start at P = 100 and max_a_int = 8, so no request grows them.
+
+  latency     wall clock around predict (host -> device copy, kernels, device -> host copy, the one synchronise) per
+              request after a warm-up of every size: median and p99 for n in --sizes
+  device      parse = ctr_din_serve_scan + ctr_tfrecord_emit_din, model = DIN.predict on the emitted batch: device time
+              from torch.profiler (CUDA activity only, in a phase of its own) per slice.  DIN.predict always runs the
+              full max_batch rows, so the model time does not shrink with n
+  throughput  Examples/s of predict at each n (n / median latency)
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+
+def _request(n, rng, F, N):
+    from tf_repos_b200.tfrecord import encode_example
+    out = []
+    for _ in range(n):
+        ex = {"feat_ids": rng.integers(1, N, F), "a_catids": rng.integers(1, N, 1), "a_shopids": rng.integers(1, N, 1),
+              "a_brandids": rng.integers(1, N, 1), "a_intids": rng.integers(1, N, int(rng.integers(1, 9)))}
+        for u, ln in zip(("cat", "shop", "brand", "int"), rng.integers(1, 101, 4)):
+            ex["u_%sids" % u] = rng.integers(1, N, ln)
+            ex["u_%svals" % u] = rng.random(ln, dtype=np.float32)
+        out.append(encode_example(ex))
+    return out
+
+
+def _kernel_ms(fn, reps):
+    """device time per call: the durations of the kernels fn launches, from torch.profiler (CUDA activity only)"""
+    from torch.autograd import DeviceType
+    fn()
+    torch.cuda.synchronize()
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        for _ in range(reps):
+            fn()
+        torch.cuda.synchronize()
+    us = sum(e.device_time_total for e in prof.key_averages() if e.device_type == DeviceType.CUDA)
+    return us / 1e3 / reps
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--sizes", default="1,16,256,4096")
+    ap.add_argument("--requests", type=int, default=200)
+    ap.add_argument("--warmup", type=int, default=20)
+    ap.add_argument("--feature_size", type=int, default=100_000_000)
+    ap.add_argument("--out", default="din_serving.json")
+    a = ap.parse_args()
+    assert torch.cuda.is_available(), "bench_din_serving measures on a GPU"
+    from tf_repos_b200 import ops
+    from tf_repos_b200.din import DIN
+    from tf_repos_b200.serving import DINServable
+
+    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip().splitlines()
+    F, N, K, B, P, A = 11, a.feature_size, 32, 4096, 100, 8
+    m = DIN(F, N, K, B, P, max_a_int=A, deep_layers="256,128,64", update_mode="lazy", device="cuda:0")
+    s = DINServable(m)
+    rng = np.random.default_rng(0)
+    sizes = [int(t) for t in a.sizes.split(",")]
+    reqs = {n: _request(n, rng, F, N) for n in sizes}
+    res = {"card": smi, "device_name": torch.cuda.get_device_name(0),
+           "model": f"DIN F'={F} N={N} K={K} deep_layers 256,128,64 attention pooling, max_batch {B}, P {P}, "
+                    f"max_a_int {A}; behaviour lists U{{1..100}}, a_int U{{1..8}}",
+           "latency_ms": {}, "examples_per_s": {}, "device_ms": {}}
+    for n in sizes:                      # every shape warmed up before any timing
+        for _ in range(a.warmup):
+            s.predict(reqs[n])
+    assert (m.P, m.max_a_int) == (P, A)
+    for n in sizes:
+        count = a.requests if n <= 256 else max(a.requests // 4, 20)
+        t = []
+        for _ in range(count):
+            t0 = time.perf_counter()
+            s.predict(reqs[n])
+            t.append((time.perf_counter() - t0) * 1e3)
+        med = float(np.median(t))
+        res["latency_ms"][str(n)] = {"median": med, "p99": float(np.percentile(t, 99)), "mean": float(np.mean(t)),
+                                     "requests": count}
+        res["examples_per_s"][str(n)] = n / (med / 1e3)
+        print(n, res["latency_ms"][str(n)], flush=True)
+    for n in sizes:
+        ex = reqs[n]
+        lens = np.array([len(r) for r in ex])
+        off = torch.tensor(np.concatenate([[0], np.cumsum(lens)]), dtype=torch.int64, device="cuda:0")
+        data = torch.tensor(np.frombuffer(b"".join(ex), dtype=np.uint8), device="cuda:0")
+        err = torch.full((1,), -1, dtype=torch.int64, device="cuda:0")
+        maxima = torch.zeros(2, dtype=torch.int32, device="cuda:0")
+        bt = s._batch
+
+        def parse():
+            ops.din_serve_scan(data, off, 0, F, B, A, s._slot_off, s._slot_len, bt["a_int_off"], maxima, err)
+            ops.tfrecord_emit_din(data, s._slot_off, s._slot_len, B, F, P, bt["a_int_off"], bt["feat_ids"],
+                                  bt["a_ids"], bt["a_int_ids"], bt["u_ids"], bt["u_wgt"], s._y)
+        reps = 50
+        d = {"parse": _kernel_ms(parse, reps), "model": _kernel_ms(lambda: m.predict(bt), reps),
+             "request_bytes": int(lens.sum())}
+        assert int(err.item()) == -1
+        d["parse_over_model"] = d["parse"] / d["model"]
+        res["device_ms"][str(n)] = d
+        print(n, d, flush=True)
+    print(json.dumps(res))
+    os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+    with open(a.out, "w") as fh:
+        json.dump(res, fh, indent=1)
+
+
+if __name__ == "__main__":
+    main()
