@@ -41,15 +41,17 @@ def log_loss(p, z, eps=LOG_EPS):
     return losses.sum() / losses.numel()
 
 
-def head_reference(y_ctr, y_cvr, y, z, w_ctr, w_cvr, dtype=torch.float32):
+def head_reference(y_ctr, y_cvr, y, z, w_ctr, w_cvr, dtype=torch.float32, pt=None, pv=None):
     """The head gradient csrc/esmm.cu implements, one rounded op at a time in TF's autodiff order (include/ctr_b200.h,
-    ctr_esmm_head); fp32 like the kernel, or fp64 to check the derivation.
-    Returns (pctr, pcvr, pctcvr, ctr_loss, cvr_loss, d_ctr, d_cvr)."""
+    ctr_esmm_head); fp32 like the kernel, or fp64 to check the derivation.  Given pt / pv (e.g. the kernel's own
+    sigmoids), the chain starts from them instead of recomputing the sigmoids, so every later op can be compared bit
+    for bit.  Returns (pctr, pcvr, pctcvr, ctr_loss, cvr_loss, d_ctr, d_cvr)."""
     f = dtype
     one = torch.ones((), dtype=f)
     n = y_ctr.numel()
     a, c, t, zz = y_ctr.to(f), y_cvr.to(f), y.to(f), z.to(f)
-    pt, pv = tfs.sigmoid(a), tfs.sigmoid(c)
+    pt = tfs.sigmoid(a) if pt is None else pt.to(f)
+    pv = tfs.sigmoid(c) if pv is None else pv.to(f)
     p = pt * pv
     g_ctr = torch.tensor(w_ctr, dtype=f) / torch.tensor(float(n), dtype=f)
     g_cvr = torch.tensor(w_cvr, dtype=f) / torch.tensor(float(n), dtype=f)
