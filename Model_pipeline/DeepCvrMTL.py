@@ -11,7 +11,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from tf_repos_b200 import flags  # noqa: E402
 from tf_repos_b200.flags import FLAGS  # noqa: E402
 
-flags.define_common(embedding_size=32, batch_size=64)
+flags.define_common(embedding_size=32, batch_size=64, checkpoint_format=False)
 flags.DEFINE_float("ctr_task_wgt", 0.5, "loss weight of ctr task")     # DeepCvrMTL.py:49
 
 

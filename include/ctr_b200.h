@@ -681,6 +681,16 @@ size_t ctr_aliccp_sample_order_workspace_bytes(int64_t n_samples);
 int ctr_aliccp_sample_order(uint64_t* s_key, int64_t* s_val, int64_t n_samples, int64_t parts, int64_t* part_bytes,
                             void* ws, size_t ws_bytes, ctr_stream_t stream);
 
+/* ---- CRC-32C of whole tensors (TensorFlow checkpoint bundles; DESIGN.md §2.11) ---------------------------------------
+ * ranges: device int64 [n][2] = {address, length in bytes}.  An address needs only 4-byte alignment; a length may be 0
+ * or exceed 2^32.  total_bytes >= the sum of the lengths (it sizes the grid and the workspace of
+ * ctr_crc32c_workspace_bytes(n, total_bytes) bytes).  crc[r] = the standard CRC-32C of range r (initial value and
+ * final XOR 0xFFFFFFFF, what tfrecord.crc32c returns); masked[r] = ((crc >> 15) | (crc << 17)) + 0xA282EAD8 (mod 2^32),
+ * the value a bundle's BundleEntryProto.crc32c holds.  Either output may be NULL, not both.  Deterministic. */
+size_t ctr_crc32c_workspace_bytes(int n, int64_t total_bytes);
+int ctr_crc32c_ranges(const int64_t* ranges, int n, int64_t total_bytes, uint32_t* crc, uint32_t* masked, void* ws,
+                      size_t ws_bytes, ctr_stream_t stream);
+
 /* ---- table initialisation (glorot_normal_initializer, DeepFM.py:115-116; truncated at 2 sigma) --- */
 int ctr_init_trunc_normal(float* t, int64_t n, float stddev, uint64_t seed, ctr_stream_t stream);
 int ctr_fill(float* t, int64_t n, float value, ctr_stream_t stream);

@@ -151,6 +151,8 @@ SIGNATURES = {
                                        c_int64, P, P, P, c_size_t, P]),
     "ctr_aliccp_sample_order_workspace_bytes": (c_size_t, [c_int64]),
     "ctr_aliccp_sample_order": (c_int, [P, P, c_int64, c_int64, P, P, c_size_t, P]),
+    "ctr_crc32c_workspace_bytes": (c_size_t, [c_int, c_int64]),
+    "ctr_crc32c_ranges": (c_int, [P, c_int, c_int64, P, P, P, c_size_t, P]),
     "ctr_init_trunc_normal": (c_int, [P, c_int64, c_float, c_uint64, P]),
     "ctr_fill": (c_int, [P, c_int64, c_float, P]),
 }

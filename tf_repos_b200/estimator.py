@@ -46,7 +46,19 @@ def _ckpt_path(model_dir: str) -> str:
     return os.path.join(model_dir, "ctr_b200.ckpt")
 
 
+def _tf_format() -> bool:
+    """--checkpoint_format=tf: model_dir holds TensorFlow bundles (tf_checkpoint.py) instead of ctr_b200.ckpt."""
+    fmt = getattr(FLAGS, "checkpoint_format", "b200")
+    if fmt not in ("b200", "tf"):
+        raise SystemExit("checkpoint_format=%r: must be one of {b200, tf}" % fmt)
+    return fmt == "tf"
+
+
 def save_checkpoint(model, model_dir: str):
+    if _tf_format():
+        from . import tf_checkpoint
+        tf_checkpoint.save(model, model_dir)
+        return
     os.makedirs(model_dir, exist_ok=True)
     state = {"variables": {k: v.detach().cpu() for k, v in model.variables().items()},
              "table_slots": {t.name: [s.cpu() for s in t.slots] for t in model.tables},
@@ -56,6 +68,15 @@ def save_checkpoint(model, model_dir: str):
 
 
 def restore_checkpoint(model, model_dir: str) -> bool:
+    if _tf_format():
+        from . import tf_checkpoint
+        p = tf_checkpoint.latest_checkpoint(model_dir)
+        if p is None:
+            return False
+        # a PREDICT / EVAL graph has no optimizer: only training needs the slots in the bundle
+        tf_checkpoint.restore(model, p, variables_only=getattr(FLAGS, "task_type", "train") != "train")
+        print("restored checkpoint %s at global_step %d" % (p, model.global_step))
+        return True
     p = _ckpt_path(model_dir)
     if not os.path.exists(p):
         return False

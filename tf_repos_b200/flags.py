@@ -76,8 +76,12 @@ def DEFINE_boolean(name, default, help=""):
 
 
 def define_common(num_threads=16, embedding_size=32, batch_size=64, learning_rate=0.0005, l2_reg=0.0001,
-                  deep_layers="256,128,64", dropout="0.5,0.5,0.5", loss_type=True, batch_norm=True):
-    """The flag block every libsvm script shares (DeepFM.py:34-60; per-model defaults: SURVEY.md app. B)."""
+                  deep_layers="256,128,64", dropout="0.5,0.5,0.5", loss_type=True, batch_norm=True,
+                  checkpoint_format=True):
+    """The flag block every libsvm script shares (DeepFM.py:34-60; per-model defaults: SURVEY.md app. B).
+    checkpoint_format=False leaves out --checkpoint_format: DeepCvrMTL.py keeps the reference's flags plus only
+    --update_mode / --input_parse, and its model_dir is always ctr_b200.ckpt (tf_checkpoint.save / restore serve ESMM
+    from Python)."""
     DEFINE_integer("dist_mode", 0, "distribuion mode {0-loacal, 1-single_dist, 2-multi_dist}")
     DEFINE_string("ps_hosts", "", "Comma-separated list of hostname:port pairs")
     DEFINE_string("worker_hosts", "", "Comma-separated list of hostname:port pairs")
@@ -110,3 +114,6 @@ def define_common(num_threads=16, embedding_size=32, batch_size=64, learning_rat
     # engine-only flag (not in the reference): how the TF-exact table update is scheduled
     DEFINE_string("update_mode", "exact_deferred", "{exact, exact_deferred, lazy}: see tf_repos_b200/engine.py (SparseUpdater)")
     DEFINE_string("input_parse", "device", "{device, host}: where the libsvm text is tokenised (same values)")
+    if checkpoint_format:   # engine-only flag: which program reads model_dir (ctr_b200.ckpt, or TensorFlow's V2 bundles)
+        DEFINE_string("checkpoint_format", "b200", "{b200, tf}: ctr_b200.ckpt, or TensorFlow checkpoints "
+                      "(model.ckpt-<step>.index/.data-*, see tf_repos_b200/tf_checkpoint.py)")

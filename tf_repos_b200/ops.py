@@ -755,3 +755,35 @@ def init_trunc_normal(t, stddev: float, seed: int):
 
 def fill(t, value: float):
     check(_L.ctr_fill(_p(t, torch.float32, "t"), t.numel(), float(value), _stream()), "ctr_fill")
+
+
+def crc32c_workspace_bytes(n: int, total_bytes: int) -> int:
+    return int(_L.ctr_crc32c_workspace_bytes(n, total_bytes))
+
+
+def crc32c(tensors, crc=None, masked=None, ws=None):
+    """CRC-32C of the bytes of each contiguous CUDA tensor (any dtype; a uint8 view gives any 4-byte aligned byte
+    range) in one ctr_crc32c_ranges call on the current stream.  Returns device int32 tensors (crc, masked): the
+    standard CRC-32C and TensorFlow's masked form, as the low 32 bits of each element (`& 0xFFFFFFFF` on the host)."""
+    tensors = list(tensors)
+    n = len(tensors)
+    if n == 0:
+        raise CtrError("crc32c: no tensors")
+    dev = tensors[0].device
+    rng = torch.empty(n, 2, dtype=torch.int64)
+    for i, t in enumerate(tensors):
+        if t.device != dev:
+            raise CtrError(f"crc32c: tensor {i} is on {t.device}, not {dev}")
+        rng[i, 0], rng[i, 1] = _p(t, None, f"tensors[{i}]"), t.numel() * t.element_size()
+    total = int(rng[:, 1].sum())
+    rng = rng.to(dev)
+    i32 = dict(dtype=torch.int32, device=dev)
+    crc = torch.empty(n, **i32) if crc is None else crc
+    masked = torch.empty(n, **i32) if masked is None else masked
+    need = crc32c_workspace_bytes(n, total)
+    if ws is None or ws.numel() < need:
+        ws = torch.empty(need, dtype=torch.uint8, device=dev)
+    check(_L.ctr_crc32c_ranges(_p(rng, torch.int64, "ranges"), n, total, _p(crc, torch.int32, "crc"),
+                               _p(masked, torch.int32, "masked"), _p(ws, torch.uint8, "ws"), ws.numel(), _stream()),
+          "ctr_crc32c_ranges")
+    return crc, masked
