@@ -64,8 +64,9 @@ def test_criteo_like_file_matches_host_and_oracle(tmp_path):
         assert np.array_equal(dev[0][r].cpu().numpy(), o_ids)
         assert np.array_equal(dev[1][r].cpu().numpy().view(np.uint32), o_vals.view(np.uint32))
         assert np.float32(dev[2][r].item()) == o_lab
-    d = input_fn.decode_libsvm_file_device(path, 39)
-    assert np.array_equal(d[0].cpu().numpy(), h[0]) and np.array_equal(d[1].cpu().numpy(), h[1])
+    (d, _), = input_fn.input_fn(path, batch_size=3000, field_size=39, device="cuda")
+    assert np.array_equal(d["feat_ids"][..., 0].cpu().numpy(), h[0])
+    assert np.array_equal(d["feat_vals"][..., 0].cpu().numpy(), h[1])
     # unterminated last line, CRLF, runs of spaces
     data2 = data.rstrip(b"\n").replace(b"\n", b"\r\n", 5).replace(b" ", b"   ", 7)
     _same(_device(data2, 39), _host(data2, 39))
@@ -139,3 +140,59 @@ def test_input_fn_device_batches_equal_host_batches(tmp_path):
         assert df["feat_ids"].is_cuda and df["feat_ids"].shape == hf["feat_ids"].shape
         assert torch.equal(df["feat_ids"].cpu(), hf["feat_ids"]) and torch.equal(df["feat_vals"].cpu(), hf["feat_vals"])
         assert torch.equal(dl.cpu(), hl)
+
+
+def _lines(n, F, seed):
+    from tf_repos_b200 import synth
+    ids, vals, labels = (t.numpy() for t in synth.criteo_batch(n, 5000, F, seed=seed))
+    return ["%d " % labels[r] + " ".join("%d:%.6g" % (ids[r, f], vals[r, f]) for f in range(F)) for r in range(n)]
+
+
+def _batches(files, device, **kw):
+    """the batches as host tensors, or the ValueError the generator raised"""
+    from tf_repos_b200 import input_fn
+    out = []
+    try:
+        for feats, labels in input_fn.input_fn(files, device=device, **kw):
+            out.append((feats["feat_ids"].cpu(), feats["feat_vals"].cpu(), labels.cpu()))
+    except ValueError as e:
+        return str(e)
+    return out
+
+
+@pytest.mark.parametrize("field_size", [0, 15])
+def test_streamed_device_batches_equal_host_batches(tmp_path, field_size):
+    lines = _lines(300, 15, 30)
+    lines[120] = ""                                                   # declined pieces in the middle of the file
+    for row, pair in ((150, "3:0.12345678901234567"), (180, "4:inf"), (200, "5:%s1.5" % ("0" * 5000))):
+        lines[row] = lines[row].replace(" ", " %s " % pair, 1).rsplit(" ", 1)[0]     # 17 digits, inf, a long line
+    files = [os.path.join(tmp_path, n) for n in ("tr0.libsvm", "empty.libsvm", "tr1.libsvm")]
+    open(files[0], "w").write("\n".join(lines) + "\n")
+    open(files[1], "w").write("")
+    open(files[2], "w").write("\n".join(_lines(97, 15, 31)))           # no '\n' at the end
+    assert os.path.getsize(files[0]) > 10 * 4096
+    kw = dict(batch_size=37, num_epochs=3, field_size=field_size)
+    host = _batches(files, None, **kw)
+    dev = _batches(files, "cuda", chunk_bytes=4096, **kw)
+    assert [b[2].shape[0] for b in host] == [37] * (3 * 396 // 37) + [3 * 396 % 37]
+    assert len(dev) == len(host)
+    for d, h in zip(dev, host):
+        assert all(a.dtype == b.dtype and a.shape == b.shape for a, b in zip(d, h))
+        assert torch.equal(d[0], h[0]) and torch.equal(d[1].view(torch.int32), h[1].view(torch.int32))
+        assert torch.equal(d[2].view(torch.int32), h[2].view(torch.int32))
+    assert torch.isinf(torch.cat([h[1] for h in host])).any()
+
+
+def test_streamed_device_error_is_the_host_error(tmp_path, monkeypatch):
+    from tf_repos_b200 import input_fn, text_chunks
+    monkeypatch.setattr(input_fn, "CHUNK", 4096)                     # the host path cuts the device path's pieces
+    lines = _lines(100, 15, 32)
+    lines[30] = lines[30].rsplit(" ", 1)[0]                           # 14 pairs
+    path = os.path.join(tmp_path, "tr.libsvm")
+    open(path, "w").write("\n".join(lines) + "\n")
+    n0, n1 = (p.count(b"\n") for p in list(text_chunks.pieces(path, 4096))[:2])
+    assert n0 <= 30 < n0 + n1                                         # the ragged row is in the second piece
+    host = _batches([path], None, batch_size=8)
+    dev = _batches([path], "cuda", batch_size=8, chunk_bytes=4096)
+    assert isinstance(host, str) and dev == host
+    assert "row %d has 14 id:val pairs, field_size is 15" % (30 - n0) in host

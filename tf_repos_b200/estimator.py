@@ -18,7 +18,7 @@ from typing import Callable, Dict
 import numpy as np
 import torch
 
-from .flags import FLAGS
+from .flags import FLAGS, input_parse_device
 from .input_fn import input_fn
 
 
@@ -128,9 +128,9 @@ def run(build_model: Callable[[], object], model_name: str):
     restore_checkpoint(model, FLAGS.model_dir)
     dev = model.device
     F = FLAGS.field_size
+    parse_dev = input_parse_device(dev)
 
     def batches(files, epochs):
-        parse_dev = dev if getattr(FLAGS, "input_parse", "device") == "device" else None
         for feats, labels in input_fn(files, num_epochs=epochs, batch_size=FLAGS.batch_size, field_size=F,
                                       device=parse_dev):
             yield (feats["feat_ids"].reshape(-1, F).to(dev, non_blocking=True),

@@ -117,3 +117,11 @@ def define_common(num_threads=16, embedding_size=32, batch_size=64, learning_rat
     if checkpoint_format:   # engine-only flag: which program reads model_dir (ctr_b200.ckpt, or TensorFlow's V2 bundles)
         DEFINE_string("checkpoint_format", "b200", "{b200, tf}: ctr_b200.ckpt, or TensorFlow checkpoints "
                       "(model.ckpt-<step>.index/.data-*, see tf_repos_b200/tf_checkpoint.py)")
+
+
+def input_parse_device(dev):
+    """--input_parse, where the input text is tokenised: dev for "device", None (the host parser) for "host".  Any
+    other value stops the script."""
+    if FLAGS.input_parse not in ("device", "host"):
+        raise SystemExit("input_parse must be one of {device, host}")
+    return dev if FLAGS.input_parse == "device" else None

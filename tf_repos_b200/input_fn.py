@@ -19,29 +19,22 @@ from typing import Dict, Iterator, List, Sequence, Tuple, Union
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, ops, text_chunks
 
 _L = _lib.raw()
-CHUNK = 32 << 20  # bytes per parse task
+CHUNK = 32 << 20  # bytes per piece of text: a parse task of the host path, a piece of the device path
 
 
-def _split_chunks(data: bytes) -> List[Tuple[int, int]]:
-    out, pos, n = [], 0, len(data)
-    while pos < n:
-        end = min(n, pos + CHUNK)
-        if end < n:
-            nl = data.find(b"\n", end)
-            end = n if nl < 0 else nl + 1
-        out.append((pos, end))
-        pos = end
-    return out
+def _max_rows(n_bytes: int, F: int) -> int:
+    return max(1, n_bytes // max(2 * F + 2, 1))  # every row has >= 2F+2 characters
 
 
 def _parse(data: bytes, lo: int, hi: int, F: int):
+    """ctr_parse_libsvm of data[lo:hi], whole lines; the row numbers in its errors count from lo."""
     view = memoryview(data)[lo:hi]
     buf = ctypes.c_char_p(bytes(view)) if lo or hi != len(data) else ctypes.c_char_p(data)
     n_bytes = hi - lo
-    max_rows = max(1, n_bytes // max(2 * F + 2, 1))  # every row has >= 2F+2 characters
+    max_rows = _max_rows(n_bytes, F)
     ids = np.empty((max_rows, F), dtype=np.int32)
     vals = np.empty((max_rows, F), dtype=np.float32)
     labels = np.empty(max_rows, dtype=np.float32)
@@ -53,126 +46,82 @@ def _parse(data: bytes, lo: int, hi: int, F: int):
     return ids[:rows], vals[:rows], labels[:rows]
 
 
+def _count_fields(path: str) -> int:
+    """The id:val pairs of the file's first line that is not blank (0 when there is none)."""
+    for data in text_chunks.chunks(path, 1 << 16):
+        if data.strip(b" \r\n"):
+            return _L.ctr_libsvm_count_fields(data, len(data))
+    return 0
+
+
 def decode_libsvm_file(path: str, field_size: int = 0, threads: int = 10):
     """Whole file -> (ids int32 [n,F], vals f32 [n,F], labels f32 [n]).  field_size 0 = infer from line 1."""
-    with open(path, "rb") as fh:
-        data = fh.read()
-    F = field_size or _L.ctr_libsvm_count_fields(data, len(data))
-    if F <= 0 or len(data) == 0:
+    F = field_size or _count_fields(path)
+    parts = list(text_chunks.pieces(path, CHUNK)) if F > 0 else []
+    if not parts:
         return (np.empty((0, max(field_size, 0)), np.int32), np.empty((0, max(field_size, 0)), np.float32),
                 np.empty(0, np.float32))
-    chunks = _split_chunks(data)
-    if len(chunks) == 1:
-        parts = [_parse(data, chunks[0][0], chunks[0][1], F)]
-    else:
-        with ThreadPoolExecutor(max_workers=threads) as ex:
-            parts = list(ex.map(lambda c: _parse(data, c[0], c[1], F), chunks))
-    return (np.concatenate([p[0] for p in parts]), np.concatenate([p[1] for p in parts]),
-            np.concatenate([p[2] for p in parts]))
-
-
-def decode_libsvm_file_device(path: str, field_size: int = 0, device="cuda", chunk_bytes: int = 256 << 20):
-    """Whole file -> (ids, vals, labels) as CUDA tensors, tokenised on the GPU (ctr_parse_libsvm_device): the file
-    is read in chunks cut at line ends, copied to the device and parsed there; a chunk the device parser
-    declines (blank/malformed line, a number only strtof may decide) is re-parsed by the host parser, so results and
-    error messages are exactly those of decode_libsvm_file."""
-    from . import ops
-    with open(path, "rb") as fh:
-        data = fh.read()
-    F = field_size or _L.ctr_libsvm_count_fields(data, len(data))
-    dev = torch.device(device)
-    if F <= 0 or len(data) == 0:
-        return (torch.empty(0, max(field_size, 0), dtype=torch.int32, device=dev),
-                torch.empty(0, max(field_size, 0), dtype=torch.float32, device=dev),
-                torch.empty(0, dtype=torch.float32, device=dev))
-    parts = []
-    pos, n = 0, len(data)
-    while pos < n:
-        end = min(n, pos + chunk_bytes)
-        if end < n:
-            nl = data.find(b"\n", end)
-            end = n if nl < 0 else nl + 1
-        raw = np.frombuffer(data, dtype=np.uint8, count=end - pos, offset=pos)
-        text = torch.from_numpy(raw.copy()).to(dev, non_blocking=False)
-        max_rows = max(1, (end - pos) // max(2 * F + 2, 1))
-        ids, vals, labels, consumed, needs_host = ops.parse_libsvm_device(text, F, max_rows, final_chunk=True)
-        if needs_host or consumed != end - pos:
-            h = _parse(data, pos, end, F)
-            ids, vals, labels = (torch.from_numpy(a.copy()).to(dev) for a in h)
-        parts.append((ids, vals, labels))
-        pos = end
     if len(parts) == 1:
-        return parts[0]
-    return tuple(torch.cat([p[k] for p in parts]) for k in range(3))
+        return _parse(parts[0], 0, len(parts[0]), F)
+    with ThreadPoolExecutor(max_workers=threads) as ex:
+        parsed = list(ex.map(lambda data: _parse(data, 0, len(data), F), parts))
+    return tuple(np.concatenate([p[k] for p in parsed]) for k in range(3))
+
+
+def _device_parts(files: List[str], num_epochs: int, field_size: int, dev: torch.device, chunk_bytes: int):
+    """(ids, vals, labels) CUDA tensors of every piece of every file, num_epochs times (text_chunks.device_parts):
+    tokenised by ctr_parse_libsvm_device, a declined piece parsed by ctr_parse_libsvm."""
+    fields = {path: field_size or _count_fields(path) for path in files}
+
+    def tokenize(path, text, n_bytes):
+        F = fields[path]
+        max_rows = _max_rows(n_bytes, F)
+        ws = text_chunks.scratch(ops.parse_libsvm_device_workspace_bytes(n_bytes, max_rows), text.device)
+        ids, vals, labels, info = ops.parse_libsvm_device_core(text, n_bytes, F, max_rows, ws)
+        return (ids, vals, labels), info
+
+    def decode(path, data, line_base):
+        return _parse(data, 0, len(data), fields[path]), data.count(b"\n") + (not data.endswith(b"\n"))
+
+    return text_chunks.device_parts([p for p in files if fields[p] > 0], num_epochs, dev, chunk_bytes, tokenize, decode)
+
+
+def _host_parts(files: List[str], num_epochs: int, field_size: int, perform_shuffle: bool):
+    for _ in range(num_epochs):
+        for path in files:
+            ids, vals, labels = decode_libsvm_file(path, field_size)
+            if perform_shuffle:  # tf.data shuffle(buffer_size=256) window semantics
+                buf: List[int] = []
+                order = []
+                for i in range(len(labels)):
+                    if len(buf) < 256:
+                        buf.append(i)
+                        continue
+                    j = random.randrange(256)
+                    order.append(buf[j]); buf[j] = i
+                random.shuffle(buf)
+                order.extend(buf)
+                ids, vals, labels = ids[order], vals[order], labels[order]
+            yield torch.from_numpy(ids), torch.from_numpy(vals), torch.from_numpy(labels)
 
 
 def _pin(t: torch.Tensor) -> torch.Tensor:
     return t.pin_memory() if torch.cuda.is_available() else t
 
 
-def _input_fn_device(files, batch_size, num_epochs, field_size, device):
-    """Same batching (repeat before batch, last partial batch kept), tensors tokenised on and left on the GPU."""
-    carry = None
-    for _ in range(num_epochs):
-        for path in files:
-            ids, vals, labels = decode_libsvm_file_device(path, field_size, device)
-            if carry is not None:
-                ids, vals, labels = (torch.cat([c, t]) for c, t in zip(carry, (ids, vals, labels)))
-                carry = None
-            n_full = (labels.shape[0] // batch_size) * batch_size
-            for lo in range(0, n_full, batch_size):
-                hi = lo + batch_size
-                yield ({"feat_ids": ids[lo:hi].unsqueeze(-1), "feat_vals": vals[lo:hi].unsqueeze(-1)}, labels[lo:hi])
-            if n_full < labels.shape[0]:
-                carry = (ids[n_full:], vals[n_full:], labels[n_full:])
-    if carry is not None and carry[2].shape[0]:
-        yield ({"feat_ids": carry[0].unsqueeze(-1), "feat_vals": carry[1].unsqueeze(-1)}, carry[2])
-
-
 def input_fn(filenames: Union[str, Sequence[str]], batch_size: int = 32, num_epochs: int = 1,
-             perform_shuffle: bool = False, field_size: int = 0,
-             device=None) -> Iterator[Tuple[Dict[str, torch.Tensor], torch.Tensor]]:
-    """device=None: host parser, pinned host tensors.  device="cuda[:i]": the text is copied to the GPU and
-    tokenised there (ctr_parse_libsvm_device); batches are CUDA tensors.  Identical values either way."""
+             perform_shuffle: bool = False, field_size: int = 0, device=None,
+             chunk_bytes: int = CHUNK) -> Iterator[Tuple[Dict[str, torch.Tensor], torch.Tensor]]:
+    """device=None: host parser, pinned host tensors.  device="cuda[:i]": the text is streamed to the GPU in pieces of
+    chunk_bytes and tokenised there (ctr_parse_libsvm_device); batches are CUDA tensors.  Identical values either way.
+    perform_shuffle runs on the host parser."""
     print("Parsing", filenames)  # DeepFM.py:64
     files = [filenames] if isinstance(filenames, str) else list(filenames)
     if device is not None and not perform_shuffle:
-        yield from _input_fn_device(files, batch_size, num_epochs, field_size, device)
+        parts = _device_parts(files, num_epochs, field_size, torch.device(device), chunk_bytes)
+        for ids, vals, labels in text_chunks.batches(parts, batch_size):
+            yield {"feat_ids": ids.unsqueeze(-1), "feat_vals": vals.unsqueeze(-1)}, labels
         return
-
-    def rows():
-        for _ in range(num_epochs):
-            for path in files:
-                ids, vals, labels = decode_libsvm_file(path, field_size)
-                if perform_shuffle:  # tf.data shuffle(buffer_size=256) window semantics
-                    buf: List[int] = []
-                    order = []
-                    for i in range(len(labels)):
-                        if len(buf) < 256:
-                            buf.append(i)
-                            continue
-                        j = random.randrange(256)
-                        order.append(buf[j]); buf[j] = i
-                    random.shuffle(buf)
-                    order.extend(buf)
-                    ids, vals, labels = ids[order], vals[order], labels[order]
-                yield ids, vals, labels
-
-    carry = None
-    for ids, vals, labels in rows():
-        if carry is not None:
-            ids = np.concatenate([carry[0], ids]); vals = np.concatenate([carry[1], vals])
-            labels = np.concatenate([carry[2], labels])
-            carry = None
-        n_full = (len(labels) // batch_size) * batch_size
-        for lo in range(0, n_full, batch_size):
-            hi = lo + batch_size
-            yield ({"feat_ids": _pin(torch.from_numpy(ids[lo:hi].copy()).unsqueeze(-1)),
-                    "feat_vals": _pin(torch.from_numpy(vals[lo:hi].copy()).unsqueeze(-1))},
-                   _pin(torch.from_numpy(labels[lo:hi].copy())))
-        if n_full < len(labels):
-            carry = (ids[n_full:], vals[n_full:], labels[n_full:])
-    if carry is not None and len(carry[2]):
-        yield ({"feat_ids": _pin(torch.from_numpy(carry[0].copy()).unsqueeze(-1)),
-                "feat_vals": _pin(torch.from_numpy(carry[1].copy()).unsqueeze(-1))},
-               _pin(torch.from_numpy(carry[2].copy())))
+    parts = _host_parts(files, num_epochs, field_size, perform_shuffle)
+    for ids, vals, labels in text_chunks.batches(parts, batch_size):
+        yield {"feat_ids": _pin(ids.unsqueeze(-1)), "feat_vals": _pin(vals.unsqueeze(-1))}, _pin(labels)

@@ -654,21 +654,37 @@ def wd_serve_input(data, offsets, example_base: int, emb, wide_cat, wide_num, wi
           "ctr_wd_serve_input")
 
 
-def parse_libsvm_device(text: torch.Tensor, F: int, max_rows: int, final_chunk: bool = True):
-    """decode_libsvm (DeepFM.py:65-81) on a uint8 CUDA tensor of text.  Returns (ids int32 [rows,F], vals f32 [rows,F],
-    labels f32 [rows], consumed bytes, needs_host) -- when needs_host is True the chunk holds something only the host
-    parser may decide (blank/malformed line, exotic number) and the outputs must be discarded."""
-    assert text.is_cuda and text.dtype == torch.uint8 and text.is_contiguous()
-    dev, n = text.device, text.numel()
+def parse_libsvm_device_workspace_bytes(n_bytes: int, max_rows: int) -> int:
+    return int(_L.ctr_parse_libsvm_device_workspace_bytes(n_bytes, max_rows))
+
+
+def parse_libsvm_device_core(text: torch.Tensor, n_bytes: int, F: int, max_rows: int, ws: torch.Tensor,
+                             final_chunk: bool = True):
+    """decode_libsvm (DeepFM.py:65-81) of text[:n_bytes], a uint8 CUDA tensor; ws holds at least
+    parse_libsvm_device_workspace_bytes(n_bytes, max_rows) device bytes.  Returns (ids int32 [max_rows,F], vals f32
+    [max_rows,F], labels f32 [max_rows], info int64 [5] on the device) without waiting for the device: info = (rows,
+    bytes consumed, blank lines, malformed lines, lines with a number for the host), and when any of the last three is
+    non-zero the piece holds something only the host parser may decide and the outputs must be discarded."""
+    assert text.is_cuda and text.dtype == torch.uint8 and text.is_contiguous() and 0 <= n_bytes <= text.numel()
+    dev = text.device
     ids = torch.empty(max_rows, F, dtype=torch.int32, device=dev)
     vals = torch.empty(max_rows, F, dtype=torch.float32, device=dev)
     labels = torch.empty(max_rows, dtype=torch.float32, device=dev)
     info = torch.empty(5, dtype=torch.int64, device=dev)
-    ws_bytes = int(_L.ctr_parse_libsvm_device_workspace_bytes(n, max_rows))
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    check(_L.ctr_parse_libsvm_device(text.data_ptr(), n, F, max_rows, int(final_chunk), ids.data_ptr(), vals.data_ptr(),
-                                     labels.data_ptr(), info.data_ptr(), ws.data_ptr(), ws_bytes, _stream()),
-          "ctr_parse_libsvm_device")
+    check(_L.ctr_parse_libsvm_device(text.data_ptr(), n_bytes, F, max_rows, int(final_chunk), ids.data_ptr(),
+                                     vals.data_ptr(), labels.data_ptr(), info.data_ptr(), _p(ws, torch.uint8, "ws"),
+                                     ws.numel(), _stream()), "ctr_parse_libsvm_device")
+    return ids, vals, labels, info
+
+
+def parse_libsvm_device(text: torch.Tensor, F: int, max_rows: int, final_chunk: bool = True):
+    """parse_libsvm_device_core of the whole of text with its own workspace, waiting for the result.  Returns (ids
+    int32 [rows,F], vals f32 [rows,F], labels f32 [rows], consumed bytes, needs_host) -- when needs_host is True the
+    chunk holds something only the host parser may decide (blank/malformed line, exotic number) and the outputs must
+    be discarded."""
+    n = text.numel()
+    ws = torch.empty(parse_libsvm_device_workspace_bytes(n, max_rows), dtype=torch.uint8, device=text.device)
+    ids, vals, labels, info = parse_libsvm_device_core(text, n, F, max_rows, ws, final_chunk)
     rows, consumed, blank, bad, host = (int(x) for x in info.tolist())
     return ids[:rows], vals[:rows], labels[:rows], consumed, bool(blank or bad or host)
 

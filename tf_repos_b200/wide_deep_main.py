@@ -20,8 +20,9 @@ from typing import Iterator, List, Sequence, Tuple
 import numpy as np
 import torch
 
+from . import ops, text_chunks
 from .estimator import auc_200
-from .flags import FLAGS
+from .flags import FLAGS, input_parse_device
 
 N_NUM, N_CAT = 13, 26
 
@@ -63,122 +64,41 @@ def decode_csv_bytes(data: bytes, path: str, line_base: int = 0):
     return arrays + (n_lines,)
 
 
-def _csv_device_parts(files: Sequence[str], num_epochs: int, dev: torch.device, chunk_bytes: int):
-    """(labels, dense, cat) CUDA tensors of every piece of every file, num_epochs times: the file is read in pieces of
-    whole lines (text_chunks.pieces), a piece is staged in pinned memory, copied on a side stream and tokenised by
-    ctr_parse_csv_device; a piece the kernel declines is decoded by decode_csv_bytes, which owns the error messages.
-    Piece i+1 is read and its copy queued before piece i's counters are read back, so the copy runs under piece i's
-    kernel and under whatever the consumer queues for piece i's batches; that read-back is the only synchronise."""
-    from . import ops, text_chunks
-    main, side = torch.cuda.current_stream(dev), torch.cuda.Stream(dev)
-    copied = [torch.cuda.Event(), torch.cuda.Event()]
-    host = [torch.empty(max(chunk_bytes, 1), dtype=torch.uint8, pin_memory=True) for _ in range(2)]
-    text = [text_chunks.scratch(chunk_bytes, dev) for _ in range(2)]
-    ws = text_chunks.scratch(0, dev)
-
-    def stream():
-        for _ in range(num_epochs):
-            for path in files:
-                line_base = [0]                               # advanced by the consumer of each piece
-                for data in text_chunks.pieces(path, chunk_bytes):
-                    yield path, line_base, data
-
-    def upload(i: int, data: bytes):
-        """stage piece i and queue its copy.  Piece i-2's counters have been read back by now, so its copy and its
-        kernel, the last users of host[s] and text[s], are done."""
-        s, n = i % 2, len(data)
-        if host[s].numel() < n:                               # one line longer than chunk_bytes
-            host[s] = torch.empty(n, dtype=torch.uint8, pin_memory=True)
-            text[s] = text_chunks.scratch(n, dev)
-            side.wait_stream(main)                            # the new block may be memory main's queue still reads
-        host[s].numpy()[:n] = np.frombuffer(data, dtype=np.uint8)
-        with torch.cuda.stream(side):
-            text[s][:n].copy_(host[s][:n], non_blocking=True)
-            copied[s].record(side)
-
-    it = stream()
-    nxt = next(it, None)
-    if nxt is not None:
-        upload(0, nxt[2])
-    i = 0
-    try:
-        while nxt is not None:
-            path, line_base, data = nxt
-            s, n = i % 2, len(data)
-            max_rows = data.count(b"\n") + 1
-            need = ops.parse_csv_device_workspace_bytes(n, max_rows)
-            if ws.numel() < need:
-                ws = text_chunks.scratch(need, dev)
-            main.wait_event(copied[s])
-            labels, dense, cat, info = ops.parse_csv_device(text[s], n, 1 + N_NUM, N_CAT, max_rows, ws)
-            nxt = next(it, None)
-            if nxt is not None:
-                upload(i + 1, nxt[2])
-            rows, consumed, blank, bad, number = info.tolist()
-            if blank or bad or number or consumed != n:
-                labels, dense, cat, n_lines = decode_csv_bytes(data, path, line_base[0])
-                labels, dense, cat = (torch.from_numpy(a).to(dev) for a in (labels, dense, cat))
-                line_base[0] += n_lines
-            else:
-                labels, dense, cat = labels[:rows], dense[:rows], cat[:rows]
-                line_base[0] += rows
-            yield labels, dense, cat
-            i += 1
-    finally:
-        side.synchronize()                                    # no copy out of the pinned buffers is left in flight
-
-
-def _input_fn_device(files, num_epochs, batch_size, dev, chunk_bytes):
-    """The host generator's batching over device pieces: repeat before batch, batches straddle pieces, files and
-    epochs, the last partial batch is kept."""
-    carry = None                                              # fewer than batch_size rows waiting for the next piece
-    for part in _csv_device_parts(files, num_epochs, dev, chunk_bytes):
-        lo, n = 0, part[0].shape[0]
-        if carry is not None:
-            lo = min(batch_size - carry[0].shape[0], n)
-            carry = tuple(torch.cat([c, p[:lo]]) for c, p in zip(carry, part))
-            if carry[0].shape[0] < batch_size:
-                continue
-            yield carry[1], carry[2], carry[0]
-            carry = None
-        n_full = lo + ((n - lo) // batch_size) * batch_size
-        for b in range(lo, n_full, batch_size):
-            yield part[1][b:b + batch_size], part[2][b:b + batch_size], part[0][b:b + batch_size]
-        if n_full < n:
-            carry = tuple(p[n_full:] for p in part)
-    if carry is not None:
-        yield carry[1], carry[2], carry[0]
-
-
 CSV_CHUNK = 16 << 20  # bytes of text per piece of the device path
+
+
+def _tokenize(path, text, n_bytes):
+    max_rows = n_bytes // (1 + N_NUM + N_CAT) + 1      # an accepted line: 39 ',' and a '\n' (the last: maybe not)
+    ws = text_chunks.scratch(ops.parse_csv_device_workspace_bytes(n_bytes, max_rows), text.device)
+    labels, dense, cat, info = ops.parse_csv_device(text, n_bytes, 1 + N_NUM, N_CAT, max_rows, ws)
+    return (dense, cat, labels), info
+
+
+def _decode(path, data, line_base):
+    labels, dense, cat, n_lines = decode_csv_bytes(data, path, line_base)
+    return (dense, cat, labels), n_lines
+
+
+def _host_parts(files: Sequence[str], num_epochs: int):
+    for _ in range(num_epochs):
+        for path in files:
+            labels, dense, cat = decode_csv_file(path)
+            yield torch.from_numpy(dense), torch.from_numpy(cat), torch.from_numpy(labels)
 
 
 def input_fn(filenames: Sequence[str], num_epochs: int, batch_size: int = 1, device=None,
              chunk_bytes: int = CSV_CHUNK) -> Iterator[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]]:
     """yields (dense f32 [B,13], cat int32 [B,26], labels f32 [B]).  device=None: host decoder, host tensors.
     device="cuda[:i]": the text is streamed to the GPU in pieces of chunk_bytes and tokenised there
-    (ctr_parse_csv_device); batches are CUDA tensors.  Identical values either way."""
+    (ctr_parse_csv_device, a declined piece decoded by decode_csv_bytes); batches are CUDA tensors.  Identical values
+    either way."""
     print("Parsing", filenames)
     files = [filenames] if isinstance(filenames, str) else list(filenames)
     if device is not None:
-        yield from _input_fn_device(files, num_epochs, batch_size, torch.device(device), chunk_bytes)
-        return
-    carry = None
-    for _ in range(num_epochs):
-        for path in files:
-            part = decode_csv_file(path)
-            if carry is not None:
-                part = tuple(np.concatenate([c, p]) for c, p in zip(carry, part))
-                carry = None
-            labels, dense, cat = part
-            n_full = (len(labels) // batch_size) * batch_size
-            for lo in range(0, n_full, batch_size):
-                hi = lo + batch_size
-                yield torch.from_numpy(dense[lo:hi].copy()), torch.from_numpy(cat[lo:hi].copy()), torch.from_numpy(labels[lo:hi].copy())
-            if n_full < len(labels):
-                carry = (labels[n_full:], dense[n_full:], cat[n_full:])
-    if carry is not None and len(carry[0]):
-        yield torch.from_numpy(carry[1].copy()), torch.from_numpy(carry[2].copy()), torch.from_numpy(carry[0].copy())
+        parts = text_chunks.device_parts(files, num_epochs, torch.device(device), chunk_bytes, _tokenize, _decode)
+    else:
+        parts = _host_parts(files, num_epochs)
+    yield from text_chunks.batches(parts, batch_size)
 
 
 def _ckpt(model_dir: str) -> str:
@@ -242,9 +162,7 @@ def run():
     restore_checkpoint(model, FLAGS.model_dir)
     dev = model.device
 
-    if FLAGS.input_parse not in ("device", "host"):
-        raise SystemExit("input_parse must be one of {device, host}")
-    parse_dev = dev if FLAGS.input_parse == "device" else None
+    parse_dev = input_parse_device(dev)
 
     def batches(files, epochs):
         for batch in input_fn(files, epochs, FLAGS.batch_size, device=parse_dev):
