@@ -22,7 +22,7 @@
 //   6 id outside [0, 2^31) (arg = key)
 #include "common.cuh"
 #include "crc32c.cuh"
-#include "example_wire.cuh"   // tr_byte, tr_u32, tr_float, tr_varint, tr_field, tr_utf8
+#include "example_wire.cuh"   // tr_map_entries, tr_feature_kind and the wire helpers
 #include "scan_sort.cuh"      // cta_scan_kernel
 
 namespace ctr {
@@ -126,34 +126,21 @@ __device__ bool tr_list(const uint8_t* d, int s, int e, TrFeat& r, void* out, in
   return true;
 }
 
-// a Feature message [s, e) read as tfrecord._parse_feature does: its first field numbered 1..3 sets the kind and the
-// values; later kind fields only set `multi`.  false = malformed.
+// a Feature message [s, e) with its values (example_wire.cuh's kind rule).  false = malformed.
 __device__ bool tr_feature(const uint8_t* d, int s, int e, TrFeat& r, void* out, int limit, int range_n) {
-  r.kind = KIND_NONE; r.count = 0; r.multi = false; r.range_bad = false;
-  for (int p = s; p < e;) {
-    TrField f;
-    p = tr_field(d, p, e, f);
-    if (p < 0) return false;
-    if (f.num < 1 || f.num > 3) continue;
-    if (r.kind != KIND_NONE) { r.multi = true; continue; }
-    if (f.wt != 2) return false;
-    r.kind = f.num;
-    if (!tr_list(d, f.vs, f.ve, r, out, limit, range_n)) return false;
-  }
-  return true;
+  r.count = 0; r.range_bad = false;
+  return tr_feature_kind(d, s, e, r, [&](int ls, int le) { return tr_list(d, ls, le, r, out, limit, range_n); });
 }
 
-// schema key of the map key [s, e): lane k compares key k.  -1 = not a schema key, -2 = not UTF-8 (the host raises)
+// schema key of the map key [s, e): lane k compares key k.  -1 = not a schema key
 __device__ int tr_match_key(const uint8_t* d, int s, int e, bool want_z) {
   const int lane = tr_lane(), n = e - s;
-  bool hit = false, high = false;
+  bool hit = false;
   if (lane < TR_KEYS && n == kTrKeyLen[lane] && (lane != TK_Z || want_z)) {
     hit = true;
     for (int i = 0; i < n && hit; ++i) hit = tr_byte(d, s + i) == (uint32_t)(uint8_t)kTrKey[lane][i];
   }
-  for (int i = lane; i < n; i += 32) high |= tr_byte(d, s + i) >= 0x80;
   const unsigned m = __ballot_sync(FULL_MASK, hit);
-  if (__any_sync(FULL_MASK, high) && !tr_utf8(d, s, e)) return -2;
   return m ? __ffs(m) - 1 : -1;
 }
 
@@ -168,43 +155,20 @@ __device__ __forceinline__ int tr_range_n(int key) {
                                                                                 : 0;
 }
 
-// Example -> Features -> map entries of the record [0, L): slot[k] = the last entry of schema key k.  scan: every keyed
-// entry's Feature is parsed (the host parses them all) and slot[k].r holds the counts.  false = malformed.
+// the map entries of the record [0, L) (example_wire.cuh's walk): slot[k] = the last entry of schema key k.  scan:
+// every keyed entry's Feature is parsed (the host parses them all) and slot[k].r holds the counts; emit: only the
+// Feature bytes are recorded.  false = malformed.
 __device__ bool tr_walk(const uint8_t* d, int L, TrSlot* slot, bool want_z, bool scan) {
   const int lane = tr_lane();
   if (lane < TR_KEYS) slot[lane].fs = -1;
-  __syncwarp();
-  bool ok = true;
-  for (int p = 0; p < L && ok;) {
-    TrField f;
-    p = tr_field(d, p, L, f);
-    if (p < 0) { ok = false; break; }
-    if (f.num != 1) continue;
-    if (f.wt != 2) { ok = false; break; }
-    for (int q = f.vs; q < f.ve;) {            // Features: map entries
-      TrField g;
-      q = tr_field(d, q, f.ve, g);
-      if (q < 0 || (g.num == 1 && g.wt != 2)) { ok = false; break; }
-      if (g.num != 1) continue;
-      int ks = -1, ke = 0, fs = 0, fe = 0;     // no value field = an empty Feature
-      for (int r = g.vs; r < g.ve;) {
-        TrField h;
-        r = tr_field(d, r, g.ve, h);
-        if (r < 0 || ((h.num == 1 || h.num == 2) && h.wt != 2)) { ok = false; break; }
-        if (h.num == 1) { ks = h.vs; ke = h.ve; }
-        if (h.num == 2) { fs = h.vs; fe = h.ve; }
-      }
-      if (!ok) break;
-      if (ks < 0) continue;                    // an entry without a key is skipped unparsed
-      const int key = tr_match_key(d, ks, ke, want_z);
-      if (key == -2) { ok = false; break; }
-      TrFeat r{};
-      if (scan && !tr_feature(d, fs, fe, r, nullptr, 0, key >= 0 ? tr_range_n(key) : 0)) { ok = false; break; }
-      if (key >= 0 && lane == 0) { slot[key].fs = fs; slot[key].fe = fe; slot[key].r = r; }
-    }
-  }
-  __syncwarp();
-  return ok;
+  return tr_map_entries(
+      d, L, [&](int ks, int ke) { return tr_match_key(d, ks, ke, want_z); },
+      [&](int key, int fs, int fe) {
+        TrFeat r{};
+        if (scan && !tr_feature(d, fs, fe, r, nullptr, 0, key >= 0 ? tr_range_n(key) : 0)) return false;
+        if (key >= 0 && lane == 0) { slot[key].fs = fs; slot[key].fe = fe; slot[key].r = r; }
+        return true;
+      });
 }
 
 // the checks of decode_tfrecord_files, in its order, then the deviations -> (check << 8) | arg, or -1

@@ -30,13 +30,9 @@ struct WsSlot {
   float val;    // the last float of a FloatList
 };
 
-// map key [s, e) -> 0..38 for I1..I13 / C14..C39 (decoded as 'I' or 'C' and a canonical decimal), -1 for any other key,
-// -2 when it is not UTF-8 (the host parser raises)
+// map key [s, e) -> 0..38 for I1..I13 / C14..C39 (decoded as 'I' or 'C' and a canonical decimal), -1 for any other key
 __device__ int ws_key(const uint8_t* d, int s, int e) {
   const int n = e - s;
-  bool high = false;
-  for (int i = (threadIdx.x & 31); i < n; i += 32) high |= tr_byte(d, s + i) >= 0x80;
-  if (__any_sync(FULL_MASK, high) && !tr_utf8(d, s, e)) return -2;
   if (n < 2 || n > 3) return -1;
   const uint32_t c = tr_byte(d, s), d1 = tr_byte(d, s + 1), d2 = n == 3 ? tr_byte(d, s + 2) : '0';
   if ((c != 'I' && c != 'C') || d1 < '1' || d1 > '9' || d2 < '0' || d2 > '9') return -1;
@@ -45,8 +41,33 @@ __device__ int ws_key(const uint8_t* d, int s, int e) {
   return num > WS_NUM && num <= WS_KEYS ? num - 1 : -1;
 }
 
-// the value count of a BytesList / FloatList / Int64List [s, e) of kind r.kind, appended to r.count; false = malformed
+// the values of an Int64List [s, e), in order, to add(v); false = malformed (a packed varint unterminated, over 10
+// bytes or >= 2^64)
+template <class Add>
+__device__ __forceinline__ bool ws_ints(const uint8_t* d, int s, int e, Add add) {
+  for (int p = s; p < e;) {
+    TrField f;
+    p = tr_field(d, p, e, f);
+    if (p < 0) return false;
+    if (f.num != 1) continue;
+    if (f.wt == 2) {
+      for (int q = f.vs; q < f.ve;) {
+        uint64_t v;
+        q = tr_varint(d, q, f.ve, v);
+        if (q < 0) return false;
+        add(v);
+      }
+    } else if (f.wt == 0) {
+      add(f.v);
+    }
+  }
+  return true;
+}
+
+// the value count of a BytesList / FloatList / Int64List [s, e) of kind r.kind, appended to r.count, and a FloatList's
+// last value; false = malformed
 __device__ bool ws_list(const uint8_t* d, int s, int e, WsSlot& r) {
+  if (r.kind == WK_INT) return ws_ints(d, s, e, [&](uint64_t) { ++r.count; });
   for (int p = s; p < e;) {
     TrField f;
     p = tr_field(d, p, e, f);
@@ -54,82 +75,16 @@ __device__ bool ws_list(const uint8_t* d, int s, int e, WsSlot& r) {
     if (f.num != 1) continue;
     if (r.kind == WK_BYTES) {
       ++r.count;
-    } else if (r.kind == WK_FLOAT) {
-      if (f.wt == 2) {
-        if ((f.ve - f.vs) & 3) return false;
-        if (f.ve > f.vs) r.val = tr_float(tr_u32(d, f.ve - 4));
-        r.count += (f.ve - f.vs) >> 2;
-      } else if (f.wt == 5) {
-        r.val = tr_float(tr_u32(d, f.vs));
-        ++r.count;
-      }
-    } else {
-      if (f.wt == 2) {
-        for (int q = f.vs; q < f.ve; ++r.count) {
-          uint64_t v;
-          q = tr_varint(d, q, f.ve, v);
-          if (q < 0) return false;
-        }
-      } else if (f.wt == 0) {
-        ++r.count;
-      }
+    } else if (f.wt == 2) {
+      if ((f.ve - f.vs) & 3) return false;
+      if (f.ve > f.vs) r.val = tr_float(tr_u32(d, f.ve - 4));
+      r.count += (f.ve - f.vs) >> 2;
+    } else if (f.wt == 5) {
+      r.val = tr_float(tr_u32(d, f.vs));
+      ++r.count;
     }
   }
   return true;
-}
-
-// a Feature [s, e): its first field numbered 1..3 sets the kind and the values, later ones set `multi`
-__device__ bool ws_feature(const uint8_t* d, int s, int e, WsSlot& r) {
-  r.present = 1; r.kind = WK_NONE; r.count = 0; r.multi = 0; r.ls = r.le = 0; r.val = 0.f;
-  for (int p = s; p < e;) {
-    TrField f;
-    p = tr_field(d, p, e, f);
-    if (p < 0) return false;
-    if (f.num < 1 || f.num > 3) continue;
-    if (r.kind != WK_NONE) { r.multi = 1; continue; }
-    if (f.wt != 2) return false;
-    r.kind = f.num; r.ls = f.vs; r.le = f.ve;
-    if (!ws_list(d, f.vs, f.ve, r)) return false;
-  }
-  return true;
-}
-
-// Example -> Features -> map entries of [0, L): slot[k] = the last entry of key k; every keyed entry's Feature is
-// checked for well-formedness, as the host parser parses them all.  false = malformed.
-__device__ bool ws_walk(const uint8_t* d, int L, WsSlot* slot) {
-  const int lane = threadIdx.x & 31;
-  for (int k = lane; k < WS_KEYS; k += 32) slot[k].present = 0;
-  __syncwarp();
-  bool ok = true;
-  for (int p = 0; p < L && ok;) {
-    TrField f;
-    p = tr_field(d, p, L, f);
-    if (p < 0) { ok = false; break; }
-    if (f.num != 1) continue;
-    if (f.wt != 2) { ok = false; break; }
-    for (int q = f.vs; q < f.ve;) {            // Features: map entries
-      TrField g;
-      q = tr_field(d, q, f.ve, g);
-      if (q < 0 || (g.num == 1 && g.wt != 2)) { ok = false; break; }
-      if (g.num != 1) continue;
-      int ks = -1, ke = 0, fs = 0, fe = 0;     // no value field = an empty Feature
-      for (int r = g.vs; r < g.ve;) {
-        TrField h;
-        r = tr_field(d, r, g.ve, h);
-        if (r < 0 || ((h.num == 1 || h.num == 2) && h.wt != 2)) { ok = false; break; }
-        if (h.num == 1) { ks = h.vs; ke = h.ve; }
-        if (h.num == 2) { fs = h.vs; fe = h.ve; }
-      }
-      if (!ok) break;
-      if (ks < 0) continue;                    // an entry without a key is skipped unparsed
-      const int key = ws_key(d, ks, ke);
-      WsSlot r;
-      if (key == -2 || !ws_feature(d, fs, fe, r)) { ok = false; break; }
-      if (key >= 0 && lane == 0) slot[key] = r;
-    }
-  }
-  __syncwarp();
-  return ok;
 }
 
 __device__ __forceinline__ int ws_check(const WsSlot& s, int k) {
@@ -166,8 +121,19 @@ wd_serve_input_kernel(const uint8_t* __restrict__ data, const int64_t* __restric
   for (int64_t b = (int64_t)blockIdx.x * WS_WARPS + wib; b < n; b += (int64_t)gridDim.x * WS_WARPS) {
     const int64_t L = off[b + 1] - off[b];
     const uint8_t* d = data + off[b];
+    for (int k = lane; k < WS_KEYS; k += 32) slot[k].present = 0;
+    // slot[k] = the last entry of key k; every keyed entry's Feature must be well formed
+    auto entry = [&](int key, int fs, int fe) {
+      WsSlot r{1, WK_NONE, 0, 0, 0, 0, 0.f};
+      if (!tr_feature_kind(d, fs, fe, r, [&](int ls, int le) { r.ls = ls; r.le = le; return ws_list(d, ls, le, r); }))
+        return false;
+      if (key >= 0 && lane == 0) slot[key] = r;
+      return true;
+    };
     int word = WE_MALFORMED << 8;
-    if (L >= 0 && L <= 0x7FFFFFFF && ws_walk(d, (int)L, slot)) word = ws_checks(slot);
+    if (L >= 0 && L <= 0x7FFFFFFF &&
+        tr_map_entries(d, (int)L, [&](int ks, int ke) { return ws_key(d, ks, ke); }, entry))
+      word = ws_checks(slot);
     if (word >= 0) {
       if (lane == 0) atomicMin(err, (unsigned long long)(example_base + b) << 16 | (unsigned)word);
       __syncwarp();
@@ -190,22 +156,7 @@ wd_serve_input_kernel(const uint8_t* __restrict__ data, const int64_t* __restric
           first = false;
           if (c == 0 && lane == f && wide_cat) acc += wide_cat[fid];
         };
-        if (bag) {
-          for (int p = s.ls; p < s.le;) {
-            TrField g;
-            p = tr_field(d, p, s.le, g);
-            if (g.num != 1) continue;
-            if (g.wt == 2) {
-              for (int q = g.vs; q < g.ve;) {
-                uint64_t v;
-                q = tr_varint(d, q, g.ve, v);
-                add(v);
-              }
-            } else if (g.wt == 0) {
-              add(g.v);
-            }
-          }
-        }
+        if (bag) ws_ints(d, s.ls, s.le, add);
         if (row) xr[(int64_t)f * K + k] = bag ? sum / (float)s.count : 0.f;
       }
     }

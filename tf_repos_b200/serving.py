@@ -61,6 +61,53 @@ def _build(model_name: str, p: Dict, batch_size: int, device):
     raise ValueError(f"unknown exported model {model_name!r}")
 
 
+class _Requests:
+    """The staging of a request of n serialized tf.Examples for the device parsers, in a pinned host buffer and a device
+    buffer that only grow:  prob f32 [n] (padded to 8 bytes) | error word | `extra` bytes | offsets int64 [n+1] | bytes.
+    `send` writes the error word ~0, zeroes the extra bytes and copies error word..bytes in one transfer; `receive`
+    copies prob..extra back in one transfer and waits for it."""
+
+    def __init__(self, device):
+        self.device = device
+        self._host = self._dev = None
+
+    def send(self, examples, extra: int = 0):
+        """examples: n >= 1 serialized Examples -> their device views (prob f32 [n], err int64 [1], extra uint8,
+        offsets int64 [n+1], data uint8).  Raises ValueError for an Example of 2^31 bytes or more."""
+        n = len(examples)
+        lens = np.fromiter(map(len, examples), dtype=np.int64, count=n)
+        if int(lens.max()) >= 1 << 31:
+            raise ValueError(f"example {int(np.argmax(lens >= 1 << 31))}: an Example of 2^31 bytes or more")
+        self._n, self._e = n, (4 * n + 7) & ~7
+        self._back = self._e + 8 + extra
+        head = self._back + 8 * (n + 1)
+        total = head + int(lens.sum())
+        if self._host is None or self._host.numel() < total:
+            cap = max(total, 1 << 16)
+            self._host = torch.empty(cap, dtype=torch.uint8, pin_memory=True)
+            self._dev = torch.empty(cap, dtype=torch.uint8, device=self.device)
+        e, h, dev = self._e, self._host.numpy(), self._dev
+        h[e:e + 8].view(np.int64)[0] = -1
+        h[e + 8:self._back] = 0
+        off = h[self._back:head].view(np.int64)
+        off[0] = 0
+        np.cumsum(lens, out=off[1:])
+        h[head:total] = np.frombuffer(b"".join(examples), dtype=np.uint8)
+        dev[e:total].copy_(self._host[e:total], non_blocking=True)
+        return (dev[:4 * n].view(torch.float32), dev[e:e + 8].view(torch.int64), dev[e + 8:self._back],
+                dev[self._back:head].view(torch.int64), dev[head:total])
+
+    def receive(self):
+        """-> (prob f32 [n], the error word's (example, check, arg) or None, extra uint8), host views valid until the
+        next send"""
+        self._host[:self._back].copy_(self._dev[:self._back], non_blocking=True)
+        torch.cuda.current_stream(self.device).synchronize()
+        h, e = self._host.numpy(), self._e
+        word = int(h[e:e + 8].view(np.int64)[0])        # (example << 16) | (check << 8) | arg, ~0 = none
+        error = None if word == -1 else (word >> 16, (word >> 8) & 0xFF, word & 0xFF)
+        return h[:4 * self._n].view(np.float32), error, h[e + 8:self._back]
+
+
 _WD_KEYS = ["I%d" % i for i in range(1, 14)] + ["C%d" % i for i in range(14, 40)]
 _WD_CHECKS = {1: "malformed tf.Example protobuf", 2: "required key {key!r} is missing",
               3: "key {key!r} holds several kinds or the wrong kind (I*: FloatList, C*: Int64List)",
@@ -74,7 +121,7 @@ class WideDeepServable:
 
     def __init__(self, model):
         self.model = model
-        self._host = self._dev = None
+        self._requests = _Requests(model.device)
 
     @classmethod
     def load(cls, export_dir: str, max_batch: int = 4096, device="cuda") -> "WideDeepServable":
@@ -90,50 +137,22 @@ class WideDeepServable:
         model.load_variables(v)
         return cls(model)
 
-    def _buffers(self, nbytes: int):
-        if self._host is None or self._host.numel() < nbytes:
-            cap = max(nbytes, 1 << 16)
-            self._host = torch.empty(cap, dtype=torch.uint8, pin_memory=True)
-            self._dev = torch.empty(cap, dtype=torch.uint8, device=self.model.device)
-        return self._host, self._dev
-
     def classify(self, examples) -> Dict[str, np.ndarray]:
         """examples: the string_vals of the request's `inputs` tensor (a sequence of bytes).  Raises ValueError naming
         the first rejected Example (its index in the whole request) and the key."""
         n = len(examples)
         if n == 0:
             return {"scores": np.zeros((0, 2), dtype=np.float32), "classes": np.zeros((0, 2), dtype="S1")}
-        lens = np.fromiter(map(len, examples), dtype=np.int64, count=n)
-        offsets = np.zeros(n + 1, dtype=np.int64)
-        np.cumsum(lens, out=offsets[1:])
-        if int(lens.max()) >= 1 << 31:
-            raise ValueError(f"example {int(np.argmax(lens >= 1 << 31))}: an Example of 2^31 bytes or more")
-        # device layout: prob f32 [n] (padded to 8 bytes) | err | offsets [n+1] | bytes; the first copy fills
-        # err..bytes, the last reads prob..err back
-        p_bytes = (4 * n + 7) & ~7
-        head = 8 + 8 * (n + 1)
-        total = p_bytes + head + int(offsets[-1])
-        host, dev = self._buffers(total)
-        h = host.numpy()
-        h[p_bytes:p_bytes + 8].view(np.int64)[0] = -1
-        h[p_bytes + 8:p_bytes + head].view(np.int64)[:] = offsets
-        h[p_bytes + head:total] = np.frombuffer(b"".join(examples), dtype=np.uint8)
-        dev[p_bytes:total].copy_(host[p_bytes:total], non_blocking=True)
-        pred = dev[:4 * n].view(torch.float32)
-        err = dev[p_bytes:p_bytes + 8].view(torch.int64)
-        off = dev[p_bytes + 8:p_bytes + head].view(torch.int64)
-        data = dev[p_bytes + head:total]
+        pred, err, _, off, data = self._requests.send(examples)
         B = self.model.B
         for lo in range(0, n, B):
             hi = min(lo + B, n)
             self.model.predict_examples(data, off[lo:hi + 1], err, pred[lo:hi], example_base=lo)
-        host[:p_bytes + 8].copy_(dev[:p_bytes + 8], non_blocking=True)
-        torch.cuda.current_stream(self.model.device).synchronize()
-        word = int(h[p_bytes:p_bytes + 8].view(np.int64)[0])
-        if word != -1:
-            ex, check, key = word >> 16, (word >> 8) & 0xFF, word & 0xFF
+        p, error, _ = self._requests.receive()
+        if error is not None:
+            ex, check, key = error
             raise ValueError(f"example {ex}: " + _WD_CHECKS[check].format(key=_WD_KEYS[key]))
-        p = h[:4 * n].view(np.float32).copy()
+        p = p.copy()
         return {"scores": np.stack([np.float32(1) - p, p], axis=1),
                 "classes": np.tile(np.array([b"0", b"1"], dtype="S1"), (n, 1))}
 
@@ -182,7 +201,7 @@ class DINServable:
 
     def __init__(self, model):
         self.model = model
-        self._host = self._dev = None
+        self._requests = _Requests(model.device)
         self._commit_batch(self._alloc_batch(model.P, model.max_a_int))
 
     @classmethod
@@ -223,13 +242,6 @@ class DINServable:
         self.model.grow(P, A)
         self._commit_batch(bufs)
 
-    def _buffers(self, nbytes: int):
-        if self._host is None or self._host.numel() < nbytes:
-            cap = max(nbytes, 1 << 16)
-            self._host = torch.empty(cap, dtype=torch.uint8, pin_memory=True)
-            self._dev = torch.empty(cap, dtype=torch.uint8, device=self.model.device)
-        return self._host, self._dev
-
     def _run(self, data, off, lo: int, hi: int, err, maxima, pred):
         m, bt = self.model, self._batch
         # the emit writes u_ids / u_wgt at stride P and up to B * max_a_int a_int ids: never past these tensors
@@ -249,54 +261,30 @@ class DINServable:
         if n == 0:
             return np.zeros(0, dtype=np.float32)
         m = self.model
-        lens = np.fromiter(map(len, examples), dtype=np.int64, count=n)
-        if int(lens.max()) >= 1 << 31:
-            raise ValueError(f"example {int(np.argmax(lens >= 1 << 31))}: an Example of 2^31 bytes or more")
-        offsets = np.zeros(n + 1, dtype=np.int64)
-        np.cumsum(lens, out=offsets[1:])
         slices = [(lo, min(lo + m.B, n)) for lo in range(0, n, m.B)]
         S = len(slices)
-        # device layout: prob f32 [n] (padded to 8 bytes) | err | oob int32 [2] | maxima int32 [S, 2] (padded to 8) |
-        # offsets [n+1] | bytes; the first copy fills err..bytes, the last reads prob..maxima back
-        p_bytes = (4 * n + 7) & ~7
-        m_bytes = (8 * S + 7) & ~7
-        back = p_bytes + 16 + m_bytes
-        head = back + 8 * (n + 1)
-        total = head + int(offsets[-1])
-        host, dev = self._buffers(total)
-        h = host.numpy()
-        h[p_bytes:p_bytes + 8].view(np.int64)[0] = -1
-        h[p_bytes + 8:back] = 0
-        h[back:head].view(np.int64)[:] = offsets
-        h[head:total] = np.frombuffer(b"".join(examples), dtype=np.uint8)
-        dev[p_bytes:total].copy_(host[p_bytes:total], non_blocking=True)
-        pred = dev[:4 * n].view(torch.float32)
-        err = dev[p_bytes:p_bytes + 8].view(torch.int64)
-        oob = dev[p_bytes + 8:p_bytes + 16].view(torch.int32)
-        maxima = dev[p_bytes + 16:p_bytes + 16 + 8 * S].view(torch.int32).view(S, 2)
-        off = dev[back:head].view(torch.int64)
-        data = dev[head:total]
+        # extra: the model's out-of-range id counter int32 [2], then maxima int32 [S, 2]
+        pred, err, extra, off, data = self._requests.send(examples, 8 + 8 * S)
+        oob, maxima = extra[:8].view(torch.int32), extra[8:].view(torch.int32).view(S, 2)
         todo = list(range(S))
         while True:
             P, A = m.P, m.max_a_int
             for s in todo:
                 self._run(data, off, *slices[s], err, maxima[s], pred)
             oob.copy_(m.oob)
-            host[:back].copy_(dev[:back], non_blocking=True)
-            torch.cuda.current_stream(m.device).synchronize()
-            word = int(h[p_bytes:p_bytes + 8].view(np.int64)[0])
-            n_oob = int(h[p_bytes + 8:p_bytes + 12].view(np.int32)[0])
-            if word != -1 or n_oob:
+            p, error, h_extra = self._requests.receive()
+            n_oob = int(h_extra[:4].view(np.int32)[0])
+            if error is not None or n_oob:
                 m.oob.zero_()
-                ex = word >> 16 if word != -1 else n
+                ex = error[0] if error is not None else n
                 msg = din_id_range_error(examples, ex, m.N)
-                if msg is None and word != -1:
-                    msg = din_error_message(ex, (word >> 8) & 0xFF, word & 0xFF, m.Fp)
+                if msg is None and error is not None:
+                    msg = din_error_message(*error, m.Fp)
                 raise ValueError(msg or f"an id outside [0, feature_size={m.N})")
-            mx = h[p_bytes + 16:p_bytes + 16 + 8 * S].view(np.int32).reshape(S, 2)
+            mx = h_extra[8:].view(np.int32).reshape(S, 2)
             todo = [s for s in todo if mx[s, 0] > P or mx[s, 1] > A]
             if not todo:
-                return h[:4 * n].view(np.float32).copy()
+                return p.copy()
             self._grow(int(mx[todo, 0].max()), int(mx[todo, 1].max()))
 
 
