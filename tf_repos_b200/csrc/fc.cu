@@ -201,6 +201,7 @@ int ctr_fc_bwd(const float* in, const float* Wt, const float* out, const float* 
   CTR_REQUIRE(M >= 0 && Kd > 0 && Nd > 0 && (act == 0 || act == 1 || act == 2), CTR_ERR_INVALID_ARG, "ctr_fc_bwd: bad shape/act");
   if (M == 0) return CTR_OK;
   CTR_REQUIRE(in && Wt && dOut && dW && (act == 2 || (out && db)), CTR_ERR_INVALID_ARG, "ctr_fc_bwd: null buffer");
+  CTR_REQUIRE(act == 2 || !drop_mask || keep_prob > 0.f, CTR_ERR_INVALID_ARG, "ctr_fc_bwd: keep_prob must be > 0");
   CTR_REQUIRE(ws && ws_bytes >= ctr_fc_bwd_workspace_bytes(M, Kd, Nd), CTR_ERR_WORKSPACE,
               "ctr_fc_bwd: workspace too small");
   cudaStream_t st = as_stream(stream);
