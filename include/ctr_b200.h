@@ -681,6 +681,52 @@ size_t ctr_aliccp_sample_order_workspace_bytes(int64_t n_samples);
 int ctr_aliccp_sample_order(uint64_t* s_key, int64_t* s_val, int64_t n_samples, int64_t parts, int64_t* part_bytes,
                             void* ws, size_t ws_bytes, ctr_stream_t stream);
 
+/* ---- smart and Frappe feature stages (deep_ctr/Feature_pipeline/get_smart_feature.py, get_frape_feature.py; DESIGN.md
+ * §2.12) --------------------------------------------------------------------------------------------------------------
+ * `text` is a chunk of whole lines (a last line without '\n' counts), len < 2^30.  Lines end at '\n' only and are
+ * strip()ped with Python 2's whitespace (' ', \t, \n, \r, \x0b, \x0c).
+ * map (replaces :56-63, the feature_map load): map_text[0, map_len) = the whole feature_map file, resident while the
+ *   table is used; table = ctr_smart_map_table_bytes(capacity) bytes, zeroed by the caller, capacity slots (<= 2^31).
+ *   Each line with two or more ' ' tokens maps s[0] -> s[1]; a key some lookup can reach (categorical `name|value` or a
+ *   continuous `name`) is inserted, the later line of a repeated key wins.  col_fid int64[2 * 128] = per column the
+ *   (offset, length) in map_text of the fid of its bare name (continuous columns) or of name|UNK (categorical), length
+ *   -1 = absent.  info int64[3] = {map lines, keys inserted, keys that found no slot within min(capacity, 32768) probes
+ *   -- non-zero means capacity is too small}.
+ * emit (:68-89): plan then write, over the same text and ws.  plan: info int64[3] = {lines, emitted lines, output
+ *   bytes}; a line of 130 or more fields is dropped.  write: the emitted lines to out[0, info[2]), in input order; a
+ *   fid absent from the map prints as None.
+ * build (get_feature_map, :27-53, with CSV_COLUMNS[i] at :32 read as fname): table = ctr_smart_build_table_bytes(
+ *   capacity) bytes and state int64[19], both zeroed by the caller; arena = arena_bytes bytes that hold each distinct
+ *   categorical value once, plus one byte.  insert, once per chunk of the `tr` files in order (line_base = lines before
+ *   the chunk over all of them): info int64[2] = {lines, keys that found no slot}; state[1] = keys the arena could not
+ *   hold.  Either non-zero leaves the table unusable.  finish: the keys in order of their first (line, column), info
+ *   int64[2] = {keys, map bytes}; render (after finish, same ws): out[0, info[1]) = `key fid\n` for fids 129, 130, ...
+ * frappe (get_frape_feature.py:16-29): plan: info int64[3] = {lines, kept lines, output bytes}; write: the kept lines,
+ *   label -1 rewritten to 0, to out[0, info[2]).
+ * No allocation and no synchronisation inside. */
+size_t ctr_smart_map_table_bytes(int64_t capacity);
+size_t ctr_smart_map_workspace_bytes(size_t map_len);
+int ctr_smart_map_build(const char* map_text, size_t map_len, void* table, int64_t capacity, int64_t* col_fid,
+                        int64_t* info, void* ws, size_t ws_bytes, ctr_stream_t stream);
+size_t ctr_smart_emit_workspace_bytes(size_t len);
+int ctr_smart_emit_plan(const char* text, size_t len, const char* map_text, const void* table, int64_t capacity,
+                        const int64_t* col_fid, int64_t* info, void* ws, size_t ws_bytes, ctr_stream_t stream);
+int ctr_smart_emit_write(const char* text, size_t len, const char* map_text, const void* table, int64_t capacity,
+                         const int64_t* col_fid, char* out, const void* ws, size_t ws_bytes, ctr_stream_t stream);
+size_t ctr_smart_build_table_bytes(int64_t capacity);
+size_t ctr_smart_build_insert_workspace_bytes(size_t len);
+int ctr_smart_build_insert(const char* text, size_t len, int64_t line_base, void* table, int64_t capacity,
+                           uint8_t* arena, int64_t arena_bytes, int64_t* state, int64_t* info, void* ws,
+                           size_t ws_bytes, ctr_stream_t stream);
+size_t ctr_smart_build_workspace_bytes(int64_t capacity);
+int ctr_smart_build_finish(const void* table, int64_t capacity, const uint8_t* arena, const int64_t* state,
+                           int64_t* info, void* ws, size_t ws_bytes, ctr_stream_t stream);
+int ctr_smart_build_render(const void* table, int64_t capacity, const uint8_t* arena, char* out, const void* ws,
+                           size_t ws_bytes, ctr_stream_t stream);
+size_t ctr_frappe_workspace_bytes(size_t len);
+int ctr_frappe_plan(const char* text, size_t len, int64_t* info, void* ws, size_t ws_bytes, ctr_stream_t stream);
+int ctr_frappe_write(const char* text, size_t len, char* out, const void* ws, size_t ws_bytes, ctr_stream_t stream);
+
 /* ---- CRC-32C of whole tensors (TensorFlow checkpoint bundles; DESIGN.md §2.11) ---------------------------------------
  * ranges: device int64 [n][2] = {address, length in bytes}.  An address needs only 4-byte alignment; a length may be 0
  * or exceed 2^32.  total_bytes >= the sum of the lengths (it sizes the grid and the workspace of

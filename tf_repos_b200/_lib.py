@@ -151,6 +151,21 @@ SIGNATURES = {
                                        c_int64, P, P, P, c_size_t, P]),
     "ctr_aliccp_sample_order_workspace_bytes": (c_size_t, [c_int64]),
     "ctr_aliccp_sample_order": (c_int, [P, P, c_int64, c_int64, P, P, c_size_t, P]),
+    "ctr_smart_map_table_bytes": (c_size_t, [c_int64]),
+    "ctr_smart_map_workspace_bytes": (c_size_t, [c_size_t]),
+    "ctr_smart_map_build": (c_int, [P, c_size_t, P, c_int64, P, P, P, c_size_t, P]),
+    "ctr_smart_emit_workspace_bytes": (c_size_t, [c_size_t]),
+    "ctr_smart_emit_plan": (c_int, [P, c_size_t, P, P, c_int64, P, P, P, c_size_t, P]),
+    "ctr_smart_emit_write": (c_int, [P, c_size_t, P, P, c_int64, P, P, P, c_size_t, P]),
+    "ctr_smart_build_table_bytes": (c_size_t, [c_int64]),
+    "ctr_smart_build_insert_workspace_bytes": (c_size_t, [c_size_t]),
+    "ctr_smart_build_insert": (c_int, [P, c_size_t, c_int64, P, c_int64, P, c_int64, P, P, P, c_size_t, P]),
+    "ctr_smart_build_workspace_bytes": (c_size_t, [c_int64]),
+    "ctr_smart_build_finish": (c_int, [P, c_int64, P, P, P, P, c_size_t, P]),
+    "ctr_smart_build_render": (c_int, [P, c_int64, P, P, P, c_size_t, P]),
+    "ctr_frappe_workspace_bytes": (c_size_t, [c_size_t]),
+    "ctr_frappe_plan": (c_int, [P, c_size_t, P, P, c_size_t, P]),
+    "ctr_frappe_write": (c_int, [P, c_size_t, P, P, c_size_t, P]),
     "ctr_crc32c_workspace_bytes": (c_size_t, [c_int, c_int64]),
     "ctr_crc32c_ranges": (c_int, [P, c_int, c_int64, P, P, P, c_size_t, P]),
     "ctr_init_trunc_normal": (c_int, [P, c_int64, c_float, c_uint64, P]),

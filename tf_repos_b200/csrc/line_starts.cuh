@@ -1,5 +1,5 @@
 // line_starts.cuh -- line starts of a text buffer in device memory, shared by the tokenizers
-// (libsvm_device.cu, csv_device.cu, criteo_feature.cu, aliccp_tfrecord.cu, aliccp_sample.cu).
+// (libsvm_device.cu, csv_device.cu, criteo_feature.cu, aliccp_tfrecord.cu, aliccp_sample.cu, smart_feature.cu).
 //
 // Kernels: (1) count '\n' per 4 KB block; (2) scan the block counts (cta_scan_kernel); (3) emit line starts.
 // LineStarts is their workspace and launches them; line_bounds / chunk_lines read the result in the per-line kernels.

@@ -1,5 +1,5 @@
 // scan_sort.cuh -- the one-CTA exclusive scan and the stable LSD radix sort over device-resident counts, shared by the
-// text pipelines (line_starts.cuh, criteo_feature.cu, aliccp_sample.cu).
+// text pipelines (line_starts.cuh, criteo_feature.cu, aliccp_sample.cu, smart_feature.cu).
 //
 // The sort takes uint64 keys with an optional uint32 value, 8-bit digits: per-CTA digit histograms, a one-CTA scan of
 // the digit-major histogram, then a scatter that keeps index order within a CTA (warp match + per-warp digit counts).
