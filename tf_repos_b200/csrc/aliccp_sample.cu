@@ -470,7 +470,6 @@ __device__ __forceinline__ int64_t as_lookup(const uint64_t* __restrict__ vocab,
 template <bool W>
 __device__ void as_remap(const uint8_t* t, int64_t s, int64_t e, const uint64_t* vocab, int64_t n_vocab, char* o,
                          int64_t& pos, int64_t& kept) {
-  const int lane = lane_id();
   as_tokens(t, s, e, [&](bool end, int64_t ts, int64_t q) {
     AsTok k;
     int64_t id = -1;
@@ -482,13 +481,10 @@ __device__ void as_remap(const uint8_t* t, int64_t s, int64_t e, const uint64_t*
     const bool sep = kept + __popc(km & lanemask_lt()) > 0;
     const int nd = id >= 0 ? dec_digits((uint64_t)id) : 0;
     const int64_t L = id >= 0 ? (sep ? 1 : 0) + (k.p2 - ts) + 1 + nd + 1 + (q - k.p3 - 1) : 0;
-    int64_t x = L;
-    for (int d = 1; d < 32; d <<= 1) {
-      const int64_t y = __shfl_up_sync(FULL_MASK, x, d);
-      if (lane >= d) x += y;
-    }
+    int64_t tot;
+    const int64_t before = warp_scan_excl(L, tot);
     if (W && id >= 0) {
-      char* d = o + pos + x - L;
+      char* d = o + pos + before;
       if (sep) *d++ = ' ';
       for (int64_t p = ts; p < k.p2; ++p) *d++ = (char)byte_at(t, p);
       *d++ = ':';
@@ -497,7 +493,7 @@ __device__ void as_remap(const uint8_t* t, int64_t s, int64_t e, const uint64_t*
       *d++ = ':';
       for (int64_t p = k.p3 + 1; p < q; ++p) *d++ = (char)byte_at(t, p);
     }
-    pos += __shfl_sync(FULL_MASK, x, 31);
+    pos += tot;
     kept += __popc(km);
   });
 }
@@ -720,13 +716,9 @@ int ctr_aliccp_sample_classify(const char* text, size_t len, int64_t n_lines, in
         t, (int64_t)len, W.line_start, W.n_newlines, n_lines, mode, AsCnt(count_table, count_capacity),
         AsMd5(md5_table, md5_capacity), W.P, W.info);
     CTR_LAUNCHED("ctr_aliccp_sample_classify");
-    const int64_t* cnt = W.info + AI_LINES;
-    cta_scan_kernel<int32_t><<<1, 1024, 0, st>>>(W.P.coff, cnt, 0, W.info + AI_CBYTES);
-    CTR_LAUNCHED("ctr_aliccp_sample_classify(scan)");
-    cta_scan_kernel<int32_t><<<1, 1024, 0, st>>>(W.P.cord, cnt, 0, W.info + AI_COMMONS);
-    CTR_LAUNCHED("ctr_aliccp_sample_classify(scan)");
-    cta_scan_kernel<int32_t><<<1, 1024, 0, st>>>(W.P.sord, cnt, 0, W.info + AI_SAMPLES);
-    CTR_LAUNCHED("ctr_aliccp_sample_classify(scan)");
+    if (int rc = cta_scan({W.P.coff, W.P.cord, W.P.sord}, {W.info + AI_CBYTES, W.info + AI_COMMONS, W.info + AI_SAMPLES},
+                          W.info + AI_LINES, 0, st, "ctr_aliccp_sample_classify(scan)"))
+      return rc;
   }
   CTR_REQUIRE(cudaMemcpyAsync(info, W.info, AI_N * 8, cudaMemcpyDeviceToDevice, st) == cudaSuccess, CTR_ERR_CUDA,
               "ctr_aliccp_sample_classify: copy of info failed");
@@ -809,8 +801,7 @@ int ctr_aliccp_sample_vocab(const void* count_table, int64_t count_capacity, int
     return rc;
   as_heads_kernel<<<g, AS_THREADS, 0, st>>>(sk, V.counts + 1, V.head);
   CTR_LAUNCHED("ctr_aliccp_sample_vocab(heads)");
-  cta_scan_kernel<int32_t><<<1, 1024, 0, st>>>(V.head, V.counts + 1, 0, V.n_vocab);
-  CTR_LAUNCHED("ctr_aliccp_sample_vocab(scan)");
+  if (int rc = cta_scan({V.head}, {V.n_vocab}, V.counts + 1, 0, st, "ctr_aliccp_sample_vocab(scan)")) return rc;
   as_unique_kernel<<<g, AS_THREADS, 0, st>>>(sk, V.counts + 1, V.head, vocab);
   CTR_LAUNCHED("ctr_aliccp_sample_vocab(unique)");
   // entries: LSD by fid, then field bytes 8..15, then field bytes 0..7
@@ -831,8 +822,7 @@ int ctr_aliccp_sample_vocab(const void* count_table, int64_t count_capacity, int
   }
   as_feat_cnts_kernel<false><<<g, AS_THREADS, 0, st>>>(V.E, V.perm, V.counts, V.lens, nullptr);
   CTR_LAUNCHED("ctr_aliccp_sample_vocab(feat_cnts)");
-  cta_scan_kernel<int64_t><<<1, 1024, 0, st>>>(V.lens, V.counts, 0, V.fc_bytes);
-  CTR_LAUNCHED("ctr_aliccp_sample_vocab(scan)");
+  if (int rc = cta_scan({V.lens}, {V.fc_bytes}, V.counts, 0, st, "ctr_aliccp_sample_vocab(scan)")) return rc;
   CTR_REQUIRE(cudaMemcpyAsync(info, V.counts, 5 * 8, cudaMemcpyDeviceToDevice, st) == cudaSuccess, CTR_ERR_CUDA,
               "ctr_aliccp_sample_vocab: copy of info failed");
   return CTR_OK;
@@ -866,9 +856,7 @@ int ctr_aliccp_sample_render(const uint8_t* arena, const int64_t* rec_off, const
                                                         nullptr);
       CTR_LAUNCHED("ctr_aliccp_sample_render(plan)");
     }
-    cta_scan_kernel<int64_t><<<1, 1024, 0, st>>>(r_off, nullptr, n_records + 1, nullptr);
-    CTR_LAUNCHED("ctr_aliccp_sample_render(scan)");
-    return CTR_OK;
+    return cta_scan({r_off}, {nullptr}, nullptr, n_records + 1, st, "ctr_aliccp_sample_render(scan)");
   }
   if (n_records == 0) return CTR_OK;
   as_render_kernel<true><<<g, AS_THREADS, 0, st>>>(arena, rec_off, rec_len, mult, n_records, vocab, n_vocab, r_off, out);
@@ -901,8 +889,7 @@ int ctr_aliccp_sample_emit(const char* text, size_t len, int64_t n_lines, int64_
   as_classify_kernel<<<g, AS_THREADS, 0, st>>>(t, (int64_t)len, W.line_start, W.n_newlines, n_lines, 0, AsCnt(),
                                                AsMd5(), W.P, W.info);
   CTR_LAUNCHED("ctr_aliccp_sample_emit(classify)");
-  cta_scan_kernel<int32_t><<<1, 1024, 0, st>>>(W.P.sord, W.info + AI_LINES, 0, nullptr);
-  CTR_LAUNCHED("ctr_aliccp_sample_emit(scan)");
+  if (int rc = cta_scan({W.P.sord}, {nullptr}, W.info + AI_LINES, 0, st, "ctr_aliccp_sample_emit(scan)")) return rc;
   AsEmitArgs a{seed, line_base, sample_base, s_rec, r_off, rendered, vocab, n_vocab, s_val, lo, hi, out, info};
   if (out)
     as_emit_kernel<true><<<g, AS_THREADS, 0, st>>>(t, (int64_t)len, W.line_start, W.n_newlines, W.info, W.P, a);
@@ -942,8 +929,7 @@ int ctr_aliccp_sample_order(uint64_t* s_key, int64_t* s_val, int64_t n_samples, 
     return rc;
   as_sizes_sorted_kernel<<<g, AS_THREADS, 0, st>>>(sk, sp, s_val, n_samples, O.sz, part_bytes);
   CTR_LAUNCHED("ctr_aliccp_sample_order(sizes)");
-  cta_scan_kernel<int64_t><<<1, 1024, 0, st>>>(O.sz, O.n_dev, 0, nullptr);
-  CTR_LAUNCHED("ctr_aliccp_sample_order(scan)");
+  if (int rc = cta_scan({O.sz}, {nullptr}, O.n_dev, 0, st, "ctr_aliccp_sample_order(scan)")) return rc;
   as_offsets_kernel<<<g, AS_THREADS, 0, st>>>(sp, O.sz, n_samples, s_val);
   CTR_LAUNCHED("ctr_aliccp_sample_order(offsets)");
   return CTR_OK;

@@ -372,44 +372,6 @@ __global__ void __launch_bounds__(AL_THREADS) al_plan_kernel(const uint8_t* __re
   }
 }
 
-// exclusive scans of rec[0, n] and decl[0, n] in place (one CTA, tiles of 1024): rec[n] / decl[n] become the totals
-__global__ void __launch_bounds__(1024) al_scan_kernel(int64_t* __restrict__ rec, int64_t* __restrict__ decl,
-                                                       int64_t* __restrict__ info) {
-  __shared__ int64_t ws_a[32], ws_b[32];
-  __shared__ int64_t carry_a, carry_b;
-  const int64_t n = info[0] + 1;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (threadIdx.x == 0) { carry_a = 0; carry_b = 0; }
-  __syncthreads();
-  for (int64_t base = 0; base < n; base += 1024) {
-    const int64_t i = base + threadIdx.x;
-    const int64_t va = i < n ? rec[i] : 0, vb = i < n ? decl[i] : 0;
-    int64_t xa = va, xb = vb;
-    for (int o = 1; o < 32; o <<= 1) {
-      const int64_t ya = __shfl_up_sync(FULL_MASK, xa, o), yb = __shfl_up_sync(FULL_MASK, xb, o);
-      if (lane >= o) { xa += ya; xb += yb; }
-    }
-    if (lane == 31) { ws_a[warp] = xa; ws_b[warp] = xb; }
-    __syncthreads();
-    if (threadIdx.x < 32) {
-      int64_t wa = ws_a[lane], wb = ws_b[lane];
-      for (int o = 1; o < 32; o <<= 1) {
-        const int64_t ya = __shfl_up_sync(FULL_MASK, wa, o), yb = __shfl_up_sync(FULL_MASK, wb, o);
-        if (lane >= o) { wa += ya; wb += yb; }
-      }
-      ws_a[lane] = wa; ws_b[lane] = wb;
-    }
-    __syncthreads();
-    const int64_t ba = carry_a + (warp ? ws_a[warp - 1] : 0) + xa - va;
-    const int64_t bb = carry_b + (warp ? ws_b[warp - 1] : 0) + xb - vb;
-    if (i < n) { rec[i] = ba; decl[i] = bb; }
-    __syncthreads();
-    if (threadIdx.x == 1023) { carry_a = ba + va; carry_b = bb + vb; }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) { info[2] = carry_a; info[3] = carry_b; }
-}
-
 // (row, start, end) of every declined number, at its line's decline offset
 __global__ void __launch_bounds__(AL_THREADS) al_declines_kernel(const uint8_t* __restrict__ t, int64_t len,
                                                                 const int64_t* __restrict__ line_start,
@@ -463,13 +425,9 @@ __global__ void __launch_bounds__(AL_THREADS, 2) al_write_kernel(const uint8_t* 
     // ---- layout: Example tag + length, then one map entry per key ----
     int64_t x = 0, head = 0, P = 0;
     if (lane < AL_KEYS) { P = al_payload(W, lane); x = al_entry(lane, P, head); }
-    int64_t incl = x;
-    for (int o = 1; o < 32; o <<= 1) {
-      const int64_t y = __shfl_up_sync(FULL_MASK, incl, o);
-      if (lane >= o) incl += y;
-    }
-    const int64_t entries = __shfl_sync(FULL_MASK, incl, 31);
-    const int64_t eb = 1 + al_vl(entries), at = eb + incl - x;   // this lane's entry
+    int64_t entries;
+    const int64_t before = warp_scan_excl(x, entries);
+    const int64_t eb = 1 + al_vl(entries), at = eb + before;     // this lane's entry
     const int64_t pay = at + head;                               // its payload
     if (lane == 0) { d[0] = 0x0A; al_put_varint(d + 1, entries); }
     if (lane < AL_KEYS) {
@@ -487,16 +445,13 @@ __global__ void __launch_bounds__(AL_THREADS, 2) al_write_kernel(const uint8_t* 
       if (lane == 14) al_put_f32(o, R.zs ? R.z : decl_vals[dbase + !R.ys]);
     }
     // class c's first id goes to its key's payload; feat_ids' groups follow each other in class order
-    int g = lane < AL_COMMON ? al_group(W, lane) : 0, gi = g;
-    for (int o = 1; o < 32; o <<= 1) {
-      const int y = __shfl_up_sync(FULL_MASK, gi, o);
-      if (lane >= o) gi += y;
-    }
+    int g_tot;
+    const int g_before = warp_scan_excl(lane < AL_COMMON ? al_group(W, lane) : 0, g_tot);
     const bool umh = lane >= AL_UMH && lane < AL_AD;
     const int64_t id_pay = __shfl_sync(FULL_MASK, pay, lane < AL_COMMON ? 4 : lane < AL_CLASSES ? kAlIdKey[lane - AL_UMH] : 0);
     const int64_t val_pay = __shfl_sync(FULL_MASK, pay, umh ? kAlValKey[lane - AL_UMH] : 0);
     if (lane < AL_CLASSES) {
-      const int64_t off = lane < AL_COMMON ? id_pay + gi - g : id_pay;
+      const int64_t off = lane < AL_COMMON ? id_pay + g_before : id_pay;
       W.off[lane] = off;
       W.run[lane] = 0;
       if (umh) {
@@ -597,9 +552,8 @@ int ctr_aliccp_plan(const char* text, size_t len, int64_t line_base, int64_t* in
   al_plan_kernel<<<grid_for((int64_t)len + 1, AL_WARPS, 8), AL_THREADS, 0, st>>>(
       t, (int64_t)len, A.line_start, A.n_newlines, line_base, A.rec, A.decl, info);
   CTR_LAUNCHED("ctr_aliccp_plan");
-  al_scan_kernel<<<1, 1024, 0, st>>>(A.rec, A.decl, info);
-  CTR_LAUNCHED("ctr_aliccp_plan(scan)");
-  return CTR_OK;
+  // rec[0, n] and decl[0, n] become offsets, rec[n] / decl[n] the totals
+  return cta_scan({A.rec, A.decl}, {info + 2, info + 3}, info, 1, st, "ctr_aliccp_plan(scan)");
 }
 
 int ctr_aliccp_declines(const char* text, size_t len, const void* ws, size_t ws_bytes, int64_t* spans,

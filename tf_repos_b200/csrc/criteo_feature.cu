@@ -288,28 +288,6 @@ __global__ void __launch_bounds__(CF_THREADS) cf_stats_kernel(const unsigned cha
   }
 }
 
-// CTA-wide exclusive scan of two int64 values (CF_THREADS threads); returns the CTA totals through s_a / s_b
-__device__ __forceinline__ void cf_block_scan2(int64_t& a, int64_t& b, int64_t& s_a, int64_t& s_b) {
-  __shared__ int64_t wa[CF_THREADS / 32], wb[CF_THREADS / 32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int64_t xa = a, xb = b;
-  for (int o = 1; o < 32; o <<= 1) {
-    const int64_t ya = __shfl_up_sync(FULL_MASK, xa, o), yb = __shfl_up_sync(FULL_MASK, xb, o);
-    if (lane >= o) { xa += ya; xb += yb; }
-  }
-  if (lane == 31) { wa[warp] = xa; wb[warp] = xb; }
-  __syncthreads();
-  int64_t ba = 0, bb = 0;
-  s_a = 0; s_b = 0;
-  for (int w = 0; w < CF_THREADS / 32; ++w) {
-    if (w < warp) { ba += wa[w]; bb += wb[w]; }
-    s_a += wa[w]; s_b += wb[w];
-  }
-  a = ba + xa - a;
-  b = bb + xb - b;
-  __syncthreads();
-}
-
 // per line: output length; per tile of CF_THREADS lines: tr bytes, va bytes, tr lines
 __global__ void __launch_bounds__(CF_THREADS) cf_plan_kernel(const unsigned char* __restrict__ t, int64_t len,
                                                             const int64_t* __restrict__ line_start,
@@ -333,10 +311,10 @@ __global__ void __launch_bounds__(CF_THREADS) cf_plan_kernel(const unsigned char
       line_len[row] = (int32_t)L;
       tr = a.test || to_train[row];
     }
-    int64_t x_tr = tr ? L : 0, x_va = tr ? 0 : L, s_tr, s_va;
-    cf_block_scan2(x_tr, x_va, s_tr, s_va);
+    int64_t x[2] = {tr ? L : 0, tr ? 0 : L}, s[2];   // tr bytes, va bytes
+    block_scan_excl<CF_THREADS>(x, s);
     const int n_tr = __syncthreads_count(row < n_lines && tr);
-    if (threadIdx.x == 0) { tile_tr[tile] = s_tr; tile_va[tile] = s_va; tile_trn[tile] = n_tr; }
+    if (threadIdx.x == 0) { tile_tr[tile] = s[0]; tile_va[tile] = s[1]; tile_trn[tile] = n_tr; }
   }
 }
 
@@ -353,13 +331,13 @@ __global__ void __launch_bounds__(CF_THREADS) cf_write_kernel(const unsigned cha
     const int64_t row = tile * CF_THREADS + threadIdx.x;
     const bool live = row < n_lines, tr = !live || a.test || to_train[row];
     const int64_t L = live ? line_len[row] : 0;
-    int64_t x_tr = tr ? L : 0, x_va = tr ? 0 : L, s_tr, s_va;
-    cf_block_scan2(x_tr, x_va, s_tr, s_va);
+    int64_t x[2] = {tr ? L : 0, tr ? 0 : L}, s[2];   // tr bytes, va bytes
+    block_scan_excl<CF_THREADS>(x, s);
     if (live) {
       int64_t p, e;
       line_bounds(line_start, nn, len, row, p, e);
       uint64_t err = ~0ull;
-      char* o = tr ? out_tr + tile_tr[tile] + x_tr : out_va + tile_va[tile] + x_va;
+      char* o = tr ? out_tr + tile_tr[tile] + x[0] : out_va + tile_va[tile] + x[1];
       cf_emit_line<true>(t, p, e, a, row, err, o);
     }
   }
@@ -584,13 +562,8 @@ int ctr_criteo_emit_plan(const char* text, size_t len, int test, int64_t line_ba
       t, (int64_t)len, E.line_start, E.n_newlines, line_base, to_train, a, E.line_len, E.tile_tr, E.tile_va, E.tile_trn,
       E.n_tiles, info);
   CTR_LAUNCHED("ctr_criteo_emit_plan");
-  cta_scan_kernel<int64_t><<<1, 1024, 0, st>>>(E.tile_tr, E.n_tiles, 0, info + 3);
-  CTR_LAUNCHED("ctr_criteo_emit_plan(scan)");
-  cta_scan_kernel<int64_t><<<1, 1024, 0, st>>>(E.tile_va, E.n_tiles, 0, info + 4);
-  CTR_LAUNCHED("ctr_criteo_emit_plan(scan)");
-  cta_scan_kernel<int64_t><<<1, 1024, 0, st>>>(E.tile_trn, E.n_tiles, 0, info + 2);
-  CTR_LAUNCHED("ctr_criteo_emit_plan(scan)");
-  return CTR_OK;
+  return cta_scan({E.tile_tr, E.tile_va, E.tile_trn}, {info + 3, info + 4, info + 2}, E.n_tiles, 0, st,
+                  "ctr_criteo_emit_plan(scan)");
 }
 
 int ctr_criteo_emit_write(const char* text, size_t len, int test, const uint8_t* to_train, const void* table,

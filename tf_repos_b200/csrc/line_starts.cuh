@@ -51,20 +51,11 @@ __global__ void __launch_bounds__(LS_THREADS) ls_count_kernel(const unsigned cha
 __global__ void __launch_bounds__(LS_THREADS) ls_emit_kernel(const unsigned char* __restrict__ text, int64_t len,
                                                             const int32_t* __restrict__ block_offsets, int64_t max_rows,
                                                             int64_t* __restrict__ line_start) {
-  __shared__ int warp_tot[LS_THREADS / 32];
   const int64_t pos = ((int64_t)blockIdx.x * LS_THREADS + threadIdx.x) * LS_BYTES_PER_THREAD;
   uint32_t mask = 0;
-  const int c = pos < len ? count_nl16(text, pos, len, mask) : 0;
-  int x = c;
-  for (int o = 1; o < 32; o <<= 1) {
-    const int y = __shfl_up_sync(FULL_MASK, x, o);
-    if ((threadIdx.x & 31) >= o) x += y;
-  }
-  if ((threadIdx.x & 31) == 31) warp_tot[threadIdx.x >> 5] = x;
-  __syncthreads();
-  int before = x - c;
-  for (int w = 0; w < (int)(threadIdx.x >> 5); ++w) before += warp_tot[w];
-  int64_t k = (int64_t)block_offsets[blockIdx.x] + before;
+  int before[1] = {pos < len ? count_nl16(text, pos, len, mask) : 0}, tot[1];
+  block_scan_excl<LS_THREADS>(before, tot);
+  int64_t k = (int64_t)block_offsets[blockIdx.x] + before[0];
   if (blockIdx.x == 0 && threadIdx.x == 0) line_start[0] = 0;
   while (mask) {
     const int b = __ffs(mask) - 1;
@@ -111,8 +102,7 @@ struct LineStarts {
   int launch(const uint8_t* t, size_t len, cudaStream_t st, const char* what) const {
     ls_count_kernel<<<n_blocks, LS_THREADS, 0, st>>>(t, (int64_t)len, block_counts);
     CTR_LAUNCHED(what);
-    cta_scan_kernel<int32_t><<<1, 1024, 0, st>>>(block_counts, nullptr, n_blocks, n_newlines);
-    CTR_LAUNCHED(what);
+    if (int rc = cta_scan({block_counts}, {n_newlines}, nullptr, n_blocks, st, what)) return rc;
     ls_emit_kernel<<<n_blocks, LS_THREADS, 0, st>>>(t, (int64_t)len, block_counts, max_rows, line_start);
     CTR_LAUNCHED(what);
     return CTR_OK;

@@ -1,6 +1,9 @@
-// scan_sort.cuh -- the one-CTA exclusive scan and the stable LSD radix sort over device-resident counts, shared by the
-// text pipelines (line_starts.cuh, criteo_feature.cu, aliccp_sample.cu, smart_feature.cu).
+// scan_sort.cuh -- the integer prefix scans and the stable LSD radix sort over device-resident counts, shared by the
+// text pipelines (line_starts.cuh, criteo_feature.cu, smart_feature.cu, aliccp_tfrecord.cu, aliccp_sample.cu,
+// tfrecord_device.cu).
 //
+// Scans, each level built on the one below: warp_scan_excl (N values per lane), block_scan_excl (N values per thread
+// of a CTA), and cta_scan_kernel (N arrays of one device-resident length scanned by one CTA), launched by cta_scan.
 // The sort takes uint64 keys with an optional uint32 value, 8-bit digits: per-CTA digit histograms, a one-CTA scan of
 // the digit-major histogram, then a scatter that keeps index order within a CTA (warp match + per-warp digit counts).
 // Multi-word keys are sorted word by word from the least significant one, carrying a permutation (iota / gather).
@@ -14,41 +17,101 @@ namespace {
 constexpr int LSD_THREADS = 256, LSD_WARPS = LSD_THREADS / 32;
 constexpr int LSD_TILE = 16 * LSD_THREADS;   // items per CTA in the radix passes
 
-// exclusive scan of a[0, n) in place (one CTA, tiles of 1024); n = *count when count is given; total -> *total
+// exclusive scan of each v[k] across the warp, in place; total[k] = the warp's sum of v[k], on every lane.
+// Every lane of the warp calls it.
+template <int N, typename T>
+__device__ __forceinline__ void warp_scan_excl(T (&v)[N], T (&total)[N]) {
+  const int lane = lane_id();
+  T x[N];
+#pragma unroll
+  for (int k = 0; k < N; ++k) x[k] = v[k];
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+      const T y = __shfl_up_sync(FULL_MASK, x[k], o);
+      if (lane >= o) x[k] += y;
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < N; ++k) {
+    total[k] = __shfl_sync(FULL_MASK, x[k], 31);
+    v[k] = x[k] - v[k];
+  }
+}
+
 template <typename T>
-__global__ void __launch_bounds__(1024) cta_scan_kernel(T* __restrict__ a, const int64_t* __restrict__ count,
-                                                        int64_t n_fixed, int64_t* __restrict__ total) {
-  __shared__ int64_t warp_sum_s[32];
-  __shared__ int64_t carry_s;
-  const int64_t n = count ? count[0] : n_fixed;
-  if (threadIdx.x == 0) carry_s = 0;
+__device__ __forceinline__ T warp_scan_excl(T v, T& total) {
+  T a[1] = {v}, t[1];
+  warp_scan_excl(a, t);
+  total = t[0];
+  return a[0];
+}
+
+// exclusive scan of each v[k] across a CTA of THREADS threads, in place; total[k] = the CTA's sum of v[k], on every
+// thread.  Every thread of the CTA calls it; it ends with __syncthreads(), so calls may follow each other.
+template <int THREADS, int N, typename T>
+__device__ __forceinline__ void block_scan_excl(T (&v)[N], T (&total)[N]) {
+  constexpr int WARPS = THREADS / 32;
+  static_assert(THREADS % 32 == 0 && WARPS <= 32, "block_scan_excl: whole warps, at most 1024 threads");
+  __shared__ T warp_s[N][WARPS];
+  const int lane = lane_id(), warp = threadIdx.x >> 5;
+  warp_scan_excl(v, total);
+  if (lane == 0) {
+#pragma unroll
+    for (int k = 0; k < N; ++k) warp_s[k][warp] = total[k];
+  }
   __syncthreads();
+  T w[N];   // every warp scans the warp sums and takes its own warp's offset
+#pragma unroll
+  for (int k = 0; k < N; ++k) w[k] = lane < WARPS ? warp_s[k][lane] : T(0);
+  warp_scan_excl(w, total);
+#pragma unroll
+  for (int k = 0; k < N; ++k) v[k] += __shfl_sync(FULL_MASK, w[k], warp);
+  __syncthreads();
+}
+
+template <typename T, int N>
+struct CtaScanArrays {
+  T* a[N];
+  int64_t* total[N];
+};
+
+// exclusive scans of s.a[k][0, n) in place, n = (count ? *count : 0) + extra; one CTA of 1024 threads, tiles of 1024.
+// Values are summed in int64 and written back as T; the sum of s.a[k] -> *s.total[k] where that is not null.
+template <typename T, int N>
+__global__ void __launch_bounds__(1024) cta_scan_kernel(CtaScanArrays<T, N> s, const int64_t* __restrict__ count,
+                                                        int64_t extra) {
+  const int64_t n = (count ? count[0] : 0) + extra;
+  int64_t carry[N] = {};
   for (int64_t base = 0; base < n; base += 1024) {
     const int64_t i = base + threadIdx.x;
-    const int64_t v = i < n ? (int64_t)a[i] : 0;
-    int64_t x = v;
-    for (int o = 1; o < 32; o <<= 1) {
-      const int64_t y = __shfl_up_sync(FULL_MASK, x, o);
-      if ((threadIdx.x & 31) >= o) x += y;
+    int64_t v[N], tot[N];
+#pragma unroll
+    for (int k = 0; k < N; ++k) v[k] = i < n ? (int64_t)s.a[k][i] : 0;
+    block_scan_excl<1024>(v, tot);
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+      if (i < n) s.a[k][i] = (T)(carry[k] + v[k]);
+      carry[k] += tot[k];
     }
-    if ((threadIdx.x & 31) == 31) warp_sum_s[threadIdx.x >> 5] = x;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-      int64_t w = warp_sum_s[threadIdx.x];
-      for (int o = 1; o < 32; o <<= 1) {
-        const int64_t y = __shfl_up_sync(FULL_MASK, w, o);
-        if (threadIdx.x >= o) w += y;
-      }
-      warp_sum_s[threadIdx.x] = w;
-    }
-    __syncthreads();
-    const int64_t before = carry_s + (threadIdx.x >= 32 ? warp_sum_s[(threadIdx.x >> 5) - 1] : 0) + (x - v);
-    if (i < n) a[i] = (T)before;
-    __syncthreads();
-    if (threadIdx.x == 1023) carry_s = before + v;
-    __syncthreads();
   }
-  if (threadIdx.x == 0 && total) total[0] = carry_s;
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int k = 0; k < N; ++k)
+      if (s.total[k]) *s.total[k] = carry[k];
+  }
+}
+
+// launches cta_scan_kernel over the arrays a (totals -> total, each may be null) and checks the launch
+template <typename T, int N>
+static int cta_scan(T* const (&a)[N], int64_t* const (&total)[N], const int64_t* count, int64_t extra, cudaStream_t st,
+                    const char* what) {
+  CtaScanArrays<T, N> s;
+  for (int k = 0; k < N; ++k) { s.a[k] = a[k]; s.total[k] = total[k]; }
+  cta_scan_kernel<T, N><<<1, 1024, 0, st>>>(s, count, extra);
+  CTR_LAUNCHED(what);
+  return CTR_OK;
 }
 
 // hist[d * nb + b] = items of CTA b with digit d
@@ -135,8 +198,7 @@ static int lsd_sort(uint64_t* keys, uint32_t* vals, uint64_t* keys2, uint32_t* v
   for (int pass = 0; pass < passes; ++pass, cur ^= 1) {
     lsd_hist_kernel<<<nb, LSD_THREADS, 0, st>>>(k[cur], n_dev, pass, hist, hist_count);
     CTR_LAUNCHED(what);
-    cta_scan_kernel<int32_t><<<1, 1024, 0, st>>>(hist, hist_count, 0, nullptr);
-    CTR_LAUNCHED(what);
+    if (int rc = cta_scan({hist}, {nullptr}, hist_count, 0, st, what)) return rc;
     lsd_scatter_kernel<<<nb, LSD_THREADS, 0, st>>>(k[cur], v[cur], n_dev, pass, hist, k[cur ^ 1], v[cur ^ 1]);
     CTR_LAUNCHED(what);
   }

@@ -131,18 +131,6 @@ struct SfFields {
   __device__ int64_t fe(int i) const { return i < nc ? s + sc[i] : te; }
 };
 
-// exclusive warp scan of v; total -> tot
-__device__ __forceinline__ int64_t sf_warp_excl(int64_t v, int64_t& tot) {
-  const int lane = lane_id();
-  int64_t x = v;
-  for (int o = 1; o < 32; o <<= 1) {
-    const int64_t y = __shfl_up_sync(FULL_MASK, x, o);
-    if (lane >= o) x += y;
-  }
-  tot = __shfl_sync(FULL_MASK, x, 31);
-  return x - v;
-}
-
 // ---- the feature_map table -------------------------------------------------------------------------------------
 // ref uint64[cap] (first line + 1, 0 = empty) | win int64[cap] (largest line) | voff, foff int64[cap] | vlen, flen,
 // col int32[cap] (+ pad): 48 bytes a slot.  voff / vlen = the key's value bytes in the map text (empty for a
@@ -351,7 +339,7 @@ __global__ void __launch_bounds__(SF_THREADS) sf_emit_kernel(const uint8_t* __re
       const int i = i0 + lane;
       const int64_t L = i <= nf - 2 ? sf_feature<false>(t, F, i, a, nullptr) : 0;
       int64_t tot;
-      const int64_t x = sf_warp_excl(L, tot);
+      const int64_t x = warp_scan_excl(L, tot);
       if (W && i <= nf - 2) sf_feature<true>(t, F, i, a, o + pos + x);
       pos += tot;
     }
@@ -406,23 +394,6 @@ __global__ void __launch_bounds__(SF_THREADS) fr_emit_kernel(const uint8_t* __re
 }
 
 // ---- line offsets: tiles of SF_SCAN_TILE lengths summed, the sums scanned by one CTA, then each tile scanned ------
-__device__ __forceinline__ int64_t sf_block_excl(int64_t v, int64_t& tot) {
-  __shared__ int64_t ws[SF_SCAN_TILE / 32];
-  const int lane = lane_id(), warp = threadIdx.x >> 5;
-  int64_t wt;
-  const int64_t x = sf_warp_excl(v, wt);
-  if (lane == 0) ws[warp] = wt;
-  __syncthreads();
-  int64_t before = 0;
-  tot = 0;
-  for (int w = 0; w < SF_SCAN_TILE / 32; ++w) {
-    if (w < warp) before += ws[w];
-    tot += ws[w];
-  }
-  __syncthreads();
-  return before + x;
-}
-
 __global__ void __launch_bounds__(SF_SCAN_TILE) sf_tile_sum_kernel(const int64_t* __restrict__ a,
                                                                   const int64_t* __restrict__ n_dev,
                                                                   int64_t* __restrict__ tiles,
@@ -431,9 +402,9 @@ __global__ void __launch_bounds__(SF_SCAN_TILE) sf_tile_sum_kernel(const int64_t
   if (blockIdx.x == 0 && threadIdx.x == 0) n_tiles[0] = nt;
   for (int64_t tile = blockIdx.x; tile < nt; tile += gridDim.x) {
     const int64_t i = tile * SF_SCAN_TILE + threadIdx.x;
-    int64_t tot;
-    sf_block_excl(i < n ? a[i] : 0, tot);
-    if (threadIdx.x == 0) tiles[tile] = tot;
+    int64_t x[1] = {i < n ? a[i] : 0}, tot[1];
+    block_scan_excl<SF_SCAN_TILE>(x, tot);
+    if (threadIdx.x == 0) tiles[tile] = tot[0];
   }
 }
 
@@ -443,9 +414,9 @@ __global__ void __launch_bounds__(SF_SCAN_TILE) sf_tile_scan_kernel(int64_t* __r
   const int64_t n = n_dev[0], nt = (n + SF_SCAN_TILE - 1) / SF_SCAN_TILE;
   for (int64_t tile = blockIdx.x; tile < nt; tile += gridDim.x) {
     const int64_t i = tile * SF_SCAN_TILE + threadIdx.x;
-    int64_t tot;
-    const int64_t x = sf_block_excl(i < n ? a[i] : 0, tot);
-    if (i < n) a[i] = tiles[tile] + x;
+    int64_t x[1] = {i < n ? a[i] : 0}, tot[1];
+    block_scan_excl<SF_SCAN_TILE>(x, tot);
+    if (i < n) a[i] = tiles[tile] + x[0];
   }
 }
 
@@ -455,8 +426,7 @@ static int sf_scan(int64_t* a, const int64_t* n_dev, int64_t max_n, int64_t* til
   const unsigned g = grid_for(max_n, SF_SCAN_TILE, 2);
   sf_tile_sum_kernel<<<g, SF_SCAN_TILE, 0, st>>>(a, n_dev, tiles, n_tiles);
   CTR_LAUNCHED(what);
-  cta_scan_kernel<int64_t><<<1, 1024, 0, st>>>(tiles, n_tiles, 0, total);
-  CTR_LAUNCHED(what);
+  if (int rc = cta_scan({tiles}, {total}, n_tiles, 0, st, what)) return rc;
   sf_tile_scan_kernel<<<g, SF_SCAN_TILE, 0, st>>>(a, n_dev, tiles);
   CTR_LAUNCHED(what);
   return CTR_OK;

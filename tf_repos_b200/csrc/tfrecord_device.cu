@@ -23,7 +23,7 @@
 #include "common.cuh"
 #include "crc32c.cuh"
 #include "example_wire.cuh"   // tr_map_entries, tr_feature_kind and the wire helpers
-#include "scan_sort.cuh"      // cta_scan_kernel
+#include "scan_sort.cuh"      // cta_scan
 
 namespace ctr {
 
@@ -383,9 +383,7 @@ int ctr_din_serve_scan(const void* data, const int64_t* offsets, int64_t n, int6
   tr_din_serve_scan_kernel<<<grid_for(B, TR_WARPS, 16), TR_THREADS, 0, st>>>(
       static_cast<const uint8_t*>(data), offsets, (int)n, B, example_base, F, max_a_int, slot_off, slot_len, a_int_off,
       maxima, reinterpret_cast<unsigned long long*>(err));
-  cta_scan_kernel<int32_t><<<1, 1024, 0, st>>>(a_int_off, nullptr, (int64_t)B + 1, nullptr);
-  CTR_LAUNCHED("ctr_din_serve_scan");
-  return CTR_OK;
+  return cta_scan({a_int_off}, {nullptr}, nullptr, (int64_t)B + 1, st, "ctr_din_serve_scan");
 }
 
 int ctr_tfrecord_emit_esmm(const void* stage, const int64_t* slot_off, const int32_t* slot_len, int B, int F,
