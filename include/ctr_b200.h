@@ -179,21 +179,17 @@ int ctr_epoch_rows(int opt, int apply, float* var, float* slot0, float* slot1, u
                    const int32_t* uniq, const int32_t* n_uniq, const float* g_uniq, int64_t n_max, int K,
                    const float* hyper, const float* lr_table, int j, double* ss, ctr_stream_t stream);
 /* ctr_epoch_rows for the [N,K] table AND a scalar table [N] gathered with the same ids (fm_v + fm_w, DeepFM.py:115-116)
- * in one launch; K in {4, 8, 16, 32, 64, 128, 256}.  Same arithmetic as two ctr_epoch_rows calls. */
+ * in one launch; K in {4, 8, 16, 32, 64, 128, 256}.  Same arithmetic as two ctr_epoch_rows calls.  w_last == last: the
+ * tables share one `last` byte per row (see ctr_epoch_sweep).
+ * stage / w_stage: both NULL, or both given (device float[n_max * 3K] and float[n_max * 3], indexed by unique row).
+ * Given, the catch-up (apply=0) and the apply (apply=1) of the same step j hand the rows over through them: the catch-up
+ * writes the caught-up var | slot0 | slot1 there and only var back to the tables; the apply reads them from there and
+ * writes every row, slot and `last` byte.  Same results as without a stage.  Both calls of a step must then use the same
+ * uniq / n_uniq and stage, and between them only var of the gathered rows may be read (the slots and `last` are stale). */
 int ctr_epoch_rows2(int opt, int apply, float* var, float* slot0, float* slot1, uint8_t* last, float* w_var, float* w_slot0,
                     float* w_slot1, uint8_t* w_last, const int32_t* uniq, const int32_t* n_uniq, const float* g_uniq,
                     const float* gw_uniq, int64_t n_max, int K, const float* hyper, const float* lr_table, int j, double* ss,
-                    double* ss_w, ctr_stream_t stream);
-/* ctr_epoch_rows2 with the catch-up (apply=0) and the apply (apply=1) of the same step j handing the rows over through
- * stage (device float[n_max * 3K]) and w_stage (device float[n_max * 3]), indexed by unique row: the catch-up writes
- * the caught-up var | slot0 | slot1 there and only var back to the tables; the apply reads them from there and writes
- * every row, slot and `last` byte.  Same results as ctr_epoch_rows2.  Both calls of a step must use the same uniq /
- * n_uniq and stage, and between them only var of the gathered rows may be read (the slots and `last` are stale). */
-int ctr_epoch_rows2_staged(int opt, int apply, float* var, float* slot0, float* slot1, uint8_t* last, float* w_var,
-                           float* w_slot0, float* w_slot1, uint8_t* w_last, const int32_t* uniq, const int32_t* n_uniq,
-                           const float* g_uniq, const float* gw_uniq, int64_t n_max, int K, const float* hyper,
-                           const float* lr_table, int j, double* ss, double* ss_w, float* stage, float* w_stage,
-                           ctr_stream_t stream);
+                    double* ss_w, float* stage, float* w_stage, ctr_stream_t stream);
 /* All rows -> state after `upto` steps of this epoch.  Rows whose `last` byte equals `from` (nothing gathered
  * them since the previous sweep; from = 0 after an epoch-end sweep) replay steps from..upto-1; the others replay
  * last..upto-1.  reset != 0: epoch end, every `last` byte returns to 0; reset == 0: mid-epoch flush, `last` = upto.
@@ -201,38 +197,32 @@ int ctr_epoch_rows2_staged(int opt, int apply, float* var, float* slot0, float* 
  * 6 * ctr_device_sm_count(), so it can be sized before the first call), ZERO-INITIALISED ONCE by the caller: a call
  * rewrites, for every step < upto, one entry per CTA it launches (fewer than *n_partials_host) and ctr_epoch_reg_loss
  * sums whole rows, so the entries no CTA owns must hold 0.
- * list / list_cap / list_count / ss_rows (optional, Adam): scratch for the packed-pipe sweep (csrc/epoch_adam.cu):
- * device int32[list_cap], a device int32 counter, and the row kernels' per-step sum(var^2) accumulator (the `ss` of
- * ctr_epoch_rows).  NULL selects the scalar kernels.
+ * list / list_cap / list_count / ss_rows: required for Adam (CTR_ERR_INVALID_ARG if one is missing or list_cap is 0),
+ * unused otherwise: device int32[list_cap], a device int32 counter, and the row kernels' per-step sum(var^2)
+ * accumulator (the `ss` of ctr_epoch_rows).  Adam with K % 4 == 0 and K <= 256, or K == 1 with n_rows % 4 == 0 and a
+ * 4-byte aligned `last`, takes the packed-pipe sweep (csrc/epoch_adam.cu): it lists the rows gathered since `from`
+ * and catches them up in a second pass.
  * CAPACITY: the list receives every row whose `last` byte exceeds `from`, i.e. every row a ctr_epoch_rows call
  * gathered since the previous sweep.  With at most n_ids distinct ids per step that is at most
  * min(n_rows, n_ids * (upto - from)) <= min(n_rows, n_ids * ctr_epoch_max_steps()) rows; list_cap must be at least
  * that.  *list_count returns the number of gathered rows found.  If it exceeds list_cap, the rows beyond list_cap
- * were NOT caught up although their `last` byte is rewritten: the table is wrong.  ctr_epoch_sweep_ovf reports this. */
-int ctr_epoch_sweep(int opt, float* var, float* slot0, float* slot1, uint8_t* last, int64_t n_rows, int K,
-                    const float* hyper, const float* lr_table, int from, int upto, int reset, double* ss_partials,
-                    int* n_partials_host, int32_t* list, int64_t list_cap, int32_t* list_count, double* ss_rows,
+ * were NOT caught up although their `last` byte is rewritten: the table is wrong.
+ * list_overflow (nullable): device int32 counter to which the packed sweep ADDS the number of gathered rows it found
+ * beyond list_cap (it is not cleared here).  Non-zero after a call means the capacity rule above was broken and the
+ * table no longer holds the every-step state; the models' check_ids() raises on it.
+ * w_var, w_slot0, w_slot1, w_ss_partials, w_ss_rows: all NULL (one table), or all given: a scalar table [n_rows]
+ * gathered with the same ids as the [N,K] table (fm_v + fm_w) that shares its `last` bytes (pass the same `last` to
+ * ctr_epoch_rows2 as both last and w_last).  One launch then sweeps both tables, rows gathered since `from` go to one
+ * list, and its catch-up steps both tables; w_ss_partials / w_ss_rows are the scalar table's ss_partials / ss_rows.
+ * The list holds each gathered ROW once (not once per table), so the same list_cap covers both.  Needs
+ * ctr_epoch_shared_last_supported (Adam, K in {4, 8, ..., 256}, n_rows % 4 == 0) and a 4-byte aligned `last`;
+ * otherwise keep one `last` array per table and sweep each on its own. */
+int ctr_epoch_shared_last_supported(int opt, int64_t n_rows, int K);
+int ctr_epoch_sweep(int opt, float* var, float* slot0, float* slot1, float* w_var, float* w_slot0, float* w_slot1,
+                    uint8_t* last, int64_t n_rows, int K, const float* hyper, const float* lr_table, int from, int upto,
+                    int reset, double* ss_partials, double* w_ss_partials, int* n_partials_host, int32_t* list,
+                    int64_t list_cap, int32_t* list_count, double* ss_rows, double* w_ss_rows, int32_t* list_overflow,
                     ctr_stream_t stream);
-/* ctr_epoch_sweep, plus list_overflow (nullable): device int32 counter to which the packed sweep ADDS the number of
- * gathered rows it found beyond list_cap (it is not cleared here).  Non-zero after a call means the capacity rule
- * above was broken and the table no longer holds the every-step state; the models' check_ids() raises on it. */
-int ctr_epoch_sweep_ovf(int opt, float* var, float* slot0, float* slot1, uint8_t* last, int64_t n_rows, int K,
-                        const float* hyper, const float* lr_table, int from, int upto, int reset, double* ss_partials,
-                        int* n_partials_host, int32_t* list, int64_t list_cap, int32_t* list_count, double* ss_rows,
-                        int32_t* list_overflow, ctr_stream_t stream);
-/* ctr_epoch_sweep_ovf for the [N,K] table AND a scalar table [N] gathered with the same ids (fm_v + fm_w) that share
- * ONE `last` byte per row (pass the same `last` to ctr_epoch_rows2 as both last and w_last): one launch sweeps both
- * tables, rows gathered since `from` go to one list, and its catch-up steps both tables.  Adam with the packed sweep
- * only (ctr_epoch_sweep2_supported: K in {4, 8, ..., 256}, n_rows % 4 == 0, CTR_EPOCH_SCALAR unset); otherwise keep
- * one `last` array per table and call ctr_epoch_sweep_ovf per table.  ss_partials / w_ss_partials and ss_rows /
- * w_ss_rows are each table's as in ctr_epoch_sweep.  CAPACITY: as ctr_epoch_sweep; the list holds each gathered ROW
- * once (not once per table), so the same list_cap covers both tables, and list_overflow counts dropped rows. */
-int ctr_epoch_sweep2_supported(int opt, int64_t n_rows, int K);
-int ctr_epoch_sweep2(int opt, float* var, float* slot0, float* slot1, float* w_var, float* w_slot0, float* w_slot1,
-                     uint8_t* last, int64_t n_rows, int K, const float* hyper, const float* lr_table, int from, int upto,
-                     int reset, double* ss_partials, double* w_ss_partials, int* n_partials_host, int32_t* list,
-                     int64_t list_cap, int32_t* list_count, double* ss_rows, double* w_ss_rows, int32_t* list_overflow,
-                     ctr_stream_t stream);
 /* reg[s] (+)= scale*(ss_rows[s] + sum_b ss_partials[s][b]) for s < upto; clears ss_rows[s] */
 int ctr_epoch_reg_loss(double* ss_rows, const double* ss_partials, int n_partials, int upto, float scale,
                        float* reg, int accumulate, ctr_stream_t stream);
@@ -365,16 +355,13 @@ int ctr_esmm_head(const float* y_ctr, const float* y_cvr, const float* y, const 
  * bag_sum: tf.nn.embedding_lookup_sparse(combiner="sum") over CSR bags (a_intids, DIN.py:148; the
  *     non-attention pooling branch :180-183) and its gradient g_rows[i] = d_out[bag(i)] * w_i.
  *     An id outside [0,N) adds nothing; bag_sum_fwd_oob also counts it into oob[0] (oob[1] = first) like
- *     ctr_gather_scale_rows (TF raises InvalidArgumentError).  ctr_bag_sum_fwd is bag_sum_fwd_oob with oob = NULL.
+ *     ctr_gather_scale_rows (TF raises InvalidArgumentError); oob may be NULL.
  * din_pool: att = sigmoid(z); u[b] = sum_p (ids[b,p] > 0) * att[b,p] * E[b,p,:]   (DIN.py:169-172)
  *     bwd: dE = mask*att*du (written, not accumulated); dz = mask*att*(1-att)*(E . du)
- * group_sum: dU[b] = sum_p dZ[b*P+p]   (gradient of ctr_fc_fwd_grouped's group bias)
  * scale_rows: out[i,:] = (x[(i/G)*ld_group + (i%G)*K : +K] + add[i,:]) * w[i]  (add, w optional)
  * axpby: out = alpha*a + beta*b */
 int ctr_gather_scale_rows(const int32_t* ids, const float* wgt, const float* V, int64_t N, int64_t n, int K,
                           int G, int64_t ld_group, float* out, int32_t* oob, ctr_stream_t stream);
-int ctr_bag_sum_fwd(const int32_t* ids, const float* wgt, const int32_t* offsets, const float* V, int64_t N,
-                    int B, int K, int64_t ld, float* out, ctr_stream_t stream);
 int ctr_bag_sum_fwd_oob(const int32_t* ids, const float* wgt, const int32_t* offsets, const float* V, int64_t N,
                         int B, int K, int64_t ld, float* out, int32_t* oob, ctr_stream_t stream);
 int ctr_bag_sum_bwd(const float* d_out, int64_t ld, const float* wgt, const int32_t* offsets, int B, int K,
@@ -385,7 +372,6 @@ int ctr_din_pool_fwd(const float* E, const float* z, const int32_t* ids, int B, 
                      int64_t ld_u, ctr_stream_t stream);
 int ctr_din_pool_bwd(const float* E, const float* att, const int32_t* ids, const float* du, int64_t ld_u, int B,
                      int P, int K, float* dE, float* dz, ctr_stream_t stream);
-int ctr_group_sum(const float* dZ, int B, int P, int N, float* dU, ctr_stream_t stream);
 /* Attention unit backward through the N=1 output and the hidden layer's relu/dropout in ONE pass over the [B*P, H] hidden
  * activations Hh (autodiff of DIN.py:164-169): dZ[r][c] = dz[r]*w2[c] (*mask/keep) where Hh > 0; dU[b][c] = sum_p dZ
  * (the group-bias gradient; colsum(dU) is the layer's bias gradient); gw2_part[b][c] = sum_p dz*Hh (colsum = the output
@@ -420,14 +406,8 @@ int ctr_afm_pool_bwd(const float* pw, const float* att, const float* mask, float
 int ctr_dropout_apply(const float* x, const float* mask, float keep, int64_t n, float* out, ctr_stream_t stream);
 
 /* ---- row-sharded table routing (not in the reference; SURVEY.md 8e) ---------------------------------
- * owner(id) = id % G, local row = id / G.  bucket_ids: the *n_uniq sorted unique ids of a batch are
- * grouped by owner: counts[G]; order[pos] = index into uniq; pos_of[u] = pos; local_ids[pos] = id / G
- * (bucket-major: the send buffer of the id all-to-all).  remap_ids: out[i] = pos_of[inverse[i]] turns
- * the batch's ids into indices of the received row cache.  gather_scalar: out[i] = W[ids[i]]. */
-int ctr_a2a_bucket_ids(const int32_t* uniq, const int32_t* n_uniq, int64_t n_max, int G, int32_t* counts,
-                       int32_t* cursor, int32_t* order, int32_t* pos_of, int32_t* local_ids, ctr_stream_t stream);
-int ctr_remap_ids(const int32_t* inverse, const int32_t* pos_of, int64_t n, int32_t* out, ctr_stream_t stream);
-/* Composite routing keys (what tf_repos_b200/sharded.py uses): key(id) = (id % G) * ceil(N/G) + id / G, so that ONE
+ * owner(id) = id % G, local row = id / G.  gather_scalar: out[i] = W[ids[i]].
+ * Routing keys (tf_repos_b200/sharded.py): key(id) = (id % G) * ceil(N/G) + id / G, so that ONE
  * ctr_unique_segment of the keys yields the unique ids in bucket order (owner-major, ascending id inside an owner),
  * `inverse` = the occurrence's position in the received row cache, and perm / seg_offsets = the gradient segments in
  * cache order.  ids outside [0, N) are counted in oob (may be NULL) and routed to row 0.

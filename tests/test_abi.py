@@ -13,7 +13,7 @@ def _declared_symbols():
     return sorted(set(re.findall(r"\b(ctr_[a-z0-9_]+)\s*\(", text)))
 
 
-def test_header_symbols_are_exported_and_bound():
+def test_header_symbols_are_exported_and_bound_at_abi_2():
     from tf_repos_b200 import _lib
     names = _declared_symbols()
     assert "ctr_fm_embed_fwd" in names and len(names) >= 15
@@ -22,7 +22,7 @@ def test_header_symbols_are_exported_and_bound():
         assert hasattr(lib, n), f"{n} declared in include/ctr_b200.h but not exported"
         assert n in _lib.SIGNATURES, f"{n} has no ctypes signature in tf_repos_b200/_lib.py"
     assert set(_lib.SIGNATURES) <= set(names)
-    assert _lib.abi_version() == 1
+    assert _lib.abi_version() == 2
 
 
 def test_argument_validation_needs_no_gpu():

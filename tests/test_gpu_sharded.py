@@ -14,30 +14,18 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.mark.parametrize("G", [1, 2, 3, 8])
-def test_bucket_kernels_match_plan(G):
+def test_shard_routing_kernels_match_plan(G):
     from tf_repos_b200 import dist_plan as dp
     from tf_repos_b200 import ops
     d = torch.device("cuda:0")
     rng = np.random.default_rng(G)
     ids = rng.integers(0, 50_000, size=20_000).astype(np.int32)
-    uniq, inverse = np.unique(ids, return_inverse=True)
+    uniq = np.unique(ids)
     U = len(uniq)
     n = len(ids)
     i32 = dict(dtype=torch.int32, device=d)
-    counts = torch.zeros(G, **i32); cursor = torch.zeros(G, **i32)
-    order = torch.empty(n, **i32); pos_of = torch.empty(n, **i32); local_ids = torch.empty(n, **i32)
-    uq = torch.zeros(n, **i32); uq[:U] = torch.from_numpy(uniq).to(d)
-    ops.a2a_bucket_ids(uq, torch.tensor([U], **i32), n, G, counts, cursor, order, pos_of, local_ids)
-    ref_counts, ref_order, ref_local = dp.route_plan(uniq.astype(np.int64), G)
-    assert counts.tolist() == ref_counts.tolist()
-    o = order[:U].cpu().numpy(); p = pos_of[:U].cpu().numpy(); l = local_ids[:U].cpu().numpy()
-    assert sorted(o.tolist()) == list(range(U)) and np.array_equal(p[o], np.arange(U))
-    own = uniq[o] % G
-    assert np.all(np.diff(own) >= 0) and np.array_equal(l.astype(np.int64) * G + own, uniq[o])
-    remap = torch.empty(n, **i32)
-    ops.remap_ids(torch.from_numpy(inverse.astype(np.int32)).to(d), pos_of, n, remap)
-    assert np.array_equal(uniq[o][remap.cpu().numpy()], ids)
-    # composite routing keys: one sort gives the same plan, deterministically
+    ref_counts, _, ref_local = dp.route_plan(uniq.astype(np.int64), G)
+    # composite routing keys: one sort gives the plan, deterministically
     from tf_repos_b200.ops import UniqueWorkspace
     N = 50_000
     npad = (N + G - 1) // G

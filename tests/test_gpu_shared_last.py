@@ -1,7 +1,7 @@
 """One `last` array for an [N,K] table and the [N] table gathered with the same ids (DeepFM's fm_v and fm_w).
 
 With Adam on the packed sweep, K in {4, ..., 256} and N % 4 == 0, the updater keeps one `last` byte per row and one row
-list for both tables, and ctr_epoch_sweep2 sweeps both in one launch.  The state must stay bit for bit that of the
+list for both tables, and one ctr_epoch_sweep call sweeps both in one launch.  The state must stay bit for bit that of the
 every-step sweep; otherwise (N % 4 != 0, non-Adam) the tables keep their own `last` arrays."""
 import pytest
 import torch
@@ -97,9 +97,10 @@ def test_separate_last_arrays_where_the_pair_sweep_does_not_apply(N, optimizer):
 
 
 @pytest.mark.parametrize("K,shared", [(16, True), (16, False), (256, True)])
-def test_staged_rows_equal_unstaged_rows(K, shared):
-    """ctr_epoch_rows2_staged against ctr_epoch_rows2 on the same rows: after the catch-up `var` of both tables is the
-    same, and after the apply every array, `last` and the sum(var^2) accumulators are."""
+def test_rows2_with_stage_equals_rows2_without_stage(K, shared):
+    """ctr_epoch_rows2 with a stage against ctr_epoch_rows2 without one (stage = NULL) on the same rows: after the
+    catch-up `var` of both tables is the same, and after the apply every array, `last` and the sum(var^2) accumulators
+    are."""
     from tf_repos_b200 import ops
     from tf_repos_b200.engine import OptimizerState, Table
     dev, N, n, j = torch.device("cuda:0"), 4096, 700, 5
@@ -125,10 +126,7 @@ def test_staged_rows_equal_unstaged_rows(K, shared):
         for apply in (False, True):
             args = (opt.opt, apply, V, W, lv, lw, uniq, n_uniq, gv if apply else None, gw if apply else None, n,
                     opt.record(0), opt.lr_table, j, ss[0], ss[1])
-            if staged:
-                ops.epoch_rows2_staged(*args, *st)
-            else:
-                ops.epoch_rows2(*args)
+            ops.epoch_rows2(*args, *(st if staged else (None, None)))
             if not apply:
                 out["var_after_catch_up"] = (V.var.clone(), W.var.clone())
         torch.cuda.synchronize()

@@ -1,6 +1,6 @@
 """The measurement switches of DESIGN.md §5 ("A/B switches") must not change results: each alternative setting is run in
 its own process (the switches are read once per process) on a small DeepFM job and compared with the default run, bit
-for bit (scalar vs packed Adam epoch sweep, K1 LDG vs TMA staging).  In every process the exact-deferred state must
+for bit (K1 LDG vs TMA staging).  In every process the exact-deferred state must
 equal the every-step state bit for bit (reference semantics: DeepFM.py:188-213, every row moves every step)."""
 import json
 import os
@@ -54,7 +54,6 @@ def default_run():
 
 
 @pytest.mark.parametrize("env", [
-    {"CTR_EPOCH_SCALAR": "1"},
     {"CTR_FM_EMBED_TMA": "1"},
     {"CTR_FM_EMBED_TMA": "0"},
 ], ids=lambda e: ",".join(f"{k}={v}" for k, v in e.items()))

@@ -49,16 +49,11 @@ SIGNATURES = {
     "ctr_epoch_max_steps": (c_int, []),
     "ctr_epoch_tick": (c_int, [P, P, c_int, P, c_int, c_int, P]),
     "ctr_epoch_rows": (c_int, [c_int, c_int, P, P, P, P, P, P, P, c_int64, c_int, P, P, c_int, P, P]),
-    "ctr_epoch_rows2": (c_int, [c_int, c_int, P, P, P, P, P, P, P, P, P, P, P, P, c_int64, c_int, P, P, c_int, P, P, P]),
-    "ctr_epoch_rows2_staged": (c_int, [c_int, c_int, P, P, P, P, P, P, P, P, P, P, P, P, c_int64, c_int, P, P, c_int, P,
-                                       P, P, P, P]),
-    "ctr_epoch_sweep": (c_int, [c_int, P, P, P, P, c_int64, c_int, P, P, c_int, c_int, c_int, P,
-                                ctypes.POINTER(c_int), P, c_int64, P, P, P]),
-    "ctr_epoch_sweep_ovf": (c_int, [c_int, P, P, P, P, c_int64, c_int, P, P, c_int, c_int, c_int, P,
-                                    ctypes.POINTER(c_int), P, c_int64, P, P, P, P]),
-    "ctr_epoch_sweep2_supported": (c_int, [c_int, c_int64, c_int]),
-    "ctr_epoch_sweep2": (c_int, [c_int, P, P, P, P, P, P, P, c_int64, c_int, P, P, c_int, c_int, c_int, P, P,
-                                 ctypes.POINTER(c_int), P, c_int64, P, P, P, P, P]),
+    "ctr_epoch_rows2": (c_int, [c_int, c_int, P, P, P, P, P, P, P, P, P, P, P, P, c_int64, c_int, P, P, c_int, P, P, P,
+                                P, P]),
+    "ctr_epoch_shared_last_supported": (c_int, [c_int, c_int64, c_int]),
+    "ctr_epoch_sweep": (c_int, [c_int, P, P, P, P, P, P, P, c_int64, c_int, P, P, c_int, c_int, c_int, P, P,
+                                ctypes.POINTER(c_int), P, c_int64, P, P, P, P, P]),
     "ctr_epoch_reg_loss": (c_int, [P, P, c_int, c_int, c_float, P, c_int, P]),
     "ctr_selftest_divsqrt": (c_int, [c_uint64, c_int64, P, P]),
     "ctr_selftest_adam_packed": (c_int, [c_int, c_uint64, c_int64, c_int, c_float, c_float, P, P]),
@@ -87,13 +82,11 @@ SIGNATURES = {
     "ctr_esmm_embed_bwd": (c_int, [P, P, P, c_int, c_int, c_int, c_int64, P, P]),
     "ctr_esmm_head": (c_int, [P, P, P, P, c_int, c_int, c_float, c_float, P, P, P, P, P, P, P]),
     "ctr_gather_scale_rows": (c_int, [P, P, P, c_int64, c_int64, c_int, c_int, c_int64, P, P, P]),
-    "ctr_bag_sum_fwd": (c_int, [P, P, P, P, c_int64, c_int, c_int, c_int64, P, P]),
     "ctr_bag_sum_fwd_oob": (c_int, [P, P, P, P, c_int64, c_int, c_int, c_int64, P, P, P]),
     "ctr_bag_sum_bwd": (c_int, [P, c_int64, P, P, c_int, c_int, P, P]),
     "ctr_scale_rows": (c_int, [P, P, P, c_int64, c_int, c_int, c_int64, P, P]),
     "ctr_din_pool_fwd": (c_int, [P, P, P, c_int, c_int, c_int, P, P, c_int64, P]),
     "ctr_din_pool_bwd": (c_int, [P, P, P, P, c_int64, c_int, c_int, c_int, P, P, P]),
-    "ctr_group_sum": (c_int, [P, c_int, c_int, c_int, P, P]),
     "ctr_din_att_dz": (c_int, [P, P, c_float, P, P, c_int, c_int, c_int, P, P, P, P]),
     "ctr_colsum_rows": (c_int, [P, c_int, c_int, c_int, P, P]),
     "ctr_axpby": (c_int, [P, c_float, P, c_float, c_int64, P, P]),
@@ -104,8 +97,6 @@ SIGNATURES = {
     "ctr_afm_pool_fwd": (c_int, [P, P, P, c_float, c_int, c_int, c_int, P, P, P]),
     "ctr_afm_pool_bwd": (c_int, [P, P, P, c_float, P, c_int, c_int, c_int, P, P, P]),
     "ctr_dropout_apply": (c_int, [P, P, c_float, c_int64, P, P]),
-    "ctr_a2a_bucket_ids": (c_int, [P, P, c_int64, c_int, P, P, P, P, P, P]),
-    "ctr_remap_ids": (c_int, [P, P, c_int64, P, P]),
     "ctr_shard_keys": (c_int, [P, c_int64, c_int64, c_int, P, P, P]),
     "ctr_shard_split": (c_int, [P, P, c_int64, c_int64, c_int, P, P, P]),
     "ctr_gather_scalar": (c_int, [P, P, c_int64, c_int64, P, P]),

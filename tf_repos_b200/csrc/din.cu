@@ -186,17 +186,6 @@ din_pool_bwd_kernel(const float* __restrict__ E, const float* __restrict__ att, 
   }
 }
 
-// dU[b][n] = sum_p dZ[(b*P + p)][n]
-__global__ void __launch_bounds__(256)
-group_sum_kernel(const float* __restrict__ dZ, int B, int P, int N, float* __restrict__ dU) {
-  const int b = blockIdx.x;
-  for (int n = threadIdx.x; n < N; n += blockDim.x) {
-    float s = 0.f;
-    for (int p = 0; p < P; ++p) s += dZ[((int64_t)b * P + p) * N + n];
-    dU[(int64_t)b * N + n] = s;
-  }
-}
-
 // out = alpha*a + beta*b
 __global__ void axpby_kernel(const float* __restrict__ a, float alpha, const float* __restrict__ b, float beta,
                              int64_t n, float* __restrict__ out) {
@@ -223,7 +212,7 @@ using namespace ctr;
 // Replaces three passes over the hidden activations of a behaviour field (autodiff of DIN.py:164-169):
 //   fc1_bwd   dHh[r][c] = dz[r]*w2[c]                      (+ gw2 = sum_r dz[r]*Hh[r][c], gb2 = sum_r dz[r])
 //   fc_dz     dZ = dHh*mask/keep * (Hh > 0)                (+ db1 = colsum dZ)
-//   group_sum dU[b][c] = sum_p dZ[b*P+p][c]
+//   sum_p     dU[b][c] = sum_p dZ[b*P+p][c]              (the group-bias gradient)
 // One CTA per sample (its P rows are contiguous); a thread owns column(s) c, walks the P rows, writes dZ, and keeps
 // sum_p dZ (= dU row b; db1 = colsum(dU)) and sum_p dz*Hh (gw2 partial row b) in registers: no atomics, fixed order.
 __global__ void __launch_bounds__(256)
@@ -268,23 +257,18 @@ int ctr_gather_scale_rows(const int32_t* ids, const float* wgt, const float* V, 
   return CTR_OK;
 }
 
-int ctr_bag_sum_fwd(const int32_t* ids, const float* wgt, const int32_t* offsets, const float* V, int64_t N,
-                    int B, int K, int64_t ld, float* out, ctr_stream_t stream) {
-  return ctr_bag_sum_fwd_oob(ids, wgt, offsets, V, N, B, K, ld, out, nullptr, stream);
-}
-
 int ctr_bag_sum_fwd_oob(const int32_t* ids, const float* wgt, const int32_t* offsets, const float* V, int64_t N,
                         int B, int K, int64_t ld, float* out, int32_t* oob, ctr_stream_t stream) {
-  CTR_REQUIRE(B >= 0 && K > 0 && N > 0, CTR_ERR_INVALID_ARG, "ctr_bag_sum_fwd: bad args");
+  CTR_REQUIRE(B >= 0 && K > 0 && N > 0, CTR_ERR_INVALID_ARG, "ctr_bag_sum_fwd_oob: bad args");
   if (B == 0) return CTR_OK;
-  CTR_REQUIRE(offsets && V && out, CTR_ERR_INVALID_ARG, "ctr_bag_sum_fwd: null buffer");
+  CTR_REQUIRE(offsets && V && out, CTR_ERR_INVALID_ARG, "ctr_bag_sum_fwd_oob: null buffer");
   cudaStream_t st = as_stream(stream);
 #define BF(LPR, VEC)                                                                                                   \
   bag_sum_fwd_kernel<LPR, VEC><<<(unsigned)ceil_div64((int64_t)B * LPR, 256), 256, 0, st>>>(ids, wgt, offsets, V, N, B, \
                                                                                             ld, out, oob);
   DIN_K_SWITCH(K, BF)
 #undef BF
-  CTR_LAUNCHED("ctr_bag_sum_fwd");
+  CTR_LAUNCHED("ctr_bag_sum_fwd_oob");
   return CTR_OK;
 }
 
@@ -339,15 +323,6 @@ int ctr_din_pool_bwd(const float* E, const float* att, const int32_t* ids, const
   DIN_K_SWITCH(K, PB)
 #undef PB
   CTR_LAUNCHED("ctr_din_pool_bwd");
-  return CTR_OK;
-}
-
-int ctr_group_sum(const float* dZ, int B, int P, int N, float* dU, ctr_stream_t stream) {
-  CTR_REQUIRE(B >= 0 && P >= 0 && N > 0, CTR_ERR_INVALID_ARG, "ctr_group_sum: bad args");
-  if (B == 0) return CTR_OK;
-  CTR_REQUIRE(dZ && dU, CTR_ERR_INVALID_ARG, "ctr_group_sum: null buffer");
-  group_sum_kernel<<<B, 256, 0, as_stream(stream)>>>(dZ, B, P, N, dU);
-  CTR_LAUNCHED("ctr_group_sum");
   return CTR_OK;
 }
 

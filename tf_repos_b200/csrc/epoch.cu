@@ -15,14 +15,13 @@
 //
 // Replaces the same reference lines as optim.cu: optimizer.minimize (DeepFM.py:204-213) with the
 // dense l2_loss gradient (DeepFM.py:189-190) [TF-sem].
-#include <stdlib.h>
-
 #include "optim_steps.cuh"
 
 namespace ctr {
 
 // epoch_adam.cu: Adam sweep on the packed fp32 pipe (rows nothing gathered since `from`; the others go to `list`)
-// w_*: an optional scalar table [n_rows] that shares `last` and is swept in the same launch
+// w_*: an optional scalar table [n_rows] that shares `last` and is swept in the same launch.  Returns false if the
+// shape does not fit the packed kernels.
 bool launch_epoch_sweep_adam(float* var, float* slot0, float* slot1, const uint8_t* last, int64_t n_rows, int K,
                              const float* hyper, const float* lr_table, int from, int upto, double* ss_partials,
                              int n_partials, int32_t* list, int32_t* list_count, int64_t list_cap,
@@ -266,6 +265,7 @@ __device__ __forceinline__ void sweep_ss_flush(float (*ss_thr)[256], int upto, d
   }
 }
 
+// Adagrad / Momentum / Ftrl (Adam has its own sweep, epoch_adam.cu)
 template <int OPT>
 __global__ void __launch_bounds__(256, 3)
 epoch_sweep_kernel(float* __restrict__ var, float* __restrict__ slot0, float* __restrict__ slot1,
@@ -282,7 +282,6 @@ epoch_sweep_kernel(float* __restrict__ var, float* __restrict__ slot0, float* __
   for (int s = 0; s < upto; ++s) ss_thr[s][threadIdx.x] = 0.f;
   __syncthreads();
   Hyper h = load_hyper(hyper);
-  const AdamConsts ac = adam_consts(h);
   float4* v4 = reinterpret_cast<float4*>(var);
   float4* a4 = reinterpret_cast<float4*>(slot0);
   float4* b4 = reinterpret_cast<float4*>(slot1);
@@ -310,32 +309,15 @@ epoch_sweep_kernel(float* __restrict__ var, float* __restrict__ slot0, float* __
         l0[u] = upto;
       }
     }
-    int lmax = l0[0];
-#pragma unroll
-    for (int u = 1; u < UNROLL; ++u) lmax = max(lmax, l0[u]);
-    const int wmax = __reduce_max_sync(FULL_MASK, lmax);   // from step wmax on, the whole warp advances
 #pragma unroll 1
     for (int s = 0; s < upto; ++s) {
       h.lr = lr_s[s];
       float q = 0.f;
-      if (OPT == CTR_OPT_ADAM) {
-        if (s >= wmax) {      // common case (rows not gathered this epoch): no masks
 #pragma unroll
-          for (int u = 0; u < UNROLL; ++u) q += sq4(x[u]);
-          adam_untouched<UNROLL>(x, a, b, h, ac);
-        } else {              // some rows of this warp are already past step s
-          bool act[UNROLL];
-#pragma unroll
-          for (int u = 0; u < UNROLL; ++u) { act[u] = s >= l0[u]; q += act[u] ? sq4(x[u]) : 0.f; }
-          adam_untouched<UNROLL, true>(x, a, b, h, ac, act);
-        }
-      } else {
-#pragma unroll
-        for (int u = 0; u < UNROLL; ++u) {
-          if (s >= l0[u]) {
-            q += sq4(x[u]);
-            step_untouched4<OPT>(x[u], a[u], b[u], h);
-          }
+      for (int u = 0; u < UNROLL; ++u) {
+        if (s >= l0[u]) {
+          q += sq4(x[u]);
+          step_untouched4<OPT>(x[u], a[u], b[u], h);
         }
       }
       ss_thr[s][threadIdx.x] += q;
@@ -358,7 +340,7 @@ epoch_sweep_kernel(float* __restrict__ var, float* __restrict__ slot0, float* __
   sweep_ss_flush(ss_thr, upto, ss_partials, n_partials);
 }
 
-// K == 1 (first-order weights fm_w): a float4 spans 4 rows, each with its own `last` byte
+// K == 1 (first-order weights fm_w): a float4 spans 4 rows, each with its own `last` byte.  Adagrad / Momentum / Ftrl.
 template <int OPT>
 __global__ void __launch_bounds__(256)
 epoch_sweep_k1_kernel(float* __restrict__ var, float* __restrict__ slot0, float* __restrict__ slot1,
@@ -374,7 +356,6 @@ epoch_sweep_k1_kernel(float* __restrict__ var, float* __restrict__ slot0, float*
   for (int s = 0; s < upto; ++s) ss_thr[s][threadIdx.x] = 0.f;
   __syncthreads();
   Hyper h = load_hyper(hyper);
-  const AdamConsts ac = adam_consts(h);
   float4* v4 = reinterpret_cast<float4*>(var);
   float4* a4 = reinterpret_cast<float4*>(slot0);
   float4* b4 = reinterpret_cast<float4*>(slot1);
@@ -391,28 +372,14 @@ epoch_sweep_k1_kernel(float* __restrict__ var, float* __restrict__ slot0, float*
     }
     const int l0 = ok ? (int)(lw & 255u) : upto, l1 = ok ? (int)((lw >> 8) & 255u) : upto;
     const int l2_ = ok ? (int)((lw >> 16) & 255u) : upto, l3 = ok ? (int)(lw >> 24) : upto;
-    const int wmax = __reduce_max_sync(FULL_MASK, max(max(l0, l1), max(l2_, l3)));
 #pragma unroll 1
     for (int s = 0; s < upto; ++s) {
       h.lr = lr_s[s];
       float q = 0.f;
-      if (OPT == CTR_OPT_ADAM) {   // all 4 rows in one block; rows already past step s are restored by selects
-        const float4 xo = x, ao = a, bo = b;
-        adam_untouched4(x, a, b, h, ac);
-        if (s >= wmax) {
-          q = sq4(xo);
-        } else {
-          if (s >= l0) q += xo.x * xo.x; else { x.x = xo.x; a.x = ao.x; b.x = bo.x; }
-          if (s >= l1) q += xo.y * xo.y; else { x.y = xo.y; a.y = ao.y; b.y = bo.y; }
-          if (s >= l2_) q += xo.z * xo.z; else { x.z = xo.z; a.z = ao.z; b.z = bo.z; }
-          if (s >= l3) q += xo.w * xo.w; else { x.w = xo.w; a.w = ao.w; b.w = bo.w; }
-        }
-      } else {
       if (s >= l0) { q += x.x * x.x; step_sparse<OPT>(x.x, a.x, b.x, __fmul_rn(h.l2, x.x), h); }
       if (s >= l1) { q += x.y * x.y; step_sparse<OPT>(x.y, a.y, b.y, __fmul_rn(h.l2, x.y), h); }
       if (s >= l2_) { q += x.z * x.z; step_sparse<OPT>(x.z, a.z, b.z, __fmul_rn(h.l2, x.z), h); }
       if (s >= l3) { q += x.w * x.w; step_sparse<OPT>(x.w, a.w, b.w, __fmul_rn(h.l2, x.w), h); }
-      }
       ss_thr[s][threadIdx.x] += q;
     }
     if (ok) {
@@ -678,16 +645,15 @@ static int launch_epoch_rows2(int opt, int apply, float* var, float* slot0, floa
   return CTR_OK;
 }
 
-// The [N,K] table and a scalar table [N] gathered with the same ids (fm_v + fm_w), in ONE launch: lane 0 of every row
-// carries the scalar table's element.  Same arithmetic as two ctr_epoch_rows calls.  w_last == last: the tables share
-// one `last` byte per row (ctr_epoch_sweep2).
-static int epoch_rows2_checked(int opt, int apply, float* var, float* slot0, float* slot1, uint8_t* last, float* w_var,
-                               float* w_slot0, float* w_slot1, uint8_t* w_last, const int32_t* uniq,
-                               const int32_t* n_uniq, const float* g_uniq, const float* gw_uniq, int64_t n_max, int K,
-                               const float* hyper, const float* lr_table, int j, double* ss, double* ss_w,
-                               float* stage, float* w_stage, ctr_stream_t stream) {
+// w_last == last: the tables share one `last` byte per row (ctr_epoch_sweep with a scalar table).  stage / w_stage:
+// both NULL, or both given (the staged hand-over of the catch-up and the apply of one step, epoch_rows_kernel STAGED).
+int ctr_epoch_rows2(int opt, int apply, float* var, float* slot0, float* slot1, uint8_t* last, float* w_var, float* w_slot0,
+                    float* w_slot1, uint8_t* w_last, const int32_t* uniq, const int32_t* n_uniq, const float* g_uniq,
+                    const float* gw_uniq, int64_t n_max, int K, const float* hyper, const float* lr_table, int j, double* ss,
+                    double* ss_w, float* stage, float* w_stage, ctr_stream_t stream) {
   CTR_REQUIRE(n_max >= 0 && j >= 0 && j < EPOCH_MAX, CTR_ERR_INVALID_ARG, "ctr_epoch_rows2: bad n_max/j");
   CTR_REQUIRE(epoch_rows2_supported(K), CTR_ERR_UNSUPPORTED, "ctr_epoch_rows2: K=%d (supported: 4..256 powers of two)", K);
+  CTR_REQUIRE(!stage == !w_stage, CTR_ERR_INVALID_ARG, "ctr_epoch_rows2: stage and w_stage must both be given or both NULL");
   if (n_max == 0) return CTR_OK;
   CTR_REQUIRE(var && slot0 && last && w_var && w_slot0 && w_last && uniq && n_uniq && hyper && lr_table && ss && ss_w,
               CTR_ERR_INVALID_ARG, "ctr_epoch_rows2: null buffer");
@@ -700,97 +666,36 @@ static int epoch_rows2_checked(int opt, int apply, float* var, float* slot0, flo
                             ss, -1, as_stream(stream));
 }
 
-// The [N,K] table and a scalar table [N] gathered with the same ids (fm_v + fm_w), in ONE launch: lane 0 of every row
-// carries the scalar table's element.  Same arithmetic as two ctr_epoch_rows calls.  w_last == last: the tables share
-// one `last` byte per row (ctr_epoch_sweep2).
-int ctr_epoch_rows2(int opt, int apply, float* var, float* slot0, float* slot1, uint8_t* last, float* w_var, float* w_slot0,
-                    float* w_slot1, uint8_t* w_last, const int32_t* uniq, const int32_t* n_uniq, const float* g_uniq,
-                    const float* gw_uniq, int64_t n_max, int K, const float* hyper, const float* lr_table, int j, double* ss,
-                    double* ss_w, ctr_stream_t stream) {
-  return epoch_rows2_checked(opt, apply, var, slot0, slot1, last, w_var, w_slot0, w_slot1, w_last, uniq, n_uniq, g_uniq,
-                             gw_uniq, n_max, K, hyper, lr_table, j, ss, ss_w, nullptr, nullptr, stream);
+int ctr_epoch_shared_last_supported(int opt, int64_t n_rows, int K) {
+  return opt == CTR_OPT_ADAM && epoch_rows2_supported(K) && n_rows > 0 && n_rows % 4 == 0;
 }
 
-int ctr_epoch_rows2_staged(int opt, int apply, float* var, float* slot0, float* slot1, uint8_t* last, float* w_var,
-                           float* w_slot0, float* w_slot1, uint8_t* w_last, const int32_t* uniq, const int32_t* n_uniq,
-                           const float* g_uniq, const float* gw_uniq, int64_t n_max, int K, const float* hyper,
-                           const float* lr_table, int j, double* ss, double* ss_w, float* stage, float* w_stage,
-                           ctr_stream_t stream) {
-  CTR_REQUIRE(stage && w_stage, CTR_ERR_INVALID_ARG, "ctr_epoch_rows2_staged: null stage");
-  return epoch_rows2_checked(opt, apply, var, slot0, slot1, last, w_var, w_slot0, w_slot1, w_last, uniq, n_uniq, g_uniq,
-                             gw_uniq, n_max, K, hyper, lr_table, j, ss, ss_w, stage, w_stage, stream);
-}
-
-// CTR_EPOCH_SCALAR=1 (read once per process) routes Adam through the scalar sweep kernels (A/B against the packed one)
-static bool epoch_force_scalar() {
-  static int force = -1;
-  if (force < 0) {
-    const char* f = getenv("CTR_EPOCH_SCALAR");
-    force = f ? atoi(f) : 0;
+// the sweep kernels of Adagrad, Momentum and Ftrl (Adam takes the packed sweep of epoch_adam.cu)
+#define EPOCH_NON_ADAM_SWITCH(opt, CALL)                                 \
+  switch (opt) {                                                         \
+    case CTR_OPT_ADAGRAD: { CALL(CTR_OPT_ADAGRAD) } break;               \
+    case CTR_OPT_MOMENTUM: { CALL(CTR_OPT_MOMENTUM) } break;             \
+    case CTR_OPT_FTRL: { CALL(CTR_OPT_FTRL) } break;                     \
+    default:                                                             \
+      ::ctr::set_error("unknown optimizer %d", opt);                     \
+      return CTR_ERR_INVALID_ARG;                                        \
   }
-  return force != 0;
-}
 
-int ctr_epoch_sweep2_supported(int opt, int64_t n_rows, int K) {
-  return opt == CTR_OPT_ADAM && !epoch_force_scalar() && epoch_rows2_supported(K) && n_rows > 0 && n_rows % 4 == 0;
-}
-
-int ctr_epoch_sweep2(int opt, float* var, float* slot0, float* slot1, float* w_var, float* w_slot0, float* w_slot1,
-                     uint8_t* last, int64_t n_rows, int K, const float* hyper, const float* lr_table, int from, int upto,
-                     int reset, double* ss_partials, double* w_ss_partials, int* n_partials_host, int32_t* list,
-                     int64_t list_cap, int32_t* list_count, double* ss_rows, double* w_ss_rows, int32_t* list_overflow,
-                     ctr_stream_t stream) {
-  CTR_REQUIRE(n_rows >= 0 && from >= 0 && from <= upto && upto <= EPOCH_MAX, CTR_ERR_INVALID_ARG,
-              "ctr_epoch_sweep2: bad n_rows/from/upto");
-  CTR_REQUIRE(ctr_epoch_sweep2_supported(opt, n_rows, K), CTR_ERR_UNSUPPORTED,
-              "ctr_epoch_sweep2: needs Adam, K in {4..256} powers of two, n_rows %% 4 == 0 and the packed sweep "
-              "(K=%d, n_rows=%lld)", K, (long long)n_rows);
-  const int n_partials = sm_count() * 6;
-  if (n_partials_host) *n_partials_host = n_partials;
-  if (upto == 0) return CTR_OK;
-  CTR_REQUIRE(var && slot0 && slot1 && w_var && w_slot0 && w_slot1 && last && hyper && lr_table && ss_partials &&
-              w_ss_partials && list && list_count && ss_rows && w_ss_rows && list_cap > 0, CTR_ERR_INVALID_ARG,
-              "ctr_epoch_sweep2: null buffer");
-  CTR_REQUIRE(((uintptr_t)last & 3) == 0, CTR_ERR_INVALID_ARG, "ctr_epoch_sweep2: `last` must be 4-byte aligned");
-  cudaStream_t st = as_stream(stream);
-  if (from == upto) {   // nothing to replay (a flush reached upto already): no step's partials, `last` -> 0 on reset
-    const size_t bytes = (size_t)upto * n_partials * sizeof(double);
-    CTR_REQUIRE(cudaMemsetAsync(ss_partials, 0, bytes, st) == cudaSuccess &&
-                cudaMemsetAsync(w_ss_partials, 0, bytes, st) == cudaSuccess, CTR_ERR_CUDA, "ctr_epoch_sweep2: memset failed");
-    if (reset) {
-      epoch_last_kernel<<<sm_count() * 3, 256, 0, st>>>(last, n_rows, upto, reset);
-      CTR_LAUNCHED("ctr_epoch_sweep2(last)");
-    }
-    return CTR_OK;
-  }
-  CTR_REQUIRE(cudaMemsetAsync(list_count, 0, sizeof(int32_t), st) == cudaSuccess, CTR_ERR_CUDA,
-              "ctr_epoch_sweep2: memset failed");
-  const bool ok = launch_epoch_sweep_adam(var, slot0, slot1, last, n_rows, K, hyper, lr_table, from, upto, ss_partials,
-                                          n_partials, list, list_count, list_cap, list_overflow, st, w_var, w_slot0,
-                                          w_slot1, w_ss_partials);
-  CTR_REQUIRE(ok, CTR_ERR_UNSUPPORTED, "ctr_epoch_sweep2: packed path refused K=%d", K);
-  CTR_LAUNCHED("ctr_epoch_sweep2(adam)");
-  // rows gathered since `from`, both tables: catch up from their own `last` to upto; they get their final `last` here
-  RowsW w;
-  w.var = w_var; w.slot0 = w_slot0; w.slot1 = w_slot1; w.last = nullptr; w.g_uniq = nullptr; w.ss = w_ss_rows;
-  const int rc = launch_epoch_rows2(opt, 0, var, slot0, slot1, last, w, list, list_count, nullptr, list_cap, K, hyper,
-                                    lr_table, upto, ss_rows, reset ? 0 : upto, st);
-  if (rc != CTR_OK) return rc;
-  if (!(reset && from == 0)) {   // untouched rows hold `from`: rewrite (an epoch-end sweep leaves their 0 alone)
-    epoch_last_kernel<<<sm_count() * 3, 256, 0, st>>>(last, n_rows, upto, reset);
-    CTR_LAUNCHED("ctr_epoch_sweep2(last)");
-  }
-  return CTR_OK;
-}
-
-int ctr_epoch_sweep_ovf(int opt, float* var, float* slot0, float* slot1, uint8_t* last, int64_t n_rows, int K,
-                        const float* hyper, const float* lr_table, int from, int upto, int reset, double* ss_partials,
-                        int* n_partials_host, int32_t* list, int64_t list_cap, int32_t* list_count, double* ss_rows,
-                        int32_t* list_overflow, ctr_stream_t stream) {
+int ctr_epoch_sweep(int opt, float* var, float* slot0, float* slot1, float* w_var, float* w_slot0, float* w_slot1,
+                    uint8_t* last, int64_t n_rows, int K, const float* hyper, const float* lr_table, int from, int upto,
+                    int reset, double* ss_partials, double* w_ss_partials, int* n_partials_host, int32_t* list,
+                    int64_t list_cap, int32_t* list_count, double* ss_rows, double* w_ss_rows, int32_t* list_overflow,
+                    ctr_stream_t stream) {
   CTR_REQUIRE(n_rows >= 0 && K > 0 && from >= 0 && from <= upto && upto <= EPOCH_MAX, CTR_ERR_INVALID_ARG,
               "ctr_epoch_sweep: bad n_rows/K/from/upto");
-  // CTR_EPOCH_SCALAR=1 routes Adam through the scalar kernels below (A/B against the packed sweep)
-  const bool force_scalar = epoch_force_scalar();
+  // the scalar table that shares `last` (fm_w next to fm_v): all of its buffers or none
+  const bool with_w = w_var != nullptr;
+  CTR_REQUIRE(with_w ? (w_slot0 && w_slot1 && w_ss_partials && w_ss_rows)
+                     : !(w_slot0 || w_slot1 || w_ss_partials || w_ss_rows),
+              CTR_ERR_INVALID_ARG, "ctr_epoch_sweep: w_var, w_slot0, w_slot1, w_ss_partials, w_ss_rows: all or none");
+  CTR_REQUIRE(!with_w || ctr_epoch_shared_last_supported(opt, n_rows, K), CTR_ERR_UNSUPPORTED,
+              "ctr_epoch_sweep: a shared `last` needs Adam, K in {4..256} powers of two and n_rows %% 4 == 0 "
+              "(K=%d, n_rows=%lld)", K, (long long)n_rows);
   const int grid = sm_count() * 3;
   const int n_partials = sm_count() * 6;     // row length of ss_partials (>= every grid used here)
   if (n_partials_host) *n_partials_host = n_partials;
@@ -798,67 +703,85 @@ int ctr_epoch_sweep_ovf(int opt, float* var, float* slot0, float* slot1, uint8_t
   CTR_REQUIRE(var && slot0 && last && hyper && lr_table && ss_partials, CTR_ERR_INVALID_ARG,
               "ctr_epoch_sweep: null buffer");
   CTR_REQUIRE(n_slots_of(opt) == 1 || slot1, CTR_ERR_INVALID_ARG, "ctr_epoch_sweep: slot1 required");
+  const bool last_aligned = ((uintptr_t)last & 3) == 0;
+  CTR_REQUIRE(!with_w || last_aligned, CTR_ERR_INVALID_ARG, "ctr_epoch_sweep: a shared `last` must be 4-byte aligned");
   cudaStream_t st = as_stream(stream);
   const int64_t n_elem = n_rows * K;
   const int f4 = K / 4;
   const bool row_in_warp = K % 4 == 0 && (f4 & (f4 - 1)) == 0 && f4 <= 32;
+  const bool k1_packed = K == 1 && n_rows % 4 == 0 && last_aligned;   // a float4 holds 4 rows, a uint32 their `last`
 
-  // ---- Adam on the packed pipe (epoch_adam.cu): untouched rows here, gathered rows through `list` ----------
-  if (opt == CTR_OPT_ADAM && !force_scalar && list && list_count && ss_rows && list_cap > 0 && from < upto &&
-      epoch_rows_supported(K) && (K % 4 == 0 || (K == 1 && n_rows % 4 == 0 && ((uintptr_t)last & 3) == 0))) {
-    CTR_REQUIRE(cudaMemsetAsync(list_count, 0, sizeof(int32_t), st) == cudaSuccess, CTR_ERR_CUDA,
-                "ctr_epoch_sweep: memset failed");
-    const bool ok = launch_epoch_sweep_adam(var, slot0, slot1, last, n_rows, K, hyper, lr_table, from, upto,
-                                            ss_partials, n_partials, list, list_count, list_cap, list_overflow, st);
-    CTR_REQUIRE(ok, CTR_ERR_UNSUPPORTED, "ctr_epoch_sweep: packed path refused K=%d", K);
-    CTR_LAUNCHED("ctr_epoch_sweep(adam)");
-    // rows gathered since `from`: catch up from their own `last` to upto; they get their final `last` here
-    const int rc = launch_epoch_rows(opt, 0, var, slot0, slot1, last, list, list_count, nullptr, list_cap, K, hyper,
-                                     lr_table, upto, ss_rows, reset ? 0 : upto, st);
-    if (rc != CTR_OK) return rc;
-    if (!(reset && from == 0)) {   // untouched rows hold `from`: rewrite (an epoch-end sweep leaves their 0 alone)
-      epoch_last_kernel<<<grid, 256, 0, st>>>(last, n_rows, upto, reset);
-      CTR_LAUNCHED("ctr_epoch_sweep(last)");
+  if (opt == CTR_OPT_ADAM) {
+    CTR_REQUIRE(list && list_count && ss_rows && list_cap > 0, CTR_ERR_INVALID_ARG,
+                "ctr_epoch_sweep: Adam needs list, list_count, ss_rows and list_cap > 0");
+    if ((K % 4 == 0 && epoch_rows_supported(K)) || k1_packed) {
+      // ---- the packed pipe (epoch_adam.cu): untouched rows here, gathered rows through `list` ----------------
+      if (from == upto) {   // nothing to replay (a flush reached upto already): no step's partials, `last` -> 0 on reset
+        const size_t bytes = (size_t)upto * n_partials * sizeof(double);
+        CTR_REQUIRE(cudaMemsetAsync(ss_partials, 0, bytes, st) == cudaSuccess &&
+                    (!with_w || cudaMemsetAsync(w_ss_partials, 0, bytes, st) == cudaSuccess), CTR_ERR_CUDA,
+                    "ctr_epoch_sweep: memset failed");
+        if (reset) {
+          epoch_last_kernel<<<grid, 256, 0, st>>>(last, n_rows, upto, reset);
+          CTR_LAUNCHED("ctr_epoch_sweep(last)");
+        }
+        return CTR_OK;
+      }
+      CTR_REQUIRE(cudaMemsetAsync(list_count, 0, sizeof(int32_t), st) == cudaSuccess, CTR_ERR_CUDA,
+                  "ctr_epoch_sweep: memset failed");
+      const bool ok = launch_epoch_sweep_adam(var, slot0, slot1, last, n_rows, K, hyper, lr_table, from, upto,
+                                              ss_partials, n_partials, list, list_count, list_cap, list_overflow, st,
+                                              w_var, w_slot0, w_slot1, w_ss_partials);
+      CTR_REQUIRE(ok, CTR_ERR_UNSUPPORTED, "ctr_epoch_sweep: packed path refused K=%d", K);
+      CTR_LAUNCHED("ctr_epoch_sweep(adam)");
+      // rows gathered since `from` (both tables): catch up from their own `last` to upto; they get their final `last` here
+      int rc;
+      if (with_w) {
+        RowsW w;
+        w.var = w_var; w.slot0 = w_slot0; w.slot1 = w_slot1; w.last = nullptr; w.g_uniq = nullptr; w.ss = w_ss_rows;
+        rc = launch_epoch_rows2(opt, 0, var, slot0, slot1, last, w, list, list_count, nullptr, list_cap, K, hyper,
+                                lr_table, upto, ss_rows, reset ? 0 : upto, st);
+      } else {
+        rc = launch_epoch_rows(opt, 0, var, slot0, slot1, last, list, list_count, nullptr, list_cap, K, hyper, lr_table,
+                               upto, ss_rows, reset ? 0 : upto, st);
+      }
+      if (rc != CTR_OK) return rc;
+      if (!(reset && from == 0)) {   // untouched rows hold `from`: rewrite (an epoch-end sweep leaves their 0 alone)
+        epoch_last_kernel<<<grid, 256, 0, st>>>(last, n_rows, upto, reset);
+        CTR_LAUNCHED("ctr_epoch_sweep(last)");
+      }
+      return CTR_OK;
     }
-    return CTR_OK;
-  }
-
-  if (row_in_warp) {   // a row's float4s sit in one warp: `last` can be rewritten in place
+  } else if (row_in_warp) {   // a row's float4s sit in one warp: `last` can be rewritten in place
 #define ES_CALL(OPT)                                                                           \
   epoch_sweep_kernel<OPT><<<grid, 256, 0, st>>>(var, slot0, slot1, last, n_elem / 4, K, hyper, \
                                                 lr_table, upto, reset, ss_partials, n_partials);
-    CTR_OPT_SWITCH(opt, ES_CALL)
+    EPOCH_NON_ADAM_SWITCH(opt, ES_CALL)
 #undef ES_CALL
     CTR_LAUNCHED("ctr_epoch_sweep");
-  } else if (K == 1 && n_rows % 4 == 0 && ((uintptr_t)last & 3) == 0) {
+    return CTR_OK;
+  } else if (k1_packed) {
 #define ES1_CALL(OPT)                                                                                \
   epoch_sweep_k1_kernel<OPT><<<grid, 256, 0, st>>>(var, slot0, slot1, last, n_rows / 4, hyper, lr_table, \
                                                    upto, reset, ss_partials, n_partials);
-    CTR_OPT_SWITCH(opt, ES1_CALL)
+    EPOCH_NON_ADAM_SWITCH(opt, ES1_CALL)
 #undef ES1_CALL
     CTR_LAUNCHED("ctr_epoch_sweep(k1)");
-  } else {
-    // rows that span warps / CTAs (K/4 not a power of two <= 32) or K % 4 != 0: one thread per element, `last`
-    // rewritten by a separate pass once every element of the row has read it
+    return CTR_OK;
+  }
+  // rows that span warps / CTAs (K/4 not a power of two <= 32, Adam: K > 256) or K % 4 != 0: one thread per element,
+  // `last` rewritten by a separate pass once every element of the row has read it
 #define ESG_CALL(OPT)                                                                                \
   epoch_sweep_generic_kernel<OPT><<<grid, 256, 0, st>>>(var, slot0, slot1, last, n_elem, K, hyper,   \
                                                         lr_table, upto, reset, ss_partials, n_partials);
-    CTR_OPT_SWITCH(opt, ESG_CALL)
+  CTR_OPT_SWITCH(opt, ESG_CALL)
 #undef ESG_CALL
-    CTR_LAUNCHED("ctr_epoch_sweep(generic)");
-    epoch_last_kernel<<<grid, 256, 0, st>>>(last, n_rows, upto, reset);
-    CTR_LAUNCHED("ctr_epoch_sweep(last)");
-  }
+  CTR_LAUNCHED("ctr_epoch_sweep(generic)");
+  epoch_last_kernel<<<grid, 256, 0, st>>>(last, n_rows, upto, reset);
+  CTR_LAUNCHED("ctr_epoch_sweep(last)");
   return CTR_OK;
 }
-
-int ctr_epoch_sweep(int opt, float* var, float* slot0, float* slot1, uint8_t* last, int64_t n_rows, int K,
-                    const float* hyper, const float* lr_table, int from, int upto, int reset, double* ss_partials,
-                    int* n_partials_host, int32_t* list, int64_t list_cap, int32_t* list_count, double* ss_rows,
-                    ctr_stream_t stream) {
-  return ctr_epoch_sweep_ovf(opt, var, slot0, slot1, last, n_rows, K, hyper, lr_table, from, upto, reset, ss_partials,
-                             n_partials_host, list, list_cap, list_count, ss_rows, nullptr, stream);
-}
+#undef EPOCH_NON_ADAM_SWITCH
 
 int ctr_epoch_reg_loss(double* ss_rows, const double* ss_partials, int n_partials, int upto, float scale,
                        float* reg, int accumulate, ctr_stream_t stream) {

@@ -68,7 +68,7 @@ using namespace ctr;
 
 extern "C" {
 
-int ctr_abi_version(void) { return 1; }
+int ctr_abi_version(void) { return 2; }
 const char* ctr_last_error(void) { return ctr::g_err; }
 int64_t ctr_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 int ctr_device_sm_count(void) { return sm_count(); }

@@ -11,50 +11,6 @@ namespace ctr {
 
 constexpr int MAX_G = 64;
 
-__global__ void __launch_bounds__(256)
-bucket_count_kernel(const int32_t* __restrict__ uniq, const int32_t* __restrict__ n_uniq, int64_t n_max, int G,
-                    int32_t* __restrict__ counts) {
-  __shared__ int32_t sh[MAX_G];
-  if (threadIdx.x < G) sh[threadIdx.x] = 0;
-  __syncthreads();
-  const int64_t n = min((int64_t)n_uniq[0], n_max);
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) atomicAdd(&sh[uniq[i] % G], 1);
-  __syncthreads();
-  if (threadIdx.x < G && sh[threadIdx.x]) atomicAdd(&counts[threadIdx.x], sh[threadIdx.x]);
-}
-
-// order[pos] = u ; pos_of[u] = pos ; local_ids[pos] = uniq[u] / G, buckets in owner order.
-// (placement inside a bucket follows atomic arrival order: any order is valid as long as the same
-// `order` is used for the id exchange and, later, for the gradient exchange.)
-__global__ void __launch_bounds__(256)
-bucket_place_kernel(const int32_t* __restrict__ uniq, const int32_t* __restrict__ n_uniq, int64_t n_max, int G,
-                    const int32_t* __restrict__ counts, int32_t* __restrict__ cursor, int32_t* __restrict__ order,
-                    int32_t* __restrict__ pos_of, int32_t* __restrict__ local_ids) {
-  __shared__ int32_t off[MAX_G];
-  if (threadIdx.x == 0) {
-    int32_t run = 0;
-    for (int g = 0; g < G; ++g) { off[g] = run; run += counts[g]; }
-  }
-  __syncthreads();
-  const int64_t n = min((int64_t)n_uniq[0], n_max);
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; u < n; u += stride) {
-    const int32_t id = uniq[u];
-    const int o = id % G;
-    const int32_t pos = off[o] + atomicAdd(&cursor[o], 1);
-    order[pos] = (int32_t)u;
-    pos_of[u] = pos;
-    local_ids[pos] = id / G;
-  }
-}
-
-__global__ void remap_ids_kernel(const int32_t* __restrict__ inverse, const int32_t* __restrict__ pos_of, int64_t n,
-                                 int32_t* __restrict__ out) {
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = pos_of[inverse[i]];
-}
-
 __global__ void gather_scalar_kernel(const int32_t* __restrict__ ids, const float* __restrict__ W, int64_t N,
                                      int64_t n, float* __restrict__ out) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
@@ -112,25 +68,6 @@ using namespace ctr;
 
 extern "C" {
 
-int ctr_a2a_bucket_ids(const int32_t* uniq, const int32_t* n_uniq, int64_t n_max, int G, int32_t* counts,
-                       int32_t* cursor, int32_t* order, int32_t* pos_of, int32_t* local_ids, ctr_stream_t stream) {
-  CTR_REQUIRE(n_max >= 0 && G >= 1 && G <= MAX_G, CTR_ERR_INVALID_ARG, "ctr_a2a_bucket_ids: need 1 <= G <= %d", MAX_G);
-  CTR_REQUIRE(uniq && n_uniq && counts && cursor && order && pos_of && local_ids, CTR_ERR_INVALID_ARG,
-              "ctr_a2a_bucket_ids: null buffer");
-  cudaStream_t st = as_stream(stream);
-  if (cudaMemsetAsync(counts, 0, G * sizeof(int32_t), st) != cudaSuccess ||
-      cudaMemsetAsync(cursor, 0, G * sizeof(int32_t), st) != cudaSuccess) {
-    set_error("ctr_a2a_bucket_ids: memset failed");
-    return CTR_ERR_CUDA;
-  }
-  if (n_max == 0) return CTR_OK;
-  bucket_count_kernel<<<lin_grid(n_max), 256, 0, st>>>(uniq, n_uniq, n_max, G, counts);
-  CTR_LAUNCHED("a2a_bucket_count");
-  bucket_place_kernel<<<lin_grid(n_max), 256, 0, st>>>(uniq, n_uniq, n_max, G, counts, cursor, order, pos_of, local_ids);
-  CTR_LAUNCHED("a2a_bucket_place");
-  return CTR_OK;
-}
-
 int ctr_shard_keys(const int32_t* ids, int64_t n, int64_t N, int G, int32_t* keys, int32_t* oob, ctr_stream_t stream) {
   CTR_REQUIRE(n >= 0 && N > 0 && G >= 1 && G <= MAX_G, CTR_ERR_INVALID_ARG, "ctr_shard_keys: bad n/N/G");
   const int64_t npad = (N + G - 1) / G;
@@ -151,15 +88,6 @@ int ctr_shard_split(const int32_t* uniq_keys, const int32_t* n_uniq, int64_t n_m
   if (n_max == 0) return CTR_OK;
   shard_split_kernel<<<lin_grid(n_max), 256, 0, st>>>(uniq_keys, n_uniq, n_max, (int32_t)((N + G - 1) / G), G, counts, local_ids);
   CTR_LAUNCHED("ctr_shard_split");
-  return CTR_OK;
-}
-
-int ctr_remap_ids(const int32_t* inverse, const int32_t* pos_of, int64_t n, int32_t* out, ctr_stream_t stream) {
-  CTR_REQUIRE(n >= 0, CTR_ERR_INVALID_ARG, "ctr_remap_ids: n < 0");
-  if (n == 0) return CTR_OK;
-  CTR_REQUIRE(inverse && pos_of && out, CTR_ERR_INVALID_ARG, "ctr_remap_ids: null buffer");
-  remap_ids_kernel<<<lin_grid(n), 256, 0, as_stream(stream)>>>(inverse, pos_of, n, out);
-  CTR_LAUNCHED("ctr_remap_ids");
   return CTR_OK;
 }
 

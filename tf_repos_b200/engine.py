@@ -206,7 +206,7 @@ class SparseUpdater:
     def enable_epochs(self, P: int, tables: Sequence[Table]):
         """Allocates the per-row `last` bytes and the per-step sum(var^2) accumulators.  An [N,K] table and the [N]
         table gathered with the same ids always hold the same `last` bytes: where the packed Adam sweep can take both
-        in one pass (ops.epoch_sweep2_supported) they share ONE `last` array and one row list."""
+        in one pass (ops.epoch_shared_last_supported) they share ONE `last` array and one row list."""
         pmax = ops.epoch_max_steps()
         if not 1 <= P <= pmax:
             raise ValueError(f"epoch_steps={P}: must be in [1, {pmax}] (the `last` bytes and lr table hold {pmax} steps)")
@@ -219,7 +219,7 @@ class SparseUpdater:
         self.list_overflow = torch.zeros(1, dtype=torch.int32, device=dev)
         self.shared_last = (len(tables) == 2 and tables[1].K == 1 and tables[0].N == tables[1].N
                             and tables[0].K in ops.EPOCH_ROWS2_K
-                            and ops.epoch_sweep2_supported(self.opt.opt, tables[0].N, tables[0].K))
+                            and ops.epoch_shared_last_supported(self.opt.opt, tables[0].N, tables[0].K))
         for i, t in enumerate(tables):
             # rows gathered since the last sweep, collected by the packed Adam sweep for its second pass: at most
             # n distinct ids per step, P <= pmax steps per epoch (shared: the [N,K] table's list serves both)
@@ -244,10 +244,10 @@ class SparseUpdater:
             (V, gv), (W, gw) = tables_g            # fm_v + fm_w: one launch for both tables
             ev, ew = self.ep[V.name], self.ep[W.name]
             # the catch-up hands the caught-up rows to the apply of the same step through stage_v / stage_w (free in
-            # this mode; see ctr_epoch_rows2_staged)
-            ops.epoch_rows2_staged(o.opt, apply, V, W, ev["last"], ew["last"], uw.uniq, uw.n_uniq,
-                                   gv if apply else None, gw if apply else None, self.n, o.record(HYPER_TABLE),
-                                   o.lr_table, j, ev["ss"], ew["ss"], self.stage_v, self.stage_w)
+            # this mode; see ctr_epoch_rows2)
+            ops.epoch_rows2(o.opt, apply, V, W, ev["last"], ew["last"], uw.uniq, uw.n_uniq, gv if apply else None,
+                            gw if apply else None, self.n, o.record(HYPER_TABLE), o.lr_table, j, ev["ss"], ew["ss"],
+                            self.stage_v, self.stage_w)
             return
         for t, g in tables_g:
             e = self.ep[t.name]
@@ -255,45 +255,28 @@ class SparseUpdater:
                            g if apply else None, self.n, t.K, o.record(HYPER_TABLE), o.lr_table, j, e["ss"])
 
     def epoch_sweep(self, upto: int, reset: bool):
-        """All rows -> state after `upto` steps of this epoch; per-step l2*l2_loss terms -> ep[.]['reg']."""
+        """All rows -> state after `upto` steps of this epoch; per-step l2*l2_loss terms -> ep[.]['reg'].  One pass per
+        table, or one pass for an [N,K] + [N] pair that shares `last` (and its row list)."""
         o = self.opt
-        if self.shared_last:
-            self.epoch_sweep2(upto, reset)
-            return
-        for t in self.tables:
+        passes = [(self.tables[0], self.tables[1])] if self.shared_last else [(t, None) for t in self.tables]
+        for t, w in passes:
             e = self.ep[t.name]
+            ew = self.ep[w.name] if w is not None else dict(partials=None, ss=None)
             ev = None
             if self.sweep_events is not None and t.K > 1:
                 ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
                 ev[0].record()
             ops.epoch_sweep(o.opt, t.var, t.slot(0), t.slot(1), e["last"], t.N, t.K, o.record(HYPER_TABLE),
                             o.lr_table, self.flush_pos, upto, reset, e["partials"], e["list"], e["list_count"],
-                            e["ss"], self.list_overflow)
+                            e["ss"], self.list_overflow, W=w, w_ss_partials=ew["partials"], w_ss_rows=ew["ss"])
             if ev is not None:
                 ev[1].record()
                 self.sweep_events.append(ev)
                 self.sweep_steps.append(upto - self.flush_pos)   # optimizer steps this pass replayed per element
             # accumulate: a mid-epoch flush and the epoch-end sweep each contribute their share
-            ops.epoch_reg_loss(e["ss"], e["partials"], self.n_epart, upto, 0.5 * self.l2_reg, e["reg"], accumulate=True)
-        self.flush_pos = 0 if reset else upto
-
-    def epoch_sweep2(self, upto: int, reset: bool):
-        """epoch_sweep for an [N,K] + [N] pair that shares `last`: one pass and one row list for both tables."""
-        o = self.opt
-        (V, W), (ev, ew) = self.tables, (self.ep[self.tables[0].name], self.ep[self.tables[1].name])
-        rec = None
-        if self.sweep_events is not None:
-            rec = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
-            rec[0].record()
-        ops.epoch_sweep2(o.opt, V, W, ev["last"], o.record(HYPER_TABLE), o.lr_table, self.flush_pos, upto, reset,
-                         ev["partials"], ew["partials"], ev["list"], ev["list_count"], ev["ss"], ew["ss"],
-                         self.list_overflow)
-        if rec is not None:
-            rec[1].record()
-            self.sweep_events.append(rec)
-            self.sweep_steps.append(upto - self.flush_pos)
-        for e in (ev, ew):
-            ops.epoch_reg_loss(e["ss"], e["partials"], self.n_epart, upto, 0.5 * self.l2_reg, e["reg"], accumulate=True)
+            for x in (self.ep[u.name] for u in (t, w) if u is not None):
+                ops.epoch_reg_loss(x["ss"], x["partials"], self.n_epart, upto, 0.5 * self.l2_reg, x["reg"],
+                                   accumulate=True)
         self.flush_pos = 0 if reset else upto
 
     def check_list_overflow(self):

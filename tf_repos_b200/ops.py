@@ -385,11 +385,6 @@ def colsum_rows(part, out):
           "ctr_colsum_rows")
 
 
-def group_sum(dZ, B, P, N, dU):
-    check(_L.ctr_group_sum(_p(dZ, torch.float32, "dZ"), B, P, N, _p(dU, torch.float32, "dU"), _stream()),
-          "ctr_group_sum")
-
-
 def axpby(a, alpha, b, beta, out):
     check(_L.ctr_axpby(_p(a, torch.float32, "a"), float(alpha), _p(b, torch.float32, "b"), float(beta), a.numel(),
                        _p(out, torch.float32, "out"), _stream()), "ctr_axpby")
@@ -451,17 +446,6 @@ def dropout_apply(x, mask, keep, out):
                                _p(out, torch.float32, "out"), _stream()), "ctr_dropout_apply")
 
 
-def a2a_bucket_ids(uniq, n_uniq, n_max, G, counts, cursor, order, pos_of, local_ids):
-    check(_L.ctr_a2a_bucket_ids(_p(uniq, torch.int32), _p(n_uniq, torch.int32), n_max, G, _p(counts, torch.int32),
-                                _p(cursor, torch.int32), _p(order, torch.int32), _p(pos_of, torch.int32),
-                                _p(local_ids, torch.int32), _stream()), "ctr_a2a_bucket_ids")
-
-
-def remap_ids(inverse, pos_of, n, out):
-    check(_L.ctr_remap_ids(_p(inverse, torch.int32), _p(pos_of, torch.int32), n, _p(out, torch.int32), _stream()),
-          "ctr_remap_ids")
-
-
 def shard_keys(ids, N: int, G: int, keys, oob=None):
     check(_L.ctr_shard_keys(_p(ids, torch.int32, "ids"), ids.numel(), N, G, _p(keys, torch.int32, "keys"),
                             _p(oob, torch.int32, "oob"), _stream()), "ctr_shard_keys")
@@ -499,8 +483,10 @@ def epoch_rows(opt, apply: bool, var, slot0, slot1, last, uniq, n_uniq, g_uniq, 
         "ctr_epoch_rows")
 
 
-def epoch_rows2(opt, apply: bool, V, W, last_v, last_w, uniq, n_uniq, g_uniq, gw_uniq, n_max, hyper, lr_table, j, ss_v, ss_w):
-    """V / W: engine.Table ([N,K] and [N]) gathered with the same ids; one launch for both."""
+def epoch_rows2(opt, apply: bool, V, W, last_v, last_w, uniq, n_uniq, g_uniq, gw_uniq, n_max, hyper, lr_table, j, ss_v, ss_w,
+                stage_v=None, stage_w=None):
+    """V / W: engine.Table ([N,K] and [N]) gathered with the same ids; one launch for both.  stage_v [n_max*3K] /
+    stage_w [n_max*3] (both or neither): the catch-up and the apply of one step hand the rows over through them."""
     f = torch.float32
     check(
         _L.ctr_epoch_rows2(
@@ -508,24 +494,9 @@ def epoch_rows2(opt, apply: bool, V, W, last_v, last_w, uniq, n_uniq, g_uniq, gw
             _p(W.var, f, "w_var"), _p(W.slot(0), f), _p(W.slot(1), f), _p(last_w, torch.uint8, "w_last"),
             _p(uniq, torch.int32, "uniq"), _p(n_uniq, torch.int32, "n_uniq"), _p(g_uniq, f, "g_uniq"),
             _p(gw_uniq, f, "gw_uniq"), n_max, V.K, _p(hyper, f, "hyper"), _p(lr_table, f, "lr_table"), j,
-            _p(ss_v, torch.float64, "ss"), _p(ss_w, torch.float64, "ss_w"), _stream()),
-        "ctr_epoch_rows2")
-
-
-def epoch_rows2_staged(opt, apply: bool, V, W, last_v, last_w, uniq, n_uniq, g_uniq, gw_uniq, n_max, hyper, lr_table, j,
-                       ss_v, ss_w, stage_v, stage_w):
-    """epoch_rows2 whose catch-up and apply of one step hand the rows over through stage_v [n_max*3K] / stage_w
-    [n_max*3] (ctr_epoch_rows2_staged)."""
-    f = torch.float32
-    check(
-        _L.ctr_epoch_rows2_staged(
-            opt, int(apply), _p(V.var, f, "var"), _p(V.slot(0), f), _p(V.slot(1), f), _p(last_v, torch.uint8, "last"),
-            _p(W.var, f, "w_var"), _p(W.slot(0), f), _p(W.slot(1), f), _p(last_w, torch.uint8, "w_last"),
-            _p(uniq, torch.int32, "uniq"), _p(n_uniq, torch.int32, "n_uniq"), _p(g_uniq, f, "g_uniq"),
-            _p(gw_uniq, f, "gw_uniq"), n_max, V.K, _p(hyper, f, "hyper"), _p(lr_table, f, "lr_table"), j,
             _p(ss_v, torch.float64, "ss"), _p(ss_w, torch.float64, "ss_w"), _p(stage_v, f, "stage"),
             _p(stage_w, f, "w_stage"), _stream()),
-        "ctr_epoch_rows2_staged")
+        "ctr_epoch_rows2")
 
 
 EPOCH_ROWS2_K = (4, 8, 16, 32, 64, 128, 256)
@@ -536,44 +507,31 @@ def epoch_partials_count() -> int:
 
 
 def epoch_sweep(opt, var, slot0, slot1, last, n_rows, K, hyper, lr_table, from_: int, upto: int, reset: bool,
-                ss_partials, list_buf=None, list_count=None, ss_rows=None, list_overflow=None):
-    """list_buf / list_count / ss_rows: scratch of the packed-pipe Adam sweep (None: scalar kernels).
-    list_overflow: int32 [1] counter; gathered rows that did not fit in list_buf are added to it (see check_ids)."""
-    n_part = ctypes.c_int(0)
-    check(
-        _L.ctr_epoch_sweep_ovf(
-            opt, _p(var, torch.float32, "var"), _p(slot0, torch.float32, "slot0"),
-            _p(slot1, torch.float32, "slot1"), _p(last, torch.uint8, "last"), n_rows, K,
-            _p(hyper, torch.float32, "hyper"), _p(lr_table, torch.float32, "lr_table"), from_, upto, int(reset),
-            _p(ss_partials, torch.float64, "ss_partials"), ctypes.byref(n_part),
-            _p(list_buf, torch.int32, "list"), (list_buf.numel() if list_buf is not None else 0),
-            _p(list_count, torch.int32, "list_count"), _p(ss_rows, torch.float64, "ss_rows"),
-            _p(list_overflow, torch.int32, "list_overflow"), _stream()),
-        "ctr_epoch_sweep_ovf")
-    return n_part.value
-
-
-def epoch_sweep2_supported(opt, n_rows: int, K: int) -> bool:
-    """Whether an [n_rows, K] table and a scalar [n_rows] table can share one `last` array (ctr_epoch_sweep2)."""
-    return bool(_L.ctr_epoch_sweep2_supported(opt, n_rows, K))
-
-
-def epoch_sweep2(opt, V, W, last, hyper, lr_table, from_: int, upto: int, reset: bool, ss_partials, w_ss_partials,
-                 list_buf, list_count, ss_rows, w_ss_rows, list_overflow=None):
-    """ctr_epoch_sweep2: V [N,K] and W [N] (engine.Table) sharing `last`, one pass and one row list for both."""
+                ss_partials, list_buf=None, list_count=None, ss_rows=None, list_overflow=None, W=None,
+                w_ss_partials=None, w_ss_rows=None):
+    """list_buf / list_count / ss_rows: scratch of the Adam sweep (required for Adam).
+    list_overflow: int32 [1] counter; gathered rows that did not fit in list_buf are added to it (see check_ids).
+    W: the scalar table [n_rows] (engine.Table) that shares `last` (epoch_shared_last_supported), swept in the same
+    pass with its own w_ss_partials / w_ss_rows."""
     f = torch.float32
+    w_var, w_slot0, w_slot1 = (W.var, W.slot(0), W.slot(1)) if W is not None else (None, None, None)
     n_part = ctypes.c_int(0)
     check(
-        _L.ctr_epoch_sweep2(
-            opt, _p(V.var, f, "var"), _p(V.slot(0), f, "slot0"), _p(V.slot(1), f, "slot1"), _p(W.var, f, "w_var"),
-            _p(W.slot(0), f, "w_slot0"), _p(W.slot(1), f, "w_slot1"), _p(last, torch.uint8, "last"), V.N, V.K,
+        _L.ctr_epoch_sweep(
+            opt, _p(var, f, "var"), _p(slot0, f, "slot0"), _p(slot1, f, "slot1"), _p(w_var, f, "w_var"),
+            _p(w_slot0, f, "w_slot0"), _p(w_slot1, f, "w_slot1"), _p(last, torch.uint8, "last"), n_rows, K,
             _p(hyper, f, "hyper"), _p(lr_table, f, "lr_table"), from_, upto, int(reset),
             _p(ss_partials, torch.float64, "ss_partials"), _p(w_ss_partials, torch.float64, "w_ss_partials"),
-            ctypes.byref(n_part), _p(list_buf, torch.int32, "list"), list_buf.numel(),
+            ctypes.byref(n_part), _p(list_buf, torch.int32, "list"), (list_buf.numel() if list_buf is not None else 0),
             _p(list_count, torch.int32, "list_count"), _p(ss_rows, torch.float64, "ss_rows"),
             _p(w_ss_rows, torch.float64, "w_ss_rows"), _p(list_overflow, torch.int32, "list_overflow"), _stream()),
-        "ctr_epoch_sweep2")
+        "ctr_epoch_sweep")
     return n_part.value
+
+
+def epoch_shared_last_supported(opt, n_rows: int, K: int) -> bool:
+    """Whether an [n_rows, K] table and a scalar [n_rows] table can share one `last` array (ctr_epoch_sweep)."""
+    return bool(_L.ctr_epoch_shared_last_supported(opt, n_rows, K))
 
 
 def epoch_reg_loss(ss_rows, ss_partials, n_partials, upto, scale, reg, accumulate=False):

@@ -47,8 +47,8 @@ class TimedLib:
                 key = f"{name}[apply={a[1]},K={a[10]}]"
             elif name == "ctr_epoch_rows2":
                 key = f"{name}[apply={a[1]}]"
-            elif name in ("ctr_epoch_sweep_ovf", "ctr_epoch_sweep"):   # (opt, var, s0, s1, last, n_rows, K, ...)
-                key = f"ctr_epoch_sweep[K={a[6]}]"
+            elif name == "ctr_epoch_sweep":   # (opt, var, s0, s1, w_var, w_s0, w_s1, last, n_rows, K, ...)
+                key = f"{name}[K={a[9]}{'+W' if a[4] else ''}]"
             self.records.append((key, e0, e1))
             return r
         return call

@@ -1,10 +1,9 @@
 #!/usr/bin/env python
 """Times ctr_epoch_sweep (Adam, config-2 fm_v: 2e8 x 16, 16 steps per pass) on table states from different phases of a
-run, packed-pipe sweep (csrc/epoch_adam.cu) vs the scalar kernels (CTR_EPOCH_SCALAR=1).
+run.
 
-  python tools/time_sweep.py [fresh early parked verylong] [--scalar] [--n 200000000] [--k 16]
+  python tools/time_sweep.py [fresh early parked verylong] [--n 200000000] [--k 16]
 """
-import json
 import os
 import subprocess
 import sys
@@ -49,15 +48,12 @@ def sweep():
 if state == "early":
     for _ in range(6): sweep()     # ~100 steps in
 ts = sorted(sweep() for _ in range(4))
-print(json.dumps({"state": state, "scalar": %(scalar)d, "N": N, "K": K, "ms_median": ts[len(ts) // 2], "ms_best": ts[0],
+print(json.dumps({"state": state, "N": N, "K": K, "ms_median": ts[len(ts) // 2], "ms_best": ts[0],
                   "listed_rows": int(cnt.item()), "GBps": N * K * 24 / ts[0] / 1e6}))
 '''
 args = [a for a in sys.argv[1:] if not a.startswith("--")]
-scalar = "--scalar" in sys.argv
 n = int(sys.argv[sys.argv.index("--n") + 1]) if "--n" in sys.argv else 200_000_000
 k = int(sys.argv[sys.argv.index("--k") + 1]) if "--k" in sys.argv else 16
 args = [a for a in args if not a.isdigit()]
 for state in args or ["fresh", "early", "parked", "verylong"]:
-    for sc in ([0, 1] if scalar else [0]):
-        env = dict(os.environ, CTR_EPOCH_SCALAR=str(sc))
-        subprocess.run([sys.executable, "-c", CHILD % dict(root=ROOT, n=n, k=k, state=state, scalar=sc)], env=env, check=False)
+    subprocess.run([sys.executable, "-c", CHILD % dict(root=ROOT, n=n, k=k, state=state)], check=False)
