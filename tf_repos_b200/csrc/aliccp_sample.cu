@@ -3,10 +3,12 @@
 // get_stat_mapper.py, get_stat_reducer.py, get_remap_mapper.py; DESIGN.md §2.7).
 //
 // A raw line is `md5,feat_num,feat_list` (a common record) or `sample_id,y,z,md5,feat_num,feat_list` (a sample);
-// feat_list is `field\x02fid\x03val` tokens joined by \x01.  One warp per line (line starts from line_starts.cuh):
+// feat_list is `field\x02fid\x03val` tokens joined by \x01.  One warp per line (line starts and the warp splitting from
+// line_starts.cuh):
 //   classify  strip, the commas by ballot, the y=0/z=1 filter, the \x01 tokens from a ballot of separators (each token
 //             then split and checked by the lane that ends it), the restrictions; kept lines insert their md5 into the
-//             md5 table (lock-free, CAS on each word) and, for train samples, every (field, fid) into the count table.
+//             md5 table (lock-free, CAS on each word; key_table.cuh) and, for train samples, every (field, fid) into
+//             the count table.
 //             Three one-CTA scans give each common record its arena offset and id, each sample its ordinal.
 //   place     common records are copied into the resident arena (the md5's record is the largest id: last wins);
 //             samples keep (md5 slot, shuffle key).
@@ -18,16 +20,16 @@
 //   emit      per sample line: its exact output size (plan) or its bytes at its offset (write), the offsets coming
 //             from a stable sort of (part, r_i) over the samples in line order and an exclusive scan of the sizes.
 // Every order comes from a sort or a scan and every reduction is an integer one: two runs give the same bytes.
+#include "decimal.cuh"
+#include "key_table.cuh"
 #include "line_starts.cuh"
 
 namespace ctr {
 
 constexpr int AS_THREADS = 256, AS_WARPS = AS_THREADS / 32;
 constexpr int AS_MAX_FIELD = 16, AS_MAX_MD5 = 64, AS_MD5_WORDS = 8;
-constexpr int64_t AS_MAX_PROBE = 1 << 15;   // a key that finds no slot within this many probes overflows the table
 constexpr int64_t AS_FIRST_ID = 20;
 constexpr size_t AS_MAX_LEN = (size_t)1 << 30;
-constexpr int64_t AS_MAX_CAP = (int64_t)1 << 31;
 
 enum { AS_SKIP = 0, AS_COMMON = 1, AS_SAMPLE = 2, AS_FILTERED = 3 };
 // info of ctr_aliccp_sample_classify
@@ -42,16 +44,8 @@ __device__ __forceinline__ uint32_t as_shuffle_key(uint64_t seed, uint64_t i) {
 }
 
 // ---- tables ----------------------------------------------------------------------------------------------------
-// Lock-free open addressing: each key word is set once (CAS 0 -> value) and is final once non-zero, and every key word
-// is non-zero, so every thread inserting one key takes the same decision at every slot and all end in the same slot.
-__device__ __forceinline__ bool as_claim(uint64_t* p, uint64_t v) {
-  uint64_t k = *reinterpret_cast<volatile uint64_t*>(p);
-  if (k == 0) {
-    k = atomicCAS(reinterpret_cast<unsigned long long*>(p), 0ull, (unsigned long long)v);
-    if (k == 0) k = v;
-  }
-  return k == v;
-}
+// Lock-free open addressing (key_table.cuh): a slot belongs to the key whose words it holds, each word claimed in
+// order; every key word is non-zero.
 
 // count table: k0 = fid + 1, k1 / k2 = field bytes 0..7 / 8..15 big-endian zero-padded (k2 = 1 for fields of at most
 // 8 bytes: a longer field's byte 8 is above 3), cnt; uint64[4][cap]
@@ -83,16 +77,12 @@ __device__ __forceinline__ void as_pack_field(const uint8_t* t, int64_t s, int64
 }
 
 __device__ bool as_cnt_add(const AsCnt& T, uint64_t k0, uint64_t k1, uint64_t k2, uint64_t add) {
-  uint64_t s = __umul64hi(splitmix64_finalize(k0 ^ splitmix64_finalize(k1 ^ splitmix64_finalize(k2))), (uint64_t)T.cap);
-  const int64_t probes = T.cap < AS_MAX_PROBE ? T.cap : AS_MAX_PROBE;
-  for (int64_t i = 0; i < probes; ++i) {
-    if (as_claim(T.k0 + s, k0) && as_claim(T.k1 + s, k1) && as_claim(T.k2 + s, k2)) {
-      atomicAdd(reinterpret_cast<unsigned long long*>(T.cnt + s), (unsigned long long)add);
-      return true;
-    }
-    if (++s == (uint64_t)T.cap) s = 0;
-  }
-  return false;
+  const uint64_t h = splitmix64_finalize(k0 ^ splitmix64_finalize(k1 ^ splitmix64_finalize(k2)));
+  const int64_t slot = probe(h, T.cap, [&](uint64_t s) {
+    return claim(T.k0 + s, k0) == k0 && claim(T.k1 + s, k1) == k1 && claim(T.k2 + s, k2) == k2;
+  });
+  if (slot >= 0) atomicAdd(reinterpret_cast<unsigned long long*>(T.cnt + slot), (unsigned long long)add);
+  return slot >= 0;
 }
 
 // slot of the md5 [s, e) (1..64 bytes, no NUL), inserted when missing; -1 = the table is full.  One lane.
@@ -103,64 +93,25 @@ __device__ int64_t as_md5_insert(const AsMd5& M, const uint8_t* t, int64_t s, in
   for (int i = 0; i < n; ++i) w[i >> 3] |= (uint64_t)byte_at(t, s + i) << (8 * (i & 7));
   uint64_t h = splitmix64_finalize((uint64_t)n);
   for (int j = 0; j < nw; ++j) h = splitmix64_finalize(h ^ w[j]);
-  uint64_t slot = __umul64hi(h, (uint64_t)M.cap);
-  const int64_t probes = M.cap < AS_MAX_PROBE ? M.cap : AS_MAX_PROBE;
-  for (int64_t i = 0; i < probes; ++i) {
-    if (as_claim(M.tag + slot, (uint64_t)n + 1)) {
-      bool same = true;
-      for (int j = 0; j < nw && same; ++j) same = as_claim(M.w + slot * AS_MD5_WORDS + j, w[j]);
-      if (same) return (int64_t)slot;
-    }
-    if (++slot == (uint64_t)M.cap) slot = 0;
-  }
-  return -1;
+  return probe(h, M.cap, [&](uint64_t slot) {
+    bool same = claim(M.tag + slot, (uint64_t)n + 1) == (uint64_t)n + 1;
+    for (int j = 0; j < nw && same; ++j) same = claim(M.w + slot * AS_MD5_WORDS + j, w[j]) == w[j];
+    return same;
+  });
 }
 
 // ---- lines and tokens ------------------------------------------------------------------------------------------
 struct AsLine {
   int64_t s, te;   // line.strip()
   int nf;          // fields of .split(','); 7 = more than 6
-  int64_t c0, c1, c2, c3, c4;
+  int64_t c[5];    // the first five commas
   bool nul;
 };
 
-// line.strip() of [p, e) and its first five commas.  Warp-uniform.
+// line.strip() of [p, e) and its first five commas (line_starts.cuh); a blank line has one empty field.  Warp-uniform.
 __device__ void as_fields(const uint8_t* t, int64_t p, int64_t e, AsLine& L) {
-  const int lane = lane_id();
-  int64_t s = e, te = e;
-  for (int64_t w = p; w < e; w += 32) {
-    const int64_t q = w + lane;
-    const unsigned m = __ballot_sync(FULL_MASK, q < e && !is_py_space(byte_at(t, q)));
-    if (m) { s = w + __ffs(m) - 1; break; }
-  }
-  L.s = s; L.te = e; L.nul = false; L.nf = 1;
-  if (s == e) return;   // blank: one empty field
-  for (int64_t w = e; w > s; w -= 32) {
-    const int64_t q = w - 32 + lane;
-    const unsigned m = __ballot_sync(FULL_MASK, q >= s && !is_py_space(byte_at(t, q)));
-    if (m) { te = w - 32 + (31 - __clz(m)) + 1; break; }
-  }
-  L.te = te;
-  int nc = 0;
-  bool nul = false;
-  for (int64_t w = s; w < te && nc <= 5; w += 32) {
-    const int64_t q = w + lane;
-    const uint32_t b = q < te ? byte_at(t, q) : 1u;
-    unsigned m = __ballot_sync(FULL_MASK, b == ',');
-    nul |= __ballot_sync(FULL_MASK, b == 0) != 0;
-    while (m && nc <= 5) {
-      const int64_t c = w + __ffs(m) - 1;
-      m &= m - 1;
-      if (nc == 0) L.c0 = c;
-      if (nc == 1) L.c1 = c;
-      if (nc == 2) L.c2 = c;
-      if (nc == 3) L.c3 = c;
-      if (nc == 4) L.c4 = c;
-      ++nc;
-    }
-  }
-  L.nf = nc + 1;
-  L.nul = nul;
+  warp_strip(t, p, e, L.s, L.te);
+  L.nf = warp_seps(t, L.s, L.te, ',', L.c, L.nul) + 1;
 }
 
 struct AsSpans {
@@ -170,13 +121,13 @@ struct AsSpans {
 // get_join_mapper.py:15-33: AS_COMMON / AS_SAMPLE / AS_FILTERED by field count and the y=0 / z=1 filter, else AS_SKIP
 __device__ __forceinline__ int as_kind(const uint8_t* t, const AsLine& L, AsSpans& S) {
   if (L.nf == 3) {
-    S.md5_s = L.s; S.md5_e = L.c0; S.fs = L.c1 + 1; S.fe = L.te;
+    S.md5_s = L.s; S.md5_e = L.c[0]; S.fs = L.c[1] + 1; S.fe = L.te;
     return AS_COMMON;
   }
   if (L.nf != 6) return AS_SKIP;
-  S.md5_s = L.c2 + 1; S.md5_e = L.c3; S.fs = L.c4 + 1; S.fe = L.te;
-  const bool y0 = L.c1 - L.c0 == 2 && byte_at(t, L.c0 + 1) == '0';
-  const bool z1 = L.c2 - L.c1 == 2 && byte_at(t, L.c1 + 1) == '1';
+  S.md5_s = L.c[2] + 1; S.md5_e = L.c[3]; S.fs = L.c[4] + 1; S.fe = L.te;
+  const bool y0 = L.c[1] - L.c[0] == 2 && byte_at(t, L.c[0] + 1) == '0';
+  const bool z1 = L.c[2] - L.c[1] == 2 && byte_at(t, L.c[1] + 1) == '1';
   return y0 && z1 ? AS_FILTERED : AS_SAMPLE;
 }
 
@@ -200,34 +151,16 @@ __device__ int as_token(const uint8_t* t, int64_t s, int64_t e, AsTok& k) {
   for (int64_t p = s; p < k.p2; ++p)
     if (as_bad(byte_at(t, p))) return 2;
   // fid: 0 or [1-9][0-9]* below 2^63, so that its text and its number are one key
-  if (k.p3 == k.p2 + 1 || (byte_at(t, k.p2 + 1) == '0' && k.p3 > k.p2 + 2)) return 2;
-  uint64_t v = 0;
-  for (int64_t p = k.p2 + 1; p < k.p3; ++p) {
-    const uint64_t d = byte_at(t, p) - (uint64_t)'0';
-    if (d > 9 || v > (0x7FFFFFFFFFFFFFFFull - d) / 10) return 2;
-    v = v * 10 + d;
-  }
-  k.fid = v;
+  if ((byte_at(t, k.p2 + 1) == '0' && k.p3 > k.p2 + 2) || !parse_u63(t, k.p2 + 1, k.p3, k.fid)) return 2;
   for (int64_t p = k.p3 + 1; p < e; ++p)
     if (as_bad(byte_at(t, p))) return 2;
   return 0;
 }
 
-// feat_list.split('\x01') of [s, e) in windows of 32 bytes: visit(end, start, q) once per window (warp-uniform);
-// lanes with `end` set end the token [start, q).
-template <class Visit>
-__device__ __forceinline__ void as_tokens(const uint8_t* t, int64_t s, int64_t e, Visit&& visit) {
-  const int lane = lane_id();
-  int64_t carry = s - 1;
-  for (int64_t w = s; w <= e; w += 32) {
-    const int64_t q = w + lane;
-    const bool end = q <= e && (q == e || byte_at(t, q) == 1);
-    const unsigned m = __ballot_sync(FULL_MASK, end);
-    const unsigned below = m & lanemask_lt();
-    visit(end, (below ? w + 31 - __clz(below) : carry) + 1, q);
-    if (m) carry = w + 31 - __clz(m);
-  }
-}
+// the separator of feat_list.split('\x01'), for warp_split (line_starts.cuh)
+struct AsTokEnd {
+  __device__ bool operator()(uint32_t b) const { return b == 1; }
+};
 
 __device__ __forceinline__ bool as_any_bad(const uint8_t* t, int64_t s, int64_t e) {
   bool bad = false;
@@ -242,7 +175,7 @@ __device__ __forceinline__ bool as_any_bad(const uint8_t* t, int64_t s, int64_t 
 // restricted = it breaks a restriction (raised by the host).  Warp-uniform.
 __device__ int as_check(const uint8_t* t, const AsLine& L, const AsSpans& S, int kind, bool& restricted) {
   bool malformed = false, bad = false;
-  as_tokens(t, S.fs, S.fe, [&](bool end, int64_t s, int64_t q) {
+  warp_split(t, S.fs, S.fe, AsTokEnd{}, [&](bool end, int64_t s, int64_t q, unsigned) {
     int r = 0;
     if (end) { AsTok k; r = as_token(t, s, q, k); }
     malformed |= __ballot_sync(FULL_MASK, r == 1) != 0;
@@ -250,7 +183,7 @@ __device__ int as_check(const uint8_t* t, const AsLine& L, const AsSpans& S, int
   });
   if (malformed) return AS_SKIP;
   bad |= L.nul || S.md5_e - S.md5_s < 1 || S.md5_e - S.md5_s > AS_MAX_MD5 || as_any_bad(t, S.md5_s, S.md5_e);
-  if (kind == AS_SAMPLE) bad |= as_any_bad(t, L.s, L.c2);   // sample_id, y, z (the commas between them are not bad)
+  if (kind == AS_SAMPLE) bad |= as_any_bad(t, L.s, L.c[2]);   // sample_id, y, z (the commas between them are not bad)
   restricted = bad;
   return kind;
 }
@@ -291,7 +224,7 @@ __global__ void __launch_bounds__(AS_THREADS) as_classify_kernel(const uint8_t* 
       }
       slot = __shfl_sync(FULL_MASK, slot, 0);
       if (mode == 2 && kind == AS_SAMPLE) {   // get_stat_mapper.py:17-19 over the sample's own tokens
-        as_tokens(t, S.fs, S.fe, [&](bool end, int64_t s, int64_t q) {
+        warp_split(t, S.fs, S.fe, AsTokEnd{}, [&](bool end, int64_t s, int64_t q, unsigned) {
           if (!end) return;
           AsTok k;
           as_token(t, s, q, k);
@@ -372,7 +305,8 @@ __global__ void __launch_bounds__(AS_THREADS) as_count_commons_kernel(const uint
   for (int64_t r = (int64_t)blockIdx.x * AS_WARPS + (threadIdx.x >> 5); r < n_records; r += warps) {
     const uint32_t m = mult[r];
     if (m == 0) continue;
-    as_tokens(arena, rec_off[r], rec_off[r] + rec_len[r], [&](bool end, int64_t s, int64_t q) {
+    const int64_t s0 = rec_off[r];
+    warp_split(arena, s0, s0 + rec_len[r], AsTokEnd{}, [&](bool end, int64_t s, int64_t q, unsigned) {
       if (!end) return;
       AsTok k;
       as_token(arena, s, q, k);
@@ -470,7 +404,7 @@ __device__ __forceinline__ int64_t as_lookup(const uint64_t* __restrict__ vocab,
 template <bool W>
 __device__ void as_remap(const uint8_t* t, int64_t s, int64_t e, const uint64_t* vocab, int64_t n_vocab, char* o,
                          int64_t& pos, int64_t& kept) {
-  as_tokens(t, s, e, [&](bool end, int64_t ts, int64_t q) {
+  warp_split(t, s, e, AsTokEnd{}, [&](bool end, int64_t ts, int64_t q, unsigned) {
     AsTok k;
     int64_t id = -1;
     if (end) {
@@ -554,7 +488,7 @@ __global__ void __launch_bounds__(AS_THREADS) as_emit_kernel(const uint8_t* __re
     const uint64_t r = as_shuffle_key(a.seed, (uint64_t)(a.line_base + row));
     const int nr = dec_digits(r);
     char* o = W ? a.out + (base - a.lo) : nullptr;
-    int64_t pos = nr + 1 + (L.c2 - L.s) + 1;
+    int64_t pos = nr + 1 + (L.c[2] - L.s) + 1;
     if (W) {
       for (int64_t i = lane; i < pos; i += 32) {
         char c;
@@ -566,7 +500,7 @@ __global__ void __launch_bounds__(AS_THREADS) as_emit_kernel(const uint8_t* __re
       }
     }
     int64_t kept = 0;
-    as_remap<W>(t, L.c4 + 1, L.te, a.vocab, a.n_vocab, o, pos, kept);
+    as_remap<W>(t, L.c[4] + 1, L.te, a.vocab, a.n_vocab, o, pos, kept);
     const int32_t rec = a.s_rec[k];
     const int64_t cs = rec >= 0 ? a.r_off[rec] : 0, cl = rec >= 0 ? a.r_off[rec + 1] - cs : 0;
     if (cl > 0) {
@@ -696,9 +630,9 @@ int ctr_aliccp_sample_classify(const char* text, size_t len, int64_t n_lines, in
                                void* ws, size_t ws_bytes, ctr_stream_t stream) {
   CTR_REQUIRE((len == 0 || text) && n_lines >= 0 && mode >= 0 && mode <= 2 && info, CTR_ERR_INVALID_ARG,
               "ctr_aliccp_sample_classify: bad arguments");
-  CTR_REQUIRE(mode == 0 || (md5_table && md5_capacity > 0 && md5_capacity <= AS_MAX_CAP), CTR_ERR_INVALID_ARG,
+  CTR_REQUIRE(mode == 0 || (md5_table && md5_capacity > 0 && md5_capacity <= KT_MAX_CAP), CTR_ERR_INVALID_ARG,
               "ctr_aliccp_sample_classify: bad md5 table");
-  CTR_REQUIRE(mode != 2 || (count_table && count_capacity > 0 && count_capacity <= AS_MAX_CAP), CTR_ERR_INVALID_ARG,
+  CTR_REQUIRE(mode != 2 || (count_table && count_capacity > 0 && count_capacity <= KT_MAX_CAP), CTR_ERR_INVALID_ARG,
               "ctr_aliccp_sample_classify: bad count table");
   CTR_REQUIRE(len < AS_MAX_LEN, CTR_ERR_INVALID_ARG, "ctr_aliccp_sample_classify: chunk too large (len < 2^30)");
   CTR_REQUIRE(ws && ws_bytes >= ctr_aliccp_sample_chunk_workspace_bytes(len, n_lines), CTR_ERR_WORKSPACE,
@@ -765,7 +699,7 @@ int ctr_aliccp_sample_resolve(const void* md5_table, int64_t md5_capacity, int32
 int ctr_aliccp_sample_count_commons(const uint8_t* arena, const int64_t* rec_off, const int32_t* rec_len,
                                     const uint32_t* mult, int64_t n_records, void* count_table, int64_t count_capacity,
                                     int64_t* info, ctr_stream_t stream) {
-  CTR_REQUIRE(n_records >= 0 && count_table && count_capacity > 0 && count_capacity <= AS_MAX_CAP && info &&
+  CTR_REQUIRE(n_records >= 0 && count_table && count_capacity > 0 && count_capacity <= KT_MAX_CAP && info &&
                   (n_records == 0 || (arena && rec_off && rec_len && mult)),
               CTR_ERR_INVALID_ARG, "ctr_aliccp_sample_count_commons: bad arguments");
   cudaStream_t st = as_stream(stream);
@@ -783,7 +717,7 @@ size_t ctr_aliccp_sample_vocab_workspace_bytes(int64_t count_capacity) {
 
 int ctr_aliccp_sample_vocab(const void* count_table, int64_t count_capacity, int64_t cutoff, uint64_t* vocab,
                             int64_t* info, void* ws, size_t ws_bytes, ctr_stream_t stream) {
-  CTR_REQUIRE(count_table && count_capacity > 0 && count_capacity <= AS_MAX_CAP && vocab && info,
+  CTR_REQUIRE(count_table && count_capacity > 0 && count_capacity <= KT_MAX_CAP && vocab && info,
               CTR_ERR_INVALID_ARG, "ctr_aliccp_sample_vocab: bad arguments");
   CTR_REQUIRE(ws && ws_bytes >= ctr_aliccp_sample_vocab_workspace_bytes(count_capacity), CTR_ERR_WORKSPACE,
               "ctr_aliccp_sample_vocab: workspace too small");
@@ -830,7 +764,7 @@ int ctr_aliccp_sample_vocab(const void* count_table, int64_t count_capacity, int
 
 int ctr_aliccp_sample_feat_cnts(char* out, const void* ws, size_t ws_bytes, int64_t count_capacity,
                                 ctr_stream_t stream) {
-  CTR_REQUIRE(out && count_capacity > 0 && count_capacity <= AS_MAX_CAP, CTR_ERR_INVALID_ARG,
+  CTR_REQUIRE(out && count_capacity > 0 && count_capacity <= KT_MAX_CAP, CTR_ERR_INVALID_ARG,
               "ctr_aliccp_sample_feat_cnts: bad arguments");
   CTR_REQUIRE(ws && ws_bytes >= ctr_aliccp_sample_vocab_workspace_bytes(count_capacity), CTR_ERR_WORKSPACE,
               "ctr_aliccp_sample_feat_cnts: workspace too small");
@@ -905,7 +839,7 @@ size_t ctr_aliccp_sample_order_workspace_bytes(int64_t n_samples) {
 
 int ctr_aliccp_sample_order(uint64_t* s_key, int64_t* s_val, int64_t n_samples, int64_t parts, int64_t* part_bytes,
                             void* ws, size_t ws_bytes, ctr_stream_t stream) {
-  CTR_REQUIRE(n_samples >= 0 && n_samples < AS_MAX_CAP && parts >= 1 && parts <= (1 << 20) && part_bytes &&
+  CTR_REQUIRE(n_samples >= 0 && n_samples <= INT32_MAX && parts >= 1 && parts <= (1 << 20) && part_bytes &&
                   (n_samples == 0 || (s_key && s_val)),
               CTR_ERR_INVALID_ARG, "ctr_aliccp_sample_order: bad arguments");
   CTR_REQUIRE(ws && ws_bytes >= ctr_aliccp_sample_order_workspace_bytes(n_samples), CTR_ERR_WORKSPACE,

@@ -2,7 +2,7 @@
 // (deep_ctr/Feature_pipeline/get_aliccp_tfrecord.py gen_tfrecords, :38-102; DESIGN.md §2.6).
 //
 // A line is `sample_id,y,z,field:fid:val field:fid:val ...`.  One warp per line, three kernels over a text chunk cut
-// at line ends (line starts from line_starts.cuh):
+// at line ends (line starts and the warp splitting from line_starts.cuh):
 //   plan      strip, split at ',' (lines without exactly 4 fields are skipped), tokenise the feature list with a ballot
 //             over ' ' / ':' separators, classify every triple against the 19 kept field names, fold per-field
 //             occurrence counts and id varint bytes, and size the record exactly (16 bytes of framing plus the nested
@@ -12,13 +12,15 @@
 //   write     re-tokenises each line and writes its record at the planned offset: the 15 features in sorted key order
 //             (packed Int64List / FloatList, as tfrecord.encode_example writes them), the length header and both
 //             masked CRC-32Cs (crc32c.cuh).
-// Numbers: an id must be [0-9]+ below 2^63.  A label or value is converted here when it is plain decimal with a
-// mantissa <= 2^53 and a decimal exponent of magnitude <= 22, where one fp64 multiply or divide by an exact power of
-// ten is correctly rounded, i.e. equals Python's float(); it is then rounded to float32 as the FloatList does.  Any
-// other number is declined: the host converts it with Python float() and uploads the float32 before the write.
+// Numbers: an id must be [0-9]+ below 2^63 (parse_u63 of decimal.cuh).  A label or value is converted here when it is
+// plain decimal with a mantissa <= 2^53 and a decimal exponent of magnitude <= 22, where one fp64 multiply or divide by
+// an exact power of ten (decimal.cuh's kPow10) is correctly rounded, i.e. equals Python's float(); it is then rounded
+// to float32 as the FloatList does.  Any other number is declined: the host converts it with Python float() and
+// uploads the float32 before the write.
 // Error word (uint64, ~0 = none): (line << 8) | code, the smallest over the chunk = the first failing line.
 #include "common.cuh"
 #include "crc32c.cuh"
+#include "decimal.cuh"
 #include "line_starts.cuh"
 
 namespace ctr {
@@ -52,8 +54,6 @@ __constant__ int kAlKeySrc[AL_KEYS] = {18, 15, 17, 16, -1, 13, 13, 11, 11, 14, 1
 __constant__ int kAlKeyFloat[AL_KEYS] = {0, 0, 0, 0, 0, 0, 1, 0, 1, 0, 1, 0, 1, 1, 1};
 __constant__ int kAlIdKey[AL_CLASSES - AL_UMH] = {7, 11, 5, 9, 1, 3, 2, 0};   // class 11.. -> its ids key
 __constant__ int kAlValKey[AL_AD - AL_UMH] = {8, 12, 6, 10};                   // class 11..14 -> its vals key
-__constant__ double kAlPow10[23] = {1e0,  1e1,  1e2,  1e3,  1e4,  1e5,  1e6,  1e7,  1e8,  1e9,  1e10, 1e11,
-                                    1e12, 1e13, 1e14, 1e15, 1e16, 1e17, 1e18, 1e19, 1e20, 1e21, 1e22};
 
 __device__ __forceinline__ int al_vl(uint64_t v) { return v < 128 ? 1 : (70 - __clzll((long long)v)) / 7; }
 
@@ -73,41 +73,12 @@ struct AlLine {
 
 // line.strip().split(',') of [p, e) -> false unless it has exactly 4 fields.  Warp-uniform.
 __device__ __forceinline__ bool al_fields(const uint8_t* t, int64_t p, int64_t e, AlLine& L) {
-  const int lane = lane_id();
-  int64_t s = e, te = e;
-  for (int64_t w = p; w < e; w += 32) {
-    const int64_t q = w + lane;
-    const unsigned m = __ballot_sync(FULL_MASK, q < e && !is_py_space(byte_at(t, q)));
-    if (m) { s = w + __ffs(m) - 1; break; }
-  }
-  if (s == e) return false;   // blank
-  for (int64_t w = e; w > s; w -= 32) {
-    const int64_t q = w - 32 + lane;
-    const unsigned m = __ballot_sync(FULL_MASK, q >= s && !is_py_space(byte_at(t, q)));
-    if (m) { te = w - 32 + (31 - __clz(m)) + 1; break; }
-  }
-  int nc = 0;
-  int64_t c[3] = {0, 0, 0};
-  bool nul = false;
-  for (int64_t w = s; w < te && nc <= 3; w += 32) {
-    const int64_t q = w + lane;
-    const uint32_t b = q < te ? byte_at(t, q) : 1u;
-    unsigned m = __ballot_sync(FULL_MASK, b == ',');
-    nul |= __ballot_sync(FULL_MASK, b == 0) != 0;
-    while (m && nc <= 3) {
-      const int k = __ffs(m) - 1;
-      m &= m - 1;
-      if (nc == 0) c[0] = w + k;
-      if (nc == 1) c[1] = w + k;
-      if (nc == 2) c[2] = w + k;
-      ++nc;
-    }
-  }
-  if (nc != 3) return false;
+  int64_t s, te, c[3] = {0, 0, 0};
+  warp_strip(t, p, e, s, te);
+  if (warp_seps(t, s, te, ',', c, L.nul) != 3) return false;
   L.s1 = c[0] + 1; L.e1 = c[1];
   L.s2 = c[1] + 1; L.e2 = c[2];
   L.s3 = c[2] + 1; L.e3 = te;
-  L.nul = nul;
   return true;
 }
 
@@ -156,24 +127,10 @@ __device__ __forceinline__ bool al_value(const uint8_t* t, int64_t s, int64_t e,
   const int E = ex - frac;
   if (M != 0) {
     if (E > 22 || E < -22) return false;
-    d = E >= 0 ? __dmul_rn(d, kAlPow10[E]) : __ddiv_rn(d, kAlPow10[-E]);
+    d = E >= 0 ? __dmul_rn(d, kPow10[E]) : __ddiv_rn(d, kPow10[-E]);
   }
   const float f = __double2float_rn(d);
   out = neg ? -f : f;
-  return true;
-}
-
-// [0-9]+ below 2^63 -> true and its value.  One lane.
-__device__ __forceinline__ bool al_id(const uint8_t* t, int64_t s, int64_t e, uint64_t& v) {
-  v = 0;
-  if (e <= s) return false;
-  for (int64_t p = s; p < e; ++p) {
-    const uint32_t c = byte_at(t, p);
-    if (c < '0' || c > '9') return false;
-    const uint64_t d = c - '0';
-    if (v > (0x7FFFFFFFFFFFFFFFull - d) / 10) return false;
-    v = v * 10 + d;
-  }
   return true;
 }
 
@@ -193,23 +150,18 @@ struct AlTok {
   int idx, role, cls;   // token number, idx % 3 (0 field, 1 fid, 2 val), class of its triple's field
 };
 
-// re.split('[ :]', fields[3]) in windows of 32 bytes: visit(sep, tok, window_mask) once per window (warp-uniform);
-// lanes with sep set end a token.  -> number of tokens.
+// re.split('[ :]', fields[3]) by warp_split (line_starts.cuh): visit(sep, tok) once per window (warp-uniform); lanes
+// with sep set end a token.  -> number of tokens.
 template <class Visit>
 __device__ __forceinline__ int al_tokens(const uint8_t* t, int64_t s, int64_t e, Visit&& visit) {
   const int lane = lane_id();
   int count = 0, carry_cls = -1;
-  int64_t carry = s - 1;
-  for (int64_t w = s; w <= e; w += 32) {
-    const int64_t q = w + lane;
-    const uint32_t b = q < e ? byte_at(t, q) : ' ';
-    const bool sep = q <= e && (b == ' ' || b == ':');
-    const unsigned m = __ballot_sync(FULL_MASK, sep);
-    const unsigned below = m & lanemask_lt();
+  const auto is_sep = [](uint32_t b) { return b == ' ' || b == ':'; };
+  warp_split(t, s, e, is_sep, [&](bool sep, int64_t start, int64_t q, unsigned m) {
     AlTok k;
+    k.start = start;
     k.end = q;
-    k.start = (below ? w + 31 - __clz(below) : carry) + 1;
-    k.idx = count + __popc(below);
+    k.idx = count + __popc(m & lanemask_lt());
     k.role = k.idx % 3;
     const int cls = sep && k.role == 0 ? al_class(t, k.start, k.end) : -1;
     const unsigned fm = __ballot_sync(FULL_MASK, sep && k.role == 0);
@@ -218,10 +170,9 @@ __device__ __forceinline__ int al_tokens(const uint8_t* t, int64_t s, int64_t e,
     k.cls = fb ? from : carry_cls;
     const int last = __shfl_sync(FULL_MASK, cls, fm ? 31 - __clz(fm) : 0);
     if (fm) carry_cls = last;
-    visit(sep, k, m);
+    visit(sep, k);
     count += __popc(m);
-    if (m) carry = w + 31 - __clz(m);
-  }
+  });
   return count;
 }
 
@@ -263,13 +214,13 @@ __device__ __forceinline__ void al_pass1(const uint8_t* t, const AlLine& L, AlWa
     spans[3 * k + 2] = lane == 0 ? L.e1 : L.e2;
   }
   int ndecl = !R.ys + !R.zs, first_empty = 0x7FFFFFFF, first_bad = 0x7FFFFFFF;
-  const int n = al_tokens(t, L.s3, L.e3, [&](bool sep, const AlTok& k, unsigned) {
+  const int n = al_tokens(t, L.s3, L.e3, [&](bool sep, const AlTok& k) {
     const unsigned em = __ballot_sync(FULL_MASK, sep && k.end == k.start);
     first_empty = min(first_empty, al_first(em, k.idx));
     bool bad = false, decl = false;
     if (sep && al_is_id(k)) {
       uint64_t id;
-      bad = !al_id(t, k.start, k.end, id);
+      bad = !parse_u63(t, k.start, k.end, id);
       if (!bad) {
         atomicAdd(&W.cnt[k.cls], 1);
         atomicAdd(&W.bytes[k.cls], al_vl(id));
@@ -464,12 +415,12 @@ __global__ void __launch_bounds__(AL_THREADS, 2) al_write_kernel(const uint8_t* 
 
     // ---- pass 2: every kept id and value at its place, in line order ----
     int nd = !R.ys + !R.zs;
-    al_tokens(t, L.s3, L.e3, [&](bool sep, const AlTok& k, unsigned) {
+    al_tokens(t, L.s3, L.e3, [&](bool sep, const AlTok& k) {
       const bool id = sep && al_is_id(k), val = sep && al_is_val(k);
       uint64_t v = 0;
       float f = 0.f;
       bool simple = true;
-      if (id) al_id(t, k.start, k.end, v);
+      if (id) parse_u63(t, k.start, k.end, v);
       if (val) simple = al_value(t, k.start, k.end, f);
       const unsigned dm = __ballot_sync(FULL_MASK, val && !simple);
       if (val && !simple) f = decl_vals[dbase + nd + __popc(dm & lanemask_lt())];

@@ -4,7 +4,7 @@
 // vocabulary stay resident):
 //   stats  one thread per train line: the 13 integer columns fold their clipped min/max into int64[26] (shared-memory
 //          atomics per CTA, then global atomics: exact and order-free); the 26 categorical values count into an
-//          open-addressing table keyed by (field, 8-byte key).
+//          open-addressing table keyed by (field, 8-byte key) (probe policy: key_table.cuh).
 //   vocab  keep count >= cutoff, LSD radix sort by (field, -count, key) (13 passes of 8 bits over 104 key bits),
 //          write each id back into its table slot.
 //   emit   plan: one thread per line computes its output length (and raises what the reference raises); the tile
@@ -16,13 +16,13 @@
 // Restrictions (DESIGN.md §2.4; each raises): I values match [+-]?[0-9]+ with magnitude <= 2^53; train C values are
 // at most 8 bytes, hold no NUL and are not "<unk>", so a value packs big-endian, zero-padded into a uint64 whose
 // numeric order is Python's bytewise string order and 0 never is a key.
+#include "key_table.cuh"
 #include "line_starts.cuh"
 
 namespace ctr {
 
 constexpr int CF_NI = 13, CF_NC = 26, CF_COLS = 1 + CF_NI + CF_NC;
 constexpr int CF_THREADS = 256;                       // per-line kernels: one line per thread, one tile per CTA
-constexpr int64_t CF_MAX_PROBE = 1 << 15;             // a key that finds no slot within this many probes overflows
 constexpr uint64_t CF_UNK = 0x3C756E6B3E000000ull;    // "<unk>" packed
 constexpr int64_t CF_MAXSIZE = 0x7FFFFFFFFFFFFFFFll;  // Python 2's sys.maxsize on LP64
 
@@ -52,47 +52,31 @@ struct CfTable {
         cap(c) {}
 };
 
-__device__ __forceinline__ uint64_t cf_home(uint64_t key, int f, int64_t cap) {
-  return __umul64hi(splitmix64_finalize(key ^ ((uint64_t)(f + 1) * 0x9E3779B97F4A7C15ull)), (uint64_t)cap);
+__device__ __forceinline__ uint64_t cf_hash(uint64_t key, int f) {
+  return splitmix64_finalize(key ^ ((uint64_t)(f + 1) * 0x9E3779B97F4A7C15ull));
 }
 
-// Linear probing without locks: a slot's key is set once (CAS 0 -> key), then its tag once (CAS 0 -> field + 1).
-// Every thread inserting (f, key) takes the same decision at every slot it visits (both words are final once
-// non-zero), so all of them end in the same slot.
+// (f, key) owns the slot whose key word is key and whose tag word is f + 1; both are claimed in that order
+// (key_table.cuh).
 __device__ __forceinline__ bool cf_insert(const CfTable& T, uint64_t key, int f) {
   const uint32_t tag = (uint32_t)f + 1;
-  uint64_t s = cf_home(key, f, T.cap);
-  const int64_t probes = T.cap < CF_MAX_PROBE ? T.cap : CF_MAX_PROBE;
-  for (int64_t i = 0; i < probes; ++i) {
-    uint64_t k = *reinterpret_cast<volatile uint64_t*>(T.keys + s);
-    if (k == 0) {
-      k = atomicCAS(reinterpret_cast<unsigned long long*>(T.keys + s), 0ull, (unsigned long long)key);
-      if (k == 0) k = key;
-    }
-    if (k == key) {
-      uint32_t t = *reinterpret_cast<volatile uint32_t*>(T.tags + s);
-      if (t == 0) {
-        t = atomicCAS(T.tags + s, 0u, tag);
-        if (t == 0) t = tag;
-      }
-      if (t == tag) { atomicAdd(T.vals + s, 1u); return true; }
-    }
-    if (++s == (uint64_t)T.cap) s = 0;
-  }
-  return false;
+  const int64_t slot = probe(cf_hash(key, f), T.cap, [&](uint64_t s) {
+    return claim(T.keys + s, key) == key && claim(T.tags + s, tag) == tag;
+  });
+  if (slot >= 0) atomicAdd(T.vals + slot, 1u);
+  return slot >= 0;
 }
 
 __device__ __forceinline__ uint32_t cf_lookup(const CfTable& T, uint64_t key, int f) {
   const uint32_t tag = (uint32_t)f + 1;
-  uint64_t s = cf_home(key, f, T.cap);
-  const int64_t probes = T.cap < CF_MAX_PROBE ? T.cap : CF_MAX_PROBE;
-  for (int64_t i = 0; i < probes; ++i) {
+  uint32_t v = 0;
+  probe(cf_hash(key, f), T.cap, [&](uint64_t s) {
     const uint64_t k = T.keys[s];
-    if (k == 0) return 0;
-    if (k == key && T.tags[s] == tag) return T.vals[s];
-    if (++s == (uint64_t)T.cap) s = 0;
-  }
-  return 0;
+    const bool hit = k == key && T.tags[s] == tag;
+    if (hit) v = T.vals[s];
+    return k == 0 || hit;
+  });
+  return v;
 }
 
 // ---- tokens --------------------------------------------------------------------------------------------------
@@ -453,7 +437,6 @@ struct CfVocabWs {
 
 // chunk buffers the per-line kernels accept: len < 2^30 keeps block offsets and line lengths in int32
 constexpr size_t CF_MAX_LEN = (size_t)1 << 30;
-constexpr int64_t CF_MAX_CAP = (int64_t)1 << 31;   // slot numbers are uint32, sort positions int32
 
 }  // namespace ctr
 
@@ -469,7 +452,7 @@ int ctr_criteo_stats(const char* text, size_t len, int64_t line_base, void* tabl
                      int64_t* info, void* ws, size_t ws_bytes, ctr_stream_t stream) {
   CTR_REQUIRE(info && minmax && table && capacity > 0 && line_base >= 0 && (len == 0 || text), CTR_ERR_INVALID_ARG,
               "ctr_criteo_stats: bad arguments");
-  CTR_REQUIRE(capacity <= CF_MAX_CAP, CTR_ERR_INVALID_ARG, "ctr_criteo_stats: capacity > 2^31");
+  CTR_REQUIRE(capacity <= KT_MAX_CAP, CTR_ERR_INVALID_ARG, "ctr_criteo_stats: capacity > 2^31");
   CTR_REQUIRE(len < CF_MAX_LEN, CTR_ERR_INVALID_ARG, "ctr_criteo_stats: chunk too large (len < 2^30)");
   CTR_REQUIRE(ws && ws_bytes >= ctr_criteo_stats_workspace_bytes(len), CTR_ERR_WORKSPACE,
               "ctr_criteo_stats: workspace too small");
@@ -494,7 +477,7 @@ size_t ctr_criteo_vocab_workspace_bytes(int64_t capacity) {
 int ctr_criteo_vocab(void* table, int64_t capacity, int64_t cutoff, uint64_t* vocab_keys, int64_t* field_counts,
                      void* ws, size_t ws_bytes, ctr_stream_t stream) {
   CTR_REQUIRE(table && capacity > 0 && vocab_keys && field_counts, CTR_ERR_INVALID_ARG, "ctr_criteo_vocab: bad arguments");
-  CTR_REQUIRE(capacity <= CF_MAX_CAP, CTR_ERR_INVALID_ARG, "ctr_criteo_vocab: capacity > 2^31");
+  CTR_REQUIRE(capacity <= KT_MAX_CAP, CTR_ERR_INVALID_ARG, "ctr_criteo_vocab: capacity > 2^31");
   CTR_REQUIRE(ws && ws_bytes >= ctr_criteo_vocab_workspace_bytes(capacity), CTR_ERR_WORKSPACE,
               "ctr_criteo_vocab: workspace too small");
   cudaStream_t st = as_stream(stream);
@@ -532,7 +515,7 @@ size_t ctr_criteo_emit_workspace_bytes(size_t len) { return CfEmitWs(nullptr, le
 
 static int cf_emit_args(const void* table, int64_t capacity, const double* num_min, const double* num_den,
                         const int64_t* offsets, const char* label, int label_len, int test, CfEmitArgs& a) {
-  CTR_REQUIRE(table && capacity > 0 && capacity <= CF_MAX_CAP && num_min && num_den && offsets && label_len >= 0 &&
+  CTR_REQUIRE(table && capacity > 0 && capacity <= KT_MAX_CAP && num_min && num_den && offsets && label_len >= 0 &&
                   (label_len == 0 || label),
               CTR_ERR_INVALID_ARG, "ctr_criteo_emit: bad arguments");
   a = CfEmitArgs{CfTable(const_cast<void*>(table), capacity), num_min, num_den, offsets, label, label_len, test ? 1 : 0};

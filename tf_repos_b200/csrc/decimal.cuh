@@ -1,4 +1,6 @@
-// decimal.cuh -- the fast decimal-to-fp32 path of the text tokenizers (libsvm_device.cu, csv_device.cu).
+// decimal.cuh -- decimal numbers in device text: the fast decimal-to-fp32 path of the text tokenizers
+// (libsvm_device.cu, csv_device.cu), the powers of ten behind it (also aliccp_tfrecord.cu's values), and parse_u63,
+// the id grammar of the Ali-CCP kernels (aliccp_tfrecord.cu, aliccp_sample.cu).
 //
 // parse_float converts what it is sure about and hands everything else to the host parser: > 15 significant digits,
 // |decimal exponent| > 22, inf/nan/hex, a result outside the normal fp32 range, or a double that sits within one ulp
@@ -72,6 +74,20 @@ __device__ __forceinline__ int parse_float(const unsigned char* __restrict__ t, 
   const float f = __double2float_rn(d);
   out = neg ? -f : f;
   return LS_OK;
+}
+
+// [0-9]+ below 2^63 -> true and its value.  One thread.
+__device__ __forceinline__ bool parse_u63(const uint8_t* t, int64_t s, int64_t e, uint64_t& v) {
+  v = 0;
+  if (e <= s) return false;
+  for (int64_t p = s; p < e; ++p) {
+    const uint32_t c = byte_at(t, p);
+    if (c < '0' || c > '9') return false;
+    const uint64_t d = c - '0';
+    if (v > (0x7FFFFFFFFFFFFFFFull - d) / 10) return false;
+    v = v * 10 + d;
+  }
+  return true;
 }
 
 }  // namespace

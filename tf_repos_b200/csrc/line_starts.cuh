@@ -1,8 +1,11 @@
-// line_starts.cuh -- line starts of a text buffer in device memory, shared by the tokenizers
-// (libsvm_device.cu, csv_device.cu, criteo_feature.cu, aliccp_tfrecord.cu, aliccp_sample.cu, smart_feature.cu).
+// line_starts.cuh -- line starts of a text buffer in device memory, and the warp-per-line splitting, shared by the
+// tokenizers (libsvm_device.cu, csv_device.cu, criteo_feature.cu, aliccp_tfrecord.cu, aliccp_sample.cu,
+// smart_feature.cu).
 //
 // Kernels: (1) count '\n' per 4 KB block; (2) scan the block counts (cta_scan_kernel); (3) emit line starts.
 // LineStarts is their workspace and launches them; line_bounds / chunk_lines read the result in the per-line kernels.
+// A kernel that gives each line a warp reads it in windows of 32 bytes: warp_strip is line.strip(), warp_seps the
+// first separators of a line (its fields), warp_split its tokens.
 // They live in an anonymous namespace so that every translation unit that includes this header owns its copy.
 #pragma once
 #include "common.cuh"
@@ -77,6 +80,72 @@ __device__ __forceinline__ int64_t chunk_lines(const uint8_t* __restrict__ t, in
                                                int64_t cap = INT64_MAX) {
   const int64_t n = nn + ((len > 0 && t[len - 1] != '\n') ? 1 : 0);
   return n < cap ? n : cap;
+}
+
+// ---- one warp per line: the line's bytes in windows of 32, one byte a lane, read by ballots ----
+
+// line.strip() of [p, e) -> [s, te); s = te = e for a blank line.  Warp-uniform.
+__device__ __forceinline__ void warp_strip(const uint8_t* t, int64_t p, int64_t e, int64_t& s, int64_t& te) {
+  const int lane = lane_id();
+  s = e; te = e;
+  for (int64_t w = p; w < e; w += 32) {
+    const int64_t q = w + lane;
+    const unsigned m = __ballot_sync(FULL_MASK, q < e && !is_py_space(byte_at(t, q)));
+    if (m) { s = w + __ffs(m) - 1; break; }
+  }
+  if (s == e) return;
+  for (int64_t w = e; w > s; w -= 32) {
+    const int64_t q = w - 32 + lane;
+    const unsigned m = __ballot_sync(FULL_MASK, q >= s && !is_py_space(byte_at(t, q)));
+    if (m) { te = w - 32 + (31 - __clz(m)) + 1; break; }
+  }
+}
+
+// pos[n] = v for n < MAX, as a chain of constant indices so that pos stays in registers
+template <int K = 0, int MAX>
+__device__ __forceinline__ void seps_put(int64_t (&pos)[MAX], int n, int64_t v) {
+  if (n == K) pos[K] = v;
+  if constexpr (K + 1 < MAX) seps_put<K + 1>(pos, n, v);
+}
+
+// The first MAX bytes sep of [s, te) -> pos, nul = [s, te) holds a NUL byte (within the windows read); -> their count,
+// MAX + 1 = more than MAX.  The walk stops at the window of separator MAX + 1.  Warp-uniform.
+template <int MAX>
+__device__ __forceinline__ int warp_seps(const uint8_t* t, int64_t s, int64_t te, uint32_t sep, int64_t (&pos)[MAX],
+                                         bool& nul) {
+  const int lane = lane_id();
+  int n = 0;
+  nul = false;
+  for (int64_t w = s; w < te && n <= MAX; w += 32) {
+    const int64_t q = w + lane;
+    const uint32_t b = q < te ? byte_at(t, q) : 1u;
+    unsigned m = __ballot_sync(FULL_MASK, b == sep);
+    nul |= __ballot_sync(FULL_MASK, b == 0) != 0;
+    while (m && n <= MAX) {
+      const int c = __ffs(m) - 1;
+      m &= m - 1;
+      seps_put(pos, n, w + c);
+      ++n;
+    }
+  }
+  return n;
+}
+
+// [s, e) split at the bytes where is_sep(byte) holds, in windows of 32 bytes: visit(end, start, q, mask) once per
+// window (warp-uniform), mask = the window's ballot of ends; lanes with `end` set end the token [start, q), the last
+// one at q = e.
+template <class IsSep, class Visit>
+__device__ __forceinline__ void warp_split(const uint8_t* t, int64_t s, int64_t e, IsSep&& is_sep, Visit&& visit) {
+  const int lane = lane_id();
+  int64_t carry = s - 1;
+  for (int64_t w = s; w <= e; w += 32) {
+    const int64_t q = w + lane;
+    const bool end = q <= e && (q == e || is_sep(byte_at(t, q)));
+    const unsigned m = __ballot_sync(FULL_MASK, end);
+    const unsigned below = m & lanemask_lt();
+    visit(end, (below ? w + 31 - __clz(below) : carry) + 1, q, m);
+    if (m) carry = w + 31 - __clz(m);
+  }
 }
 
 // Workspace of a chunk of len bytes: block_counts int32[nb] | n_newlines int64[2] | line_start int64[max_rows + 1],

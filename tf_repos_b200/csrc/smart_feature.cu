@@ -5,16 +5,18 @@
 //   map    the feature_map text, resident: one thread per line strips it, splits it on ' ' and classifies its key
 //          (categorical `name|value`, or a continuous `name`; keys no lookup can reach are dropped); each kept key is
 //          inserted into an open-addressing table (CAS on the slot's first line, full-key comparison against the
-//          resident text), the largest line of a key wins by atomicMax, then a second pass fills each slot's spans.
-//   emit   one warp per CSV line: strip and the commas by ballot; each lane formats the fields it owns (a lookup per
-//          categorical field); plan = output bytes per line (a dropped line gives 0), a tiled scan, write = each line
-//          at its offset.
+//          resident text; probe policy: key_table.cuh), the largest line of a key wins by atomicMax, then a second
+//          pass fills each slot's spans.
+//   emit   one warp per CSV line: strip (line_starts.cuh) and the commas by ballot; each lane formats the fields it
+//          owns (a lookup per categorical field); plan = output bytes per line (a dropped line gives 0), a tiled scan,
+//          write = each line at its offset.
 //   build  get_feature_map with its NameError fixed: one warp per line inserts every key with the smallest global
 //          position (line << 7 | column) by atomicMax of its complement; new keys are copied from the chunk into a
 //          resident arena after each chunk; the keys are compacted, radix sorted by position and rendered with fids
 //          129, 130, ... in that order.
 // Frappe: one warp per line, the label rewrite on the same line-start / plan / scan / write skeleton.
 // Every order comes from a sort or a scan and every reduction is an integer one: two runs give the same bytes.
+#include "key_table.cuh"
 #include "line_starts.cuh"
 
 namespace ctr {
@@ -22,9 +24,7 @@ namespace ctr {
 constexpr int SF_THREADS = 256, SF_WARPS = SF_THREADS / 32;
 constexpr int SF_COLS = 128, SF_NAMED = 28, SF_CONT_LO = 11, SF_CONT_HI = 27, SF_NCONT = SF_CONT_HI - SF_CONT_LO + 1;
 constexpr int SF_MAX_FIELDS = 129;                  // a line of more fields is dropped (CSV_COLUMNS[128] raises)
-constexpr int64_t SF_MAX_PROBE = 1 << 15;           // a key that finds no slot within this many probes overflows
 constexpr size_t SF_MAX_LEN = (size_t)1 << 30;      // chunk and map bytes: line offsets stay in int32
-constexpr int64_t SF_MAX_CAP = (int64_t)1 << 31;    // slot numbers are uint32
 constexpr int SF_SCAN_TILE = 1024;
 constexpr uint64_t SF_PENDING = 1ull << 63, SF_OFF_MASK = (1ull << 56) - 1;
 constexpr uint32_t SF_CONT_ITEM = 0x80000000u;      // build items: slot number, or this | column for a continuous key
@@ -87,23 +87,6 @@ __device__ __forceinline__ bool sf_same(const uint8_t* a, const uint8_t* b, int6
 }
 
 // ---- lines -----------------------------------------------------------------------------------------------------
-// line.strip() of [p, e) -> [s, te).  Warp-uniform.
-__device__ __forceinline__ void sf_strip(const uint8_t* t, int64_t p, int64_t e, int64_t& s, int64_t& te) {
-  const int lane = lane_id();
-  s = e; te = e;
-  for (int64_t w = p; w < e; w += 32) {
-    const int64_t q = w + lane;
-    const unsigned m = __ballot_sync(FULL_MASK, q < e && !is_py_space(byte_at(t, q)));
-    if (m) { s = w + __ffs(m) - 1; break; }
-  }
-  if (s == e) return;
-  for (int64_t w = e; w > s; w -= 32) {
-    const int64_t q = w - 32 + lane;
-    const unsigned m = __ballot_sync(FULL_MASK, q >= s && !is_py_space(byte_at(t, q)));
-    if (m) { te = w - 32 + (31 - __clz(m)) + 1; break; }
-  }
-}
-
 // the commas of [s, te): the first SF_MAX_FIELDS positions (relative to s) into sc; -> their count (all of them).
 // Warp-uniform.
 __device__ __forceinline__ int sf_commas(const uint8_t* t, int64_t s, int64_t te, int* sc) {
@@ -198,29 +181,21 @@ __global__ void __launch_bounds__(SF_THREADS) sf_map_parse_kernel(const uint8_t*
 __global__ void __launch_bounds__(SF_THREADS) sf_map_insert_kernel(const uint8_t* __restrict__ t, SfMapLines L,
                                                                   SfMap M, int64_t* info) {
   const int64_t n_lines = info[0];
-  const int64_t probes = M.cap < SF_MAX_PROBE ? M.cap : SF_MAX_PROBE;
   for (int64_t row = (int64_t)blockIdx.x * SF_THREADS + threadIdx.x; row < n_lines;
        row += (int64_t)gridDim.x * SF_THREADS) {
     const int c = L.col[row];
     if (c < 0) continue;
     const int64_t vs = L.vs[row], ve = L.ve[row];
-    uint64_t slot = __umul64hi(sf_hash(c, t, vs, ve), (uint64_t)M.cap);
-    bool done = false;
-    for (int64_t i = 0; i < probes && !done; ++i) {
-      uint64_t r = *reinterpret_cast<volatile uint64_t*>(M.ref + slot);
-      if (r == 0) {
-        r = atomicCAS(reinterpret_cast<unsigned long long*>(M.ref + slot), 0ull, (unsigned long long)(row + 1));
-        if (r == 0) r = (uint64_t)(row + 1);
-      }
-      const int64_t o = (int64_t)r - 1;
-      if (L.col[o] == c && L.ve[o] - L.vs[o] == ve - vs && sf_same(t + L.vs[o], t + vs, ve - vs)) {
-        atomicMax(reinterpret_cast<long long*>(M.win + slot), (long long)row);
-        done = true;
-      }
-      if (++slot == (uint64_t)M.cap) slot = 0;
+    const int64_t slot = probe(sf_hash(c, t, vs, ve), M.cap, [&](uint64_t s) {
+      const int64_t o = (int64_t)claim(M.ref + s, (uint64_t)(row + 1)) - 1;   // the key's first line
+      return L.col[o] == c && L.ve[o] - L.vs[o] == ve - vs && sf_same(t + L.vs[o], t + vs, ve - vs);
+    });
+    if (slot < 0) {
+      atomicAdd(reinterpret_cast<unsigned long long*>(&info[2]), 1ull);
+    } else {
+      atomicMax(reinterpret_cast<long long*>(M.win + slot), (long long)row);
+      atomicAdd(reinterpret_cast<unsigned long long*>(&info[1]), 1ull);
     }
-    if (!done) atomicAdd(reinterpret_cast<unsigned long long*>(&info[2]), 1ull);
-    else atomicAdd(reinterpret_cast<unsigned long long*>(&info[1]), 1ull);
   }
 }
 
@@ -240,18 +215,14 @@ __global__ void __launch_bounds__(SF_THREADS) sf_map_fill_kernel(SfMapLines L, S
 // fid span of the key (col, v[0, n)) -> (off, len) in the map text; false = absent (the reference's None)
 __device__ bool sf_map_find(const SfMap& M, const uint8_t* map_text, int col, const uint8_t* v, int64_t n,
                             int64_t& off, int32_t& flen) {
-  uint64_t slot = __umul64hi(sf_hash(col, v, 0, n), (uint64_t)M.cap);
-  const int64_t probes = M.cap < SF_MAX_PROBE ? M.cap : SF_MAX_PROBE;
-  for (int64_t i = 0; i < probes; ++i) {
-    if (M.ref[slot] == 0) return false;
-    if (M.col[slot] == col && M.vlen[slot] == n && sf_same(map_text + M.voff[slot], v, n)) {
-      off = M.foff[slot];
-      flen = M.flen[slot];
-      return true;
-    }
-    if (++slot == (uint64_t)M.cap) slot = 0;
-  }
-  return false;
+  bool hit = false;
+  probe(sf_hash(col, v, 0, n), M.cap, [&](uint64_t s) {
+    if (M.ref[s] == 0) return true;
+    hit = M.col[s] == col && M.vlen[s] == n && sf_same(map_text + M.voff[s], v, n);
+    if (hit) { off = M.foff[s]; flen = M.flen[s]; }
+    return hit;
+  });
+  return hit;
 }
 
 // col_fid int64[2 * 128]: per column the fid span of its bare name (continuous) or of name|UNK (categorical),
@@ -323,7 +294,7 @@ __global__ void __launch_bounds__(SF_THREADS) sf_emit_kernel(const uint8_t* __re
     int64_t p, e;
     line_bounds(line_start, nn, len, row, p, e);
     SfFields F;
-    sf_strip(t, p, e, F.s, F.te);
+    warp_strip(t, p, e, F.s, F.te);
     F.sc = sc;
     F.nc = sf_commas(t, F.s, F.te, sc);
     if (F.nc >= SF_MAX_FIELDS) {                       // CSV_COLUMNS[128] raises: the line is dropped
@@ -367,7 +338,7 @@ __global__ void __launch_bounds__(SF_THREADS) fr_emit_kernel(const uint8_t* __re
   for (int64_t row = (int64_t)blockIdx.x * SF_WARPS + (threadIdx.x >> 5); row < n_lines; row += warps) {
     int64_t p, e, s, te;
     line_bounds(line_start, nn, len, row, p, e);
-    sf_strip(t, p, e, s, te);
+    warp_strip(t, p, e, s, te);
     int64_t sp = te;                                   // the first ' ' of the stripped line
     for (int64_t w = s; w < te; w += 32) {
       const int64_t q = w + lane;
@@ -451,25 +422,14 @@ __device__ __forceinline__ bool sf_key_at(const uint8_t* src, const uint8_t* v, 
 
 __device__ bool sf_build_insert(const SfBuild& B, const uint8_t* t, const uint8_t* arena, int col, int64_t fs,
                                 int64_t fe, uint64_t npos) {
-  uint64_t slot = __umul64hi(sf_hash(col, t, fs, fe), (uint64_t)B.cap);
-  const int64_t probes = B.cap < SF_MAX_PROBE ? B.cap : SF_MAX_PROBE;
   const uint64_t mine = SF_PENDING | ((uint64_t)col << 56) | (uint64_t)fs;
-  for (int64_t i = 0; i < probes; ++i) {
-    uint64_t r = *reinterpret_cast<volatile uint64_t*>(B.ref + slot);
-    if (r == 0) {
-      r = atomicCAS(reinterpret_cast<unsigned long long*>(B.ref + slot), 0ull, (unsigned long long)mine);
-      if (r == 0) r = mine;
-    }
-    if ((int)((r >> 56) & 0x7F) == col) {
-      const uint8_t* src = (r & SF_PENDING ? t : arena) + (r & SF_OFF_MASK);
-      if (sf_key_at(src, t + fs, fe - fs)) {
-        atomicMax(reinterpret_cast<unsigned long long*>(B.npos + slot), (unsigned long long)npos);
-        return true;
-      }
-    }
-    if (++slot == (uint64_t)B.cap) slot = 0;
-  }
-  return false;
+  const int64_t slot = probe(sf_hash(col, t, fs, fe), B.cap, [&](uint64_t s) {
+    const uint64_t r = claim(B.ref + s, mine);   // where the slot's key was first seen
+    return (int)((r >> 56) & 0x7F) == col &&
+           sf_key_at((r & SF_PENDING ? t : arena) + (r & SF_OFF_MASK), t + fs, fe - fs);
+  });
+  if (slot >= 0) atomicMax(reinterpret_cast<unsigned long long*>(B.npos + slot), (unsigned long long)npos);
+  return slot >= 0;
 }
 
 // one warp per line; info = {lines, keys that found no slot}
@@ -489,7 +449,7 @@ __global__ void __launch_bounds__(SF_THREADS) sf_build_insert_kernel(const uint8
     int64_t p, e;
     line_bounds(line_start, nn, len, row, p, e);
     SfFields F;
-    sf_strip(t, p, e, F.s, F.te);
+    warp_strip(t, p, e, F.s, F.te);
     F.sc = sc;
     F.nc = sf_commas(t, F.s, F.te, sc);
     // columns 1 .. len - 2, and at most 127: a longer line has inserted those when CSV_COLUMNS[128] raises
@@ -675,7 +635,7 @@ int ctr_smart_map_build(const char* map_text, size_t map_len, void* table, int64
                         int64_t* info, void* ws, size_t ws_bytes, ctr_stream_t stream) {
   CTR_REQUIRE(table && capacity > 0 && col_fid && info && (map_len == 0 || map_text), CTR_ERR_INVALID_ARG,
               "ctr_smart_map_build: bad arguments");
-  CTR_REQUIRE(capacity <= SF_MAX_CAP, CTR_ERR_INVALID_ARG, "ctr_smart_map_build: capacity > 2^31");
+  CTR_REQUIRE(capacity <= KT_MAX_CAP, CTR_ERR_INVALID_ARG, "ctr_smart_map_build: capacity > 2^31");
   CTR_REQUIRE(map_len < SF_MAX_LEN, CTR_ERR_INVALID_ARG, "ctr_smart_map_build: map too large (len < 2^30)");
   CTR_REQUIRE(ws && ws_bytes >= ctr_smart_map_workspace_bytes(map_len), CTR_ERR_WORKSPACE,
               "ctr_smart_map_build: workspace too small");
@@ -703,7 +663,7 @@ size_t ctr_smart_emit_workspace_bytes(size_t len) { return SfLinesWs(nullptr, le
 
 static int sf_emit_args(const char* map_text, const void* table, int64_t capacity, const int64_t* col_fid,
                         SfEmitArgs& a) {
-  CTR_REQUIRE(table && capacity > 0 && capacity <= SF_MAX_CAP && col_fid, CTR_ERR_INVALID_ARG,
+  CTR_REQUIRE(table && capacity > 0 && capacity <= KT_MAX_CAP && col_fid, CTR_ERR_INVALID_ARG,
               "ctr_smart_emit: bad arguments");
   a = SfEmitArgs{SfMap(const_cast<void*>(table), capacity), reinterpret_cast<const uint8_t*>(map_text), col_fid};
   return CTR_OK;
@@ -757,7 +717,7 @@ int ctr_smart_build_insert(const char* text, size_t len, int64_t line_base, void
   CTR_REQUIRE(table && capacity > 0 && arena && arena_bytes > 0 && state && info && line_base >= 0 &&
                   (len == 0 || text),
               CTR_ERR_INVALID_ARG, "ctr_smart_build_insert: bad arguments");
-  CTR_REQUIRE(capacity <= SF_MAX_CAP, CTR_ERR_INVALID_ARG, "ctr_smart_build_insert: capacity > 2^31");
+  CTR_REQUIRE(capacity <= KT_MAX_CAP, CTR_ERR_INVALID_ARG, "ctr_smart_build_insert: capacity > 2^31");
   CTR_REQUIRE(len < SF_MAX_LEN, CTR_ERR_INVALID_ARG, "ctr_smart_build_insert: chunk too large (len < 2^30)");
   CTR_REQUIRE(ws && ws_bytes >= ctr_smart_build_insert_workspace_bytes(len), CTR_ERR_WORKSPACE,
               "ctr_smart_build_insert: workspace too small");
@@ -782,7 +742,7 @@ int ctr_smart_build_finish(const void* table, int64_t capacity, const uint8_t* a
                            int64_t* info, void* ws, size_t ws_bytes, ctr_stream_t stream) {
   CTR_REQUIRE(table && capacity > 0 && arena && state && info, CTR_ERR_INVALID_ARG,
               "ctr_smart_build_finish: bad arguments");
-  CTR_REQUIRE(capacity <= SF_MAX_CAP, CTR_ERR_INVALID_ARG, "ctr_smart_build_finish: capacity > 2^31");
+  CTR_REQUIRE(capacity <= KT_MAX_CAP, CTR_ERR_INVALID_ARG, "ctr_smart_build_finish: capacity > 2^31");
   CTR_REQUIRE(ws && ws_bytes >= ctr_smart_build_workspace_bytes(capacity), CTR_ERR_WORKSPACE,
               "ctr_smart_build_finish: workspace too small");
   cudaStream_t st = as_stream(stream);
@@ -808,7 +768,7 @@ int ctr_smart_build_finish(const void* table, int64_t capacity, const uint8_t* a
 
 int ctr_smart_build_render(const void* table, int64_t capacity, const uint8_t* arena, char* out, const void* ws,
                            size_t ws_bytes, ctr_stream_t stream) {
-  CTR_REQUIRE(table && capacity > 0 && capacity <= SF_MAX_CAP && arena && out, CTR_ERR_INVALID_ARG,
+  CTR_REQUIRE(table && capacity > 0 && capacity <= KT_MAX_CAP && arena && out, CTR_ERR_INVALID_ARG,
               "ctr_smart_build_render: bad arguments");
   CTR_REQUIRE(ws && ws_bytes >= ctr_smart_build_workspace_bytes(capacity), CTR_ERR_WORKSPACE,
               "ctr_smart_build_render: workspace too small");
