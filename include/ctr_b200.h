@@ -717,6 +717,24 @@ size_t ctr_crc32c_workspace_bytes(int n, int64_t total_bytes);
 int ctr_crc32c_ranges(const int64_t* ranges, int n, int64_t total_bytes, uint32_t* crc, uint32_t* masked, void* ws,
                       size_t ws_bytes, ctr_stream_t stream);
 
+/* ---- eval / infer scoring (DESIGN.md §2.13) --------------------------------------------------------------------------
+ * auc_counts (tf.metrics.auc's 200-threshold confusion counts, DeepFM.py:194, DeepCvrMTL.py:229-233): pred, label f32
+ *   [n], n < 2^40; thresholds f32 [200] ascending.  counts int64 [2][201] += per class (row 0: label == 0, row 1:
+ *   label != 0, a NaN label included) the histogram of k = #{t : t < pred}; a NaN pred has k = 200, and a pred equal to
+ *   a threshold is not above it.  Suffix sums of row 1 (row 0) from k = i + 1 are tf's tp (fp) at threshold i.  Exact
+ *   and independent of order; the caller zeroes counts once and accumulates over calls.
+ * format_preds (pred.txt, DeepFM.py:351-353): appends row r's "%f\n" % a[r] (b NULL) or "%f\t%f\n" % (a[r], b[r]) for
+ *   r < n at out[*offset, ...), the bytes of Python's "%f" % float(x) for every float32 (nan, inf, -inf, -0.000000,
+ *   subnormals, FLT_MAX), and advances *offset (device int64) by the bytes of the rows.  A row is at most 48 bytes
+ *   per column.  Bytes at or past out_bytes are not written (*offset still advances: *offset > out_bytes after the call
+ *   means the buffer was too small).  ws = ctr_format_preds_workspace_bytes(n) bytes.
+ * n = 0 is a no-op; no allocation and no synchronisation inside. */
+int ctr_auc_counts(const float* pred, const float* label, int64_t n, const float* thresholds, int64_t* counts,
+                   ctr_stream_t stream);
+size_t ctr_format_preds_workspace_bytes(int64_t n);
+int ctr_format_preds(const float* a, const float* b, int64_t n, char* out, int64_t out_bytes, int64_t* offset,
+                     void* ws, size_t ws_bytes, ctr_stream_t stream);
+
 /* ---- table initialisation (glorot_normal_initializer, DeepFM.py:115-116; truncated at 2 sigma) --- */
 int ctr_init_trunc_normal(float* t, int64_t n, float stddev, uint64_t seed, ctr_stream_t stream);
 int ctr_fill(float* t, int64_t n, float value, ctr_stream_t stream);

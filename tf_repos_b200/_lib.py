@@ -159,6 +159,9 @@ SIGNATURES = {
     "ctr_frappe_write": (c_int, [P, c_size_t, P, P, c_size_t, P]),
     "ctr_crc32c_workspace_bytes": (c_size_t, [c_int, c_int64]),
     "ctr_crc32c_ranges": (c_int, [P, c_int, c_int64, P, P, P, c_size_t, P]),
+    "ctr_auc_counts": (c_int, [P, P, c_int64, P, P, P]),
+    "ctr_format_preds_workspace_bytes": (c_size_t, [c_int64]),
+    "ctr_format_preds": (c_int, [P, P, c_int64, P, c_int64, P, P, c_size_t, P]),
     "ctr_init_trunc_normal": (c_int, [P, c_int64, c_float, c_uint64, P]),
     "ctr_fill": (c_int, [P, c_int64, c_float, P]),
 }

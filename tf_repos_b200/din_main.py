@@ -26,8 +26,9 @@ from typing import Dict, Iterator, List, Sequence, Tuple
 import numpy as np
 import torch
 
-from .estimator import auc_200, restore_checkpoint, save_checkpoint
+from .estimator import restore_checkpoint, save_checkpoint
 from .flags import FLAGS
+from .scoring import AucCounts, PredWriter
 from .tfrecord import parse_example, read_records
 
 U_FIELDS = ("cat", "shop", "brand", "int")
@@ -158,19 +159,18 @@ def run():
                 update_mode=FLAGS.update_mode, batch_norm=FLAGS.batch_norm, batch_norm_decay=FLAGS.batch_norm_decay)
     restore_checkpoint(model, FLAGS.model_dir)
 
-    def score(d) -> Tuple[np.ndarray, np.ndarray]:
-        preds, labs = [], []
-        for batch, labels, n in d.batches(1, B, "din", P):
-            preds.append(model.predict(batch)[:n].cpu().numpy().copy()); labs.append(labels[:n].cpu().numpy())
-        model.check_ids()
-        return (np.concatenate(preds), np.concatenate(labs)) if preds else (np.zeros(0, np.float32), np.zeros(0, np.float32))
-
     def evaluate(d):
-        p, t = score(d)
-        if not len(p):
+        auc, preds, labs = AucCounts(model.device), [], []
+        for batch, labels, n in d.batches(1, B, "din", P):
+            p = model.predict(batch)[:n]
+            auc.add(p, labels[:n])
+            preds.append(p.clone()); labs.append(labels[:n])        # the loss: one copy at the end
+        model.check_ids()
+        if not preds:
             return {}
+        p, t = torch.cat(preds).cpu().numpy(), torch.cat(labs).cpu().numpy()
         pc = np.clip(p.astype(np.float64), 1e-12, 1 - 1e-12)
-        return {"auc": auc_200(t, p), "loss_ce": float(-(t * np.log(pc) + (1 - t) * np.log(1 - pc)).mean()),
+        return {"auc": auc.auc()[0], "loss_ce": float(-(t * np.log(pc) + (1 - t) * np.log(1 - pc)).mean()),
                 "global_step": model.global_step}
 
     if FLAGS.task_type == "train":
@@ -192,10 +192,10 @@ def run():
     elif FLAGS.task_type == "eval":
         print(json.dumps(evaluate(te)))
     elif FLAGS.task_type == "infer":
-        p, _ = score(te)
-        with open(FLAGS.data_dir + "/pred.txt", "w") as fo:
-            for prob in p:
-                fo.write("%f\n" % prob)
+        # check_ids before any line reaches the file: a bad id leaves pred.txt as it was
+        with PredWriter(FLAGS.data_dir + "/pred.txt", model.device, check=model.check_ids) as fo:
+            for batch, _, n in te.batches(1, B, "din", P):
+                fo.add(model.predict(batch)[:n])
     elif FLAGS.task_type == "export":
         out_dir = os.path.join(FLAGS.servable_model_dir, str(int(time.time())))
         os.makedirs(out_dir, exist_ok=True)

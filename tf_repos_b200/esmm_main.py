@@ -24,8 +24,9 @@ import numpy as np
 import torch
 
 from .din_main import U_FIELDS, decode_tfrecord_files, index_stream
-from .estimator import auc_200, restore_checkpoint, save_checkpoint
+from .estimator import restore_checkpoint, save_checkpoint
 from .flags import FLAGS
+from .scoring import AucCounts, PredWriter
 
 BAG_KEYS = tuple("u_%sids" % f for f in U_FIELDS) + ("a_int",)
 
@@ -126,22 +127,16 @@ def run():
     restore_checkpoint(model, FLAGS.model_dir)
     dev = model.device
 
-    def score(d, with_loss: bool):
-        out, losses = {"pctr": [], "pcvr": [], "pctcvr": [], "y": [], "z": []}, []
-        for batch, (y, z), n in d.batches(1, B, "esmm"):
-            p = model.predict(batch, (y, z) if with_loss else None, n)
-            for k, v in zip(("pctr", "pcvr", "pctcvr"), p):
-                out[k].append(v[:n].cpu().numpy().copy())
-            out["y"].append(y[:n].cpu().numpy()); out["z"].append(z[:n].cpu().numpy())
-            if with_loss:
-                losses.append(model.losses.tolist())
-        model.check_ids()
-        return {k: (np.concatenate(v) if v else np.zeros(0, np.float32)) for k, v in out.items()}, losses
-
     def evaluate(d):
-        s, losses = score(d, True)
-        if not len(s["y"]):
+        auc, losses = AucCounts(dev, heads=3), []
+        for batch, (y, z), n in d.batches(1, B, "esmm"):
+            pctr, pcvr, pctcvr = model.predict(batch, (y, z), n)
+            auc.add(pctr[:n], y[:n], 0); auc.add(pcvr[:n], z[:n], 1); auc.add(pctcvr[:n], z[:n], 2)
+            losses.append(model.losses.clone())                # one copy at the end
+        model.check_ids()
+        if not losses:
             return {}
+        losses = torch.stack(losses).tolist()
         reg = torch.zeros(1, dtype=torch.float32, device=dev)
         V = model.variables()["embeddings"]
         ws = torch.empty(max(int(_lib.raw().ctr_l2_loss_workspace_bytes(V.numel())), 16), dtype=torch.uint8, device=dev)
@@ -149,8 +144,9 @@ def run():
         l2 = float(reg.item())
         # tf.metrics.mean of the per-batch loss (:223), and the three AUCs of :229-233
         loss = float(np.mean([model.w_ctr * c + model.w_cvr * v + l2 for c, v in losses]))
-        return {"loss": loss, "CTR_AUC": auc_200(s["y"], s["pctr"]), "CVR_AUC": auc_200(s["z"], s["pcvr"]),
-                "CTCVR_AUC": auc_200(s["z"], s["pctcvr"]), "global_step": model.global_step}
+        ctr_auc, cvr_auc, ctcvr_auc = auc.auc()
+        return {"loss": loss, "CTR_AUC": ctr_auc, "CVR_AUC": cvr_auc, "CTCVR_AUC": ctcvr_auc,
+                "global_step": model.global_step}
 
     if FLAGS.task_type == "train":
         t0, s0, last = time.time(), model.global_step, None
@@ -173,8 +169,9 @@ def run():
     elif FLAGS.task_type == "infer":
         # DeepCvrMTL.py:379-382 asks Estimator.predict for predict_keys="prob", a key the predictions dict does not
         # have (TF raises before the first line, quirk Q10); this writes what the loop evidently intends
-        s, _ = score(te, False)
-        with open(FLAGS.data_dir + "/pred.txt", "w") as fo:
-            for pctr, pcvr in zip(s["pctr"], s["pcvr"]):
-                fo.write("%f\t%f\n" % (pctr, pcvr))
+        # check_ids before any line reaches the file: a bad id leaves pred.txt as it was
+        with PredWriter(FLAGS.data_dir + "/pred.txt", dev, columns=2, check=model.check_ids) as fo:
+            for batch, _, n in te.batches(1, B, "esmm"):
+                pctr, pcvr, _ = model.predict(batch, None, n)
+                fo.add(pctr[:n], pcvr[:n])
     return model

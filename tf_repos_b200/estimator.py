@@ -22,24 +22,34 @@ from .flags import FLAGS, input_parse_device
 from .input_fn import input_fn
 
 
-def auc_200(labels: np.ndarray, preds: np.ndarray) -> float:
-    """tf.metrics.auc(labels, pred) defaults (DeepFM.py:194) [TF-sem]: 200 thresholds, trapezoidal ROC."""
+def auc_thresholds() -> np.ndarray:
+    """tf.metrics.auc's 200 thresholds (num_thresholds default, DeepFM.py:194) [TF-sem], float32 ascending."""
     n = 200
     eps = 1e-7
-    thr = np.array([0.0 - eps] + [(i + 1) / (n - 1) for i in range(n - 2)] + [1.0 + eps], dtype=np.float32)
+    return np.array([0.0 - eps] + [(i + 1) / (n - 1) for i in range(n - 2)] + [1.0 + eps], dtype=np.float32)
+
+
+def auc_from_counts(tp: np.ndarray, fp: np.ndarray, fn: np.ndarray, tn: np.ndarray) -> float:
+    """tf.metrics.auc's trapezoidal ROC from the float32 confusion counts at its 200 thresholds."""
+    n = len(tp)
+    e = np.float32(1e-6)
+    rec = (tp + e) / (tp + fn + e)
+    fpr = fp / (fp + tn + e)
+    return float(np.sum((fpr[: n - 1] - fpr[1:]) * (rec[: n - 1] + rec[1:]) / 2.0))
+
+
+def auc_200(labels: np.ndarray, preds: np.ndarray) -> float:
+    """tf.metrics.auc(labels, pred) defaults (DeepFM.py:194) [TF-sem]: 200 thresholds, trapezoidal ROC.  The host
+    reference of scoring.AucCounts, which gets the same counts from a device histogram."""
+    thr = auc_thresholds()
     lab = labels.astype(bool)
-    order = np.sort(preds.astype(np.float32))
     pos_sorted = np.sort(preds[lab].astype(np.float32))
     neg_sorted = np.sort(preds[~lab].astype(np.float32))
     tp = (len(pos_sorted) - np.searchsorted(pos_sorted, thr, side="right")).astype(np.float32)
     fp = (len(neg_sorted) - np.searchsorted(neg_sorted, thr, side="right")).astype(np.float32)
     fn = len(pos_sorted) - tp
     tn = len(neg_sorted) - fp
-    e = np.float32(1e-6)
-    rec = (tp + e) / (tp + fn + e)
-    fpr = fp / (fp + tn + e)
-    del order
-    return float(np.sum((fpr[: n - 1] - fpr[1:]) * (rec[: n - 1] + rec[1:]) / 2.0))
+    return auc_from_counts(tp, fp, fn, tn)
 
 
 def _ckpt_path(model_dir: str) -> str:
@@ -137,18 +147,18 @@ def run(build_model: Callable[[], object], model_name: str):
                    feats["feat_vals"].reshape(-1, F).to(dev, non_blocking=True), labels.to(dev, non_blocking=True))
 
     def evaluate(files) -> Dict[str, float]:
-        preds, labs, losses = [], [], []
+        from .scoring import AucCounts
+        auc, logits, labs = AucCounts(dev), [], []
         for ids, vals, labels in batches(files, 1):
-            p = model.predict(ids, vals)
-            y = model.y[: ids.shape[0]].cpu().numpy().astype(np.float64)
-            t = labels.cpu().numpy()
-            losses.append(np.maximum(y, 0) - y * t + np.log1p(np.exp(-np.abs(y))))        # metric only, on the host
-            preds.append(p.cpu().numpy().copy()); labs.append(t)
+            auc.add(model.predict(ids, vals), labels)
+            logits.append(model.y[: ids.shape[0]].clone()); labs.append(labels)     # the loss: one copy at the end
         model.check_ids()
-        if not preds:
+        if not logits:
             return {}
-        preds, labs = np.concatenate(preds), np.concatenate(labs)
-        return {"auc": auc_200(labs, preds), "loss_ce": float(np.concatenate(losses).mean()), "global_step": model.global_step}
+        y = torch.cat(logits).cpu().numpy().astype(np.float64)
+        t = torch.cat(labs).cpu().numpy()
+        loss = np.maximum(y, 0) - y * t + np.log1p(np.exp(-np.abs(y)))         # metric only, on the host
+        return {"auc": auc.auc()[0], "loss_ce": float(loss.mean()), "global_step": model.global_step}
 
     if FLAGS.task_type == "train":
         t0, s0 = time.time(), model.global_step
@@ -177,10 +187,10 @@ def run(build_model: Callable[[], object], model_name: str):
     elif FLAGS.task_type == "eval":
         print(json.dumps(evaluate(va_files)))
     elif FLAGS.task_type == "infer":
-        with open(FLAGS.data_dir + "/pred.txt", "w") as fo:                  # DeepFM.py:351-353
+        from .scoring import PredWriter
+        with PredWriter(FLAGS.data_dir + "/pred.txt", dev) as fo:              # DeepFM.py:351-353
             for ids, vals, _ in batches(te_files, 1):
-                for prob in model.predict(ids, vals).cpu().tolist():
-                    fo.write("%f\n" % prob)
+                fo.add(model.predict(ids, vals))
         model.check_ids()
     elif FLAGS.task_type == "export":
         out_dir = os.path.join(FLAGS.servable_model_dir, str(int(time.time())))

@@ -761,3 +761,33 @@ def crc32c(tensors, crc=None, masked=None, ws=None):
                                _p(masked, torch.int32, "masked"), _p(ws, torch.uint8, "ws"), ws.numel(), _stream()),
           "ctr_crc32c_ranges")
     return crc, masked
+
+
+def auc_counts(pred, label, thresholds, counts):
+    """counts int64 [2, 201] += tf.metrics.auc's per-class histogram of #{t in thresholds : t < pred} (row 0: label 0,
+    row 1: label != 0 or NaN); a NaN pred counts above every threshold.  pred, label f32 [n]; thresholds f32 [200]."""
+    n = pred.numel()
+    if label.numel() != n:
+        raise CtrError(f"auc_counts: {n} predictions, {label.numel()} labels")
+    if thresholds.numel() != 200 or counts.numel() != 2 * 201:
+        raise CtrError("auc_counts: thresholds must be f32 [200] and counts int64 [2, 201]")
+    check(_L.ctr_auc_counts(_p(pred, torch.float32, "pred"), _p(label, torch.float32, "label"), n,
+                            _p(thresholds, torch.float32, "thresholds"), _p(counts, torch.int64, "counts"), _stream()),
+          "ctr_auc_counts")
+
+
+def format_preds_workspace_bytes(n: int) -> int:
+    return int(_L.ctr_format_preds_workspace_bytes(n))
+
+
+def format_preds(a, b, out, offset, ws):
+    """Appends "%f\\n" % a[r] (b None) or "%f\\t%f\\n" % (a[r], b[r]) for every row to the uint8 device buffer out at
+    the device int64 offset[0], and advances offset[0]; Python's "%f" bytes for every float32.  Bytes past the end of
+    out are not written, offset still advances: offset[0] > out.numel() means out was too small."""
+    n = a.numel()
+    if b is not None and b.numel() != n:
+        raise CtrError(f"format_preds: columns of {n} and {b.numel()} rows")
+    check(_L.ctr_format_preds(_p(a, torch.float32, "a"), _p(b, torch.float32, "b"), n, _p(out, torch.uint8, "out"),
+                              out.numel(), _p(offset, torch.int64, "offset"), _p(ws, torch.uint8, "ws"), ws.numel(),
+                              _stream()),
+          "ctr_format_preds")

@@ -21,8 +21,8 @@ import numpy as np
 import torch
 
 from . import ops, text_chunks
-from .estimator import auc_200
 from .flags import FLAGS, input_parse_device
+from .scoring import AucCounts, PredWriter
 
 N_NUM, N_CAT = 13, 26
 
@@ -169,14 +169,16 @@ def run():
             yield batch if parse_dev is not None else tuple(t.to(dev) for t in batch)
 
     def evaluate(files):
-        preds, labs = [], []
+        auc, preds, labs = AucCounts(dev), [], []
         for dense, cat, labels in batches(files, 1):
-            preds.append(model.predict(dense, cat).cpu().numpy().copy()); labs.append(labels.cpu().numpy())
+            p = model.predict(dense, cat)
+            auc.add(p, labels)
+            preds.append(p.clone()); labs.append(labels)            # the loss: one copy at the end
         if not preds:
             return {}
-        p, t = np.concatenate(preds), np.concatenate(labs)
+        p, t = torch.cat(preds).cpu().numpy(), torch.cat(labs).cpu().numpy()
         pc = np.clip(p.astype(np.float64), 1e-12, 1 - 1e-12)
-        return {"auc": auc_200(t, p), "average_loss": float(-(t * np.log(pc) + (1 - t) * np.log(1 - pc)).mean()),
+        return {"auc": auc.auc()[0], "average_loss": float(-(t * np.log(pc) + (1 - t) * np.log(1 - pc)).mean()),
                 "global_step": model.global_step}
 
     if FLAGS.task_type == "train":
@@ -194,10 +196,9 @@ def run():
         if va_files:
             print("INFO:Saving dict for global step %d: %s" % (model.global_step, json.dumps(evaluate(va_files))))
     elif FLAGS.task_type == "predict":
-        with open(FLAGS.data_dir + "/pred.txt", "w") as fo:
+        with PredWriter(FLAGS.data_dir + "/pred.txt", dev) as fo:
             for dense, cat, _ in batches(te_files, 1):
-                for prob in model.predict(dense, cat).cpu().numpy():
-                    fo.write("%f\n" % prob)
+                fo.add(model.predict(dense, cat))
     elif FLAGS.task_type == "export_model":
         os.makedirs(FLAGS.servable_model_dir, exist_ok=True)
         torch.save({"variables": {k: v.detach().cpu().clone() for k, v in model.variables().items()},
