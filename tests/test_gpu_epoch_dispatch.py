@@ -74,14 +74,15 @@ def _oracle_step(opt_name, var, slots, G, lr, adam):
 
 
 def _extreme(shape, gen, nonneg=False):
-    """A mix of exact zeros, denormals, values just above FLT_MIN and (a quarter) ordinary values."""
-    r = torch.randint(0, 4, shape, generator=gen)
-    sgn = torch.where(torch.rand(shape, generator=gen) < 0.5, -1.0, 1.0)
+    """A mix of exact zeros, denormals, values just above FLT_MIN and (a quarter) ordinary values, on gen's device."""
+    d = gen.device
+    r = torch.randint(0, 4, shape, generator=gen, device=d)
+    sgn = torch.where(torch.rand(shape, generator=gen, device=d) < 0.5, -1.0, 1.0)
     fmin = float(np.finfo(np.float32).tiny)
-    den = torch.randint(1, 1 << 22, shape, generator=gen).double() * 2.0 ** -149
-    near = fmin * (1.0 + 3.0 * torch.rand(shape, generator=gen).double())
-    ordinary = torch.randn(shape, generator=gen).double() * 0.1
-    x = torch.where(r == 0, torch.zeros(shape, dtype=torch.float64),
+    den = torch.randint(1, 1 << 22, shape, generator=gen, device=d).double() * 2.0 ** -149
+    near = fmin * (1.0 + 3.0 * torch.rand(shape, generator=gen, device=d).double())
+    ordinary = torch.randn(shape, generator=gen, device=d).double() * 0.1
+    x = torch.where(r == 0, torch.zeros(shape, dtype=torch.float64, device=d),
                     torch.where(r == 1, den, torch.where(r == 2, near, ordinary)))
     x = x.float()
     return x.abs() if nonneg else x * sgn.float()
