@@ -578,6 +578,27 @@ int ctr_din_serve_scan(const void* data, const int64_t* offsets, int64_t n, int6
                        int max_a_int, int64_t* slot_off, int32_t* slot_len, int32_t* a_int_off, int32_t* maxima,
                        uint64_t* err, ctr_stream_t stream);
 
+/* ---- ESMM serving input (DeepCvrMTL.py:66-83 without labels, DeepCvrMTL.py:210-217; DESIGN.md §2.14) ------------
+ * One slice of a serving request, laid out as for ctr_din_serve_scan: n serialized tf.Examples, Example b =
+ * data[offsets[b], offsets[b+1]) (device bytes, offsets int64 [n+1], each Example < 2^31 bytes), 1 <= n <= B.  One warp
+ * per batch slot b < B walks its Example (slot b >= n repeats Example 0, as esmm_main.make_batch pads) with the scan's
+ * walk and checks, minus the CRC and the labels: y and z must be well formed but are neither required nor kind-checked.
+ * Writes
+ *   slot_off int64 [B], slot_len int32 [B]   the slot's bytes, for ctr_tfrecord_emit_esmm(data, slot_off, slot_len, ...)
+ *   bag_off int32 [5B+1]                     exclusive scan (one CTA, on the device) of the bag lengths in the emit's
+ *                                            field-major order: bag j*B + b = field j (u_catids, u_shopids, u_brandids,
+ *                                            u_intids, a_intids) of slot b
+ *   total int64 [1]                          the slice's occurrences (the sum of all 5B lengths, padding slots
+ *                                            included), written by the scan.  When it exceeds occ_capacity (< 2^31)
+ *                                            every bag_off entry is 0, so the emit writes no occurrence: the caller
+ *                                            grows its bag_ids / bag_wgt to total and runs the slice again
+ *   err                                      min-folded as ctr_tfrecord_scan's with (example_base + b) << 16, b < n;
+ *                                            checks 1-6 (no CRC), arg as there (check 2: keys 2-5 only)
+ * A rejected Example's lengths are 0.  No allocation and no synchronisation inside; graph-capturable. */
+int ctr_esmm_serve_scan(const void* data, const int64_t* offsets, int64_t n, int64_t example_base, int F, int B,
+                        int64_t occ_capacity, int64_t* slot_off, int32_t* slot_len, int32_t* bag_off, int64_t* total,
+                        uint64_t* err, ctr_stream_t stream);
+
 /* ---- Ali-CCP TFRecord writer (deep_ctr/Feature_pipeline/get_aliccp_tfrecord.py; DESIGN.md §2.6) ----------------
  * Joined Ali-CCP lines `id,y,z,field:fid:val ...` -> framed tf.Example records, byte-identical to
  * tfrecord.write_records(path, [tfrecord.encode_example(features) ...]) of the features gen_tfrecords builds.  `text` is

@@ -122,6 +122,7 @@ SIGNATURES = {
     "ctr_tfrecord_emit_din": (c_int, [P, P, P, c_int, c_int, c_int, P, P, P, P, P, P, P, P]),
     "ctr_tfrecord_emit_esmm": (c_int, [P, P, P, c_int, c_int, P, P, P, P, P, P, P, P]),
     "ctr_din_serve_scan": (c_int, [P, P, c_int64, c_int64, c_int, c_int, c_int, P, P, P, P, P, P]),
+    "ctr_esmm_serve_scan": (c_int, [P, P, c_int64, c_int64, c_int, c_int, c_int64, P, P, P, P, P, P]),
     "ctr_aliccp_workspace_bytes": (c_size_t, [c_size_t]),
     "ctr_aliccp_plan": (c_int, [P, c_size_t, c_int64, P, P, c_size_t, P]),
     "ctr_aliccp_declines": (c_int, [P, c_size_t, P, c_size_t, P, P]),

@@ -264,11 +264,37 @@ __global__ void __launch_bounds__(TR_THREADS) tr_emit_din_kernel(
   }
 }
 
-// DIN serving (DESIGN.md §2.10): one warp per batch slot b of a request slice; slot b >= n repeats Example 0, as
-// make_batch pads.  The walk and checks of tr_scan_kernel without framing, CRC or labels: y and z are parsed (they must be
-// well formed) and then dropped, so neither is required nor kind-checked.  Writes the slot's bytes for the emit, its
-// a_int bag length clamped to max_a_int (so the emit stays inside B * max_a_int ids) into a_int_off[b] for the scan,
-// and folds the unclamped longest behaviour list / a_int bag of the real Examples into maxima[0] / maxima[1].
+// A serving request's batch slot b (DESIGN.md §2.10, §2.14): Example b < n, or Example 0 for b >= n, as make_batch
+// pads; its bytes are data[s, s + L).  The walk and checks of tr_scan_kernel without framing, CRC or labels: y and z
+// are parsed (they must be well formed) and then dropped, so neither is required nor kind-checked.  -> the check word
+// (-1 = accepted); len = on lanes 0-4 the value count of u_catids, u_shopids, u_brandids, u_intids, a_intids (0 when
+// rejected), 0 elsewhere.
+__device__ __forceinline__ int tr_serve_slot(const uint8_t* data, const int64_t* offsets, int n, int b, int F,
+                                             TrSlot* slot, int64_t& s, int& L, int& len) {
+  const int lane = tr_lane();
+  const int e = b < n ? b : 0;
+  s = offsets[e];
+  L = (int)(offsets[e + 1] - s);
+  int word;
+  if (!tr_walk(data + s, L, slot, false, true)) {
+    word = TE_MALFORMED << 8;
+  } else {
+    if (lane == 0) slot[TK_Y].fs = -1;
+    __syncwarp();
+    word = tr_checks(slot, F, 0);
+  }
+  len = 0;
+  if (word < 0 && lane < 5) {
+    const int k = lane < 4 ? TK_UIDS + lane : TK_AINT;
+    len = slot[k].fs < 0 ? 0 : slot[k].r.count;
+  }
+  return word;
+}
+
+// DIN serving (DESIGN.md §2.10): one warp per batch slot b of a request slice (tr_serve_slot).  Writes the slot's bytes
+// for the emit, its a_int bag length clamped to max_a_int (so the emit stays inside B * max_a_int ids) into
+// a_int_off[b] for the scan, and folds the unclamped longest behaviour list / a_int bag of the real Examples into
+// maxima[0] / maxima[1].
 __global__ void __launch_bounds__(TR_THREADS) tr_din_serve_scan_kernel(
     const uint8_t* __restrict__ data, const int64_t* __restrict__ offsets, int n, int B, int64_t example_base, int F,
     int max_a_int, int64_t* __restrict__ slot_off, int32_t* __restrict__ slot_len, int32_t* __restrict__ a_int_off,
@@ -277,22 +303,9 @@ __global__ void __launch_bounds__(TR_THREADS) tr_din_serve_scan_kernel(
   const int lane = tr_lane(), wib = threadIdx.x >> 5;
   TrSlot* slot = slots[wib];
   for (int b = blockIdx.x * TR_WARPS + wib; b < B; b += gridDim.x * TR_WARPS) {
-    const int e = b < n ? b : 0;
-    const int64_t s = offsets[e];
-    const int L = (int)(offsets[e + 1] - s);
-    int word;
-    if (!tr_walk(data + s, L, slot, false, true)) {
-      word = TE_MALFORMED << 8;
-    } else {
-      if (lane == 0) slot[TK_Y].fs = -1;
-      __syncwarp();
-      word = tr_checks(slot, F, 0);
-    }
-    int len = 0;
-    if (word < 0 && lane < 5) {
-      const int k = lane < 4 ? TK_UIDS + lane : TK_AINT;
-      len = slot[k].fs < 0 ? 0 : slot[k].r.count;
-    }
+    int64_t s;
+    int L, len;
+    const int word = tr_serve_slot(data, offsets, n, b, F, slot, s, L, len);
     const int u_max = __reduce_max_sync(FULL_MASK, lane < 4 ? len : 0);
     const int a_len = __shfl_sync(FULL_MASK, len, 4);
     if (lane == 0) {
@@ -307,6 +320,39 @@ __global__ void __launch_bounds__(TR_THREADS) tr_din_serve_scan_kernel(
     }
     __syncwarp();
   }
+}
+
+// ESMM serving (DESIGN.md §2.14): one warp per batch slot b of a request slice (tr_serve_slot).  Writes the slot's
+// bytes for the emit and its five bag lengths field-major into bag_off[j * B + b]; slot 0 also zeroes bag_off[5B], so
+// that the scan's sum of all 5B + 1 entries is the slice's occurrence total.
+__global__ void __launch_bounds__(TR_THREADS) tr_esmm_serve_scan_kernel(
+    const uint8_t* __restrict__ data, const int64_t* __restrict__ offsets, int n, int B, int64_t example_base, int F,
+    int64_t* __restrict__ slot_off, int32_t* __restrict__ slot_len, int32_t* __restrict__ bag_off,
+    unsigned long long* __restrict__ err) {
+  __shared__ TrSlot slots[TR_WARPS][TR_KEYS];
+  const int lane = tr_lane(), wib = threadIdx.x >> 5;
+  TrSlot* slot = slots[wib];
+  for (int b = blockIdx.x * TR_WARPS + wib; b < B; b += gridDim.x * TR_WARPS) {
+    int64_t s;
+    int L, len;
+    const int word = tr_serve_slot(data, offsets, n, b, F, slot, s, L, len);
+    if (lane < 5) bag_off[(int64_t)lane * B + b] = len;
+    if (lane == 0) {
+      slot_off[b] = s;
+      slot_len[b] = L;
+      if (b == 0) bag_off[(int64_t)5 * B] = 0;
+      if (b < n && word >= 0) atomicMin(err, (unsigned long long)(example_base + b) << 16 | (unsigned)word);
+    }
+    __syncwarp();
+  }
+}
+
+// after the scan: a slice whose occurrence total exceeds the capacity gets empty bags, so the emit writes no
+// occurrence (the caller grows its buffers and runs the slice again)
+__global__ void __launch_bounds__(1024) tr_esmm_occ_clamp_kernel(int32_t* __restrict__ bag_off, int64_t W,
+                                                                  const int64_t* __restrict__ total, int64_t cap) {
+  if (*total <= cap) return;
+  for (int64_t i = threadIdx.x; i < W; i += blockDim.x) bag_off[i] = 0;
 }
 
 // make_batch of esmm_main (DeepCvrMTL.py:63-105): bags u_cat, u_shop, u_brand, u_int, a_int field-major, a_int's
@@ -384,6 +430,28 @@ int ctr_din_serve_scan(const void* data, const int64_t* offsets, int64_t n, int6
       static_cast<const uint8_t*>(data), offsets, (int)n, B, example_base, F, max_a_int, slot_off, slot_len, a_int_off,
       maxima, reinterpret_cast<unsigned long long*>(err));
   return cta_scan({a_int_off}, {nullptr}, nullptr, (int64_t)B + 1, st, "ctr_din_serve_scan");
+}
+
+int ctr_esmm_serve_scan(const void* data, const int64_t* offsets, int64_t n, int64_t example_base, int F, int B,
+                        int64_t occ_capacity, int64_t* slot_off, int32_t* slot_len, int32_t* bag_off, int64_t* total,
+                        uint64_t* err, ctr_stream_t stream) {
+  const char* fn = "ctr_esmm_serve_scan";
+  CTR_REQUIRE(data && offsets && n > 0 && n <= B && example_base >= 0 && F > 0 && occ_capacity >= 0 && slot_off &&
+                  slot_len && bag_off && total && err,
+              CTR_ERR_INVALID_ARG, "%s: bad arguments", fn);
+  CTR_REQUIRE(example_base + n < ((int64_t)1 << 47) && occ_capacity < ((int64_t)1 << 31) &&
+                  (int64_t)5 * B < ((int64_t)1 << 31),
+              CTR_ERR_INVALID_ARG, "%s: example index >= 2^47, occ_capacity >= 2^31 or 5B >= 2^31", fn);
+  cudaStream_t st = as_stream(stream);
+  const int64_t W = (int64_t)5 * B + 1;
+  tr_esmm_serve_scan_kernel<<<grid_for(B, TR_WARPS, 16), TR_THREADS, 0, st>>>(
+      static_cast<const uint8_t*>(data), offsets, (int)n, B, example_base, F, slot_off, slot_len, bag_off,
+      reinterpret_cast<unsigned long long*>(err));
+  CTR_LAUNCHED(fn);
+  if (int rc = cta_scan({bag_off}, {total}, nullptr, W, st, fn)) return rc;
+  tr_esmm_occ_clamp_kernel<<<1, 1024, 0, st>>>(bag_off, W, total, occ_capacity);
+  CTR_LAUNCHED(fn);
+  return CTR_OK;
 }
 
 int ctr_tfrecord_emit_esmm(const void* stage, const int64_t* slot_off, const int32_t* slot_len, int B, int F,

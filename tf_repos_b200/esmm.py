@@ -76,6 +76,18 @@ class ESMM(SparseModel):
         self._a = {}
         self.global_step = 0
 
+    def grow(self, occ_capacity: int):
+        """For inference: let the model take batches of up to occ_capacity bag occurrences (sizes never shrink).  The
+        forward reads the bags through bag_off and holds no occurrence-sized buffer of its own, so growing allocates
+        nothing and cannot fail half way; the caller sizes its bag_ids / bag_wgt.  The training buffers, sized to the
+        old capacity, are released: a grown model predicts but no longer trains.  Variables, optimizer slots and
+        batch-norm statistics stay."""
+        cap = max(self.cap, int(occ_capacity))
+        if cap == self.cap:
+            return
+        self.cap, self.n_total = cap, self.n_fixed + cap
+        self.ids_all = self.g_all = None
+
     # ---- plumbing -------------------------------------------------------------------------------------
     def variables(self) -> Dict[str, torch.Tensor]:
         self.flush()
@@ -135,6 +147,8 @@ class ESMM(SparseModel):
         caller; the losses are means over the n_valid real samples and the padded rows' logit gradients are exactly 0,
         so the step equals TensorFlow's step on the smaller batch (not with --batch_norm: the padded rows would enter
         the batch moments)."""
+        if self.ids_all is None:
+            raise RuntimeError("this ESMM grew its occurrence capacity for inference (ESMM.grow) and no longer trains")
         upd = self.updater
         self._stage_ids(batch)
         upd.begin_step()

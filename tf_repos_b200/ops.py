@@ -713,6 +713,20 @@ def din_serve_scan(data, offsets, example_base: int, F: int, B: int, max_a_int: 
                                 _p(err, torch.int64, "err"), _stream()), "ctr_din_serve_scan")
 
 
+def esmm_serve_scan(data, offsets, example_base: int, F: int, B: int, occ_capacity: int, slot_off, slot_len, bag_off,
+                    total, err):
+    """One serving slice of serialized tf.Examples data[offsets[b], offsets[b+1]) (uint8, offsets int64 [n+1], n <= B)
+    -> slot_off int64 [B], slot_len int32 [B] and bag_off int32 [5B+1] for tfrecord_emit_esmm; total int64 [1] = the
+    slice's occurrences (bag_off is all zeros when it exceeds occ_capacity); err int64 [1] (uint64 bits, ~0 = none) is
+    folded into."""
+    n = offsets.numel() - 1
+    check(_L.ctr_esmm_serve_scan(_p(data, torch.uint8, "data"), _p(offsets, torch.int64, "offsets"), n, example_base, F,
+                                 B, occ_capacity, _p(slot_off, torch.int64, "slot_off"),
+                                 _p(slot_len, torch.int32, "slot_len"), _p(bag_off, torch.int32, "bag_off"),
+                                 _p(total, torch.int64, "total"), _p(err, torch.int64, "err"), _stream()),
+          "ctr_esmm_serve_scan")
+
+
 def tfrecord_emit_esmm(stage, slot_off, slot_len, B, F, bag_off, feat_ids, a_ids, bag_ids, bag_wgt, y, z):
     check(_L.ctr_tfrecord_emit_esmm(_p(stage, torch.uint8, "stage"), _p(slot_off, torch.int64, "slot_off"),
                                     _p(slot_len, torch.int32, "slot_len"), B, F, _p(bag_off, torch.int32, "bag_off"),

@@ -22,12 +22,22 @@ feat_vals spec its signature.json declares cannot feed DIN, quirk Q6).
 
     s = Servable.load("./servable/1700000000")
     prob = s.predict([example_bytes, ...])       # float32 [n]
+
+ESMM (DeepCvrMTL.py) declares the serving signature PredictOutput({"pcvr", "pctr", "pctcvr"}) (:210-217), but its
+`--task_type=export` is a stub that writes nothing, so there is no export directory: a servable is built from the
+`model_dir` that `--task_type=train` leaves, with the hyperparameters passed as the reference's export would read them
+from its flags (DESIGN.md §2.14).  The request is serialized tf.Examples with the training schema of DeepCvrMTL.py:66-83
+(labels not read).
+
+    s = ESMMServable.load("./model_ckpt/20260922", field_size=11, feature_size=4519540, embedding_size=16,
+                          deep_layers="256,128")        # checkpoint_format="tf": a bundle from tf_checkpoint.save
+    out = s.predict([example_bytes, ...])        # {"pctr", "pcvr", "pctcvr"}: float32 [n] each
 """
 from __future__ import annotations
 
 import json
 import os
-from typing import Dict
+from typing import Dict, Optional
 
 import numpy as np
 import torch
@@ -63,22 +73,22 @@ def _build(model_name: str, p: Dict, batch_size: int, device):
 
 class _Requests:
     """The staging of a request of n serialized tf.Examples for the device parsers, in a pinned host buffer and a device
-    buffer that only grow:  prob f32 [n] (padded to 8 bytes) | error word | `extra` bytes | offsets int64 [n+1] | bytes.
-    `send` writes the error word ~0, zeroes the extra bytes and copies error word..bytes in one transfer; `receive`
-    copies prob..extra back in one transfer and waits for it."""
+    buffer that only grow:  prob f32 [outputs * n] (padded to 8 bytes) | error word | `extra` bytes | offsets int64
+    [n+1] | bytes.  `send` writes the error word ~0, zeroes the extra bytes and copies error word..bytes in one
+    transfer; `receive` copies prob..extra back in one transfer and waits for it."""
 
     def __init__(self, device):
         self.device = device
         self._host = self._dev = None
 
-    def send(self, examples, extra: int = 0):
-        """examples: n >= 1 serialized Examples -> their device views (prob f32 [n], err int64 [1], extra uint8,
-        offsets int64 [n+1], data uint8).  Raises ValueError for an Example of 2^31 bytes or more."""
+    def send(self, examples, extra: int = 0, outputs: int = 1):
+        """examples: n >= 1 serialized Examples -> their device views (prob f32 [outputs * n], err int64 [1], extra
+        uint8, offsets int64 [n+1], data uint8).  Raises ValueError for an Example of 2^31 bytes or more."""
         n = len(examples)
         lens = np.fromiter(map(len, examples), dtype=np.int64, count=n)
         if int(lens.max()) >= 1 << 31:
             raise ValueError(f"example {int(np.argmax(lens >= 1 << 31))}: an Example of 2^31 bytes or more")
-        self._n, self._e = n, (4 * n + 7) & ~7
+        self._n, self._e = outputs * n, (4 * outputs * n + 7) & ~7
         self._back = self._e + 8 + extra
         head = self._back + 8 * (n + 1)
         total = head + int(lens.sum())
@@ -94,12 +104,12 @@ class _Requests:
         np.cumsum(lens, out=off[1:])
         h[head:total] = np.frombuffer(b"".join(examples), dtype=np.uint8)
         dev[e:total].copy_(self._host[e:total], non_blocking=True)
-        return (dev[:4 * n].view(torch.float32), dev[e:e + 8].view(torch.int64), dev[e + 8:self._back],
+        return (dev[:4 * self._n].view(torch.float32), dev[e:e + 8].view(torch.int64), dev[e + 8:self._back],
                 dev[self._back:head].view(torch.int64), dev[head:total])
 
     def receive(self):
-        """-> (prob f32 [n], the error word's (example, check, arg) or None, extra uint8), host views valid until the
-        next send"""
+        """-> (prob f32 [outputs * n], the error word's (example, check, arg) or None, extra uint8), host views valid
+        until the next send"""
         self._host[:self._back].copy_(self._dev[:self._back], non_blocking=True)
         torch.cuda.current_stream(self.device).synchronize()
         h, e = self._host.numpy(), self._e
@@ -286,6 +296,130 @@ class DINServable:
             if not todo:
                 return p.copy()
             self._grow(int(mx[todo, 0].max()), int(mx[todo, 1].max()))
+
+
+ESMM_OUTPUTS = ("pctr", "pcvr", "pctcvr")       # PredictOutput of DeepCvrMTL.py:210-217
+
+
+class ESMMServable:
+    """serving_default of a trained ESMM (DeepCvrMTL.py:210-217, DESIGN.md §2.14): serialized tf.Examples with the
+    training schema of DeepCvrMTL.py:66-83 (labels not read) in, pctr / pcvr / pctcvr out.  Per request: one pinned
+    host->device copy (error word, occurrence totals, offsets and bytes); per slice of at most max_batch Examples
+    ctr_esmm_serve_scan, ctr_tfrecord_emit_esmm and ESMM.predict; one device->host copy (the three outputs, error word,
+    out-of-range id counter, occurrence totals) after the only synchronisation.  A slice whose bag occurrences outgrow
+    the occurrence buffers is run again after ESMM.grow, which costs a second round trip.  Growth is permanent.  A
+    failed growth (out of memory) raises and leaves the servable as it was."""
+
+    def __init__(self, model):
+        self.model = model
+        self._requests = _Requests(model.device)
+        self._commit_batch(self._alloc_batch(model.cap))
+
+    @classmethod
+    def load(cls, model_dir: str, field_size: int, feature_size: int, embedding_size: int,
+             deep_layers: str = "256,128,64", batch_norm: bool = False, batch_norm_decay: float = 0.9,
+             max_batch: int = 4096, device="cuda", occ_capacity: Optional[int] = None,
+             checkpoint_format: str = "b200") -> "ESMMServable":
+        """model_dir as `DeepCvrMTL.py --task_type=train` leaves it (ctr_b200.ckpt), or with checkpoint_format="tf" a
+        TensorFlow bundle written by tf_checkpoint.save.  The hyperparameters are DeepCvrMTL.py's flags of the same
+        names.  occ_capacity: the starting bag-occurrence capacity per slice; default the one esmm_shapes.json in
+        model_dir records."""
+        from .esmm import ESMM
+        from .estimator import _ckpt_path
+        if checkpoint_format not in ("b200", "tf"):
+            raise ValueError(f"checkpoint_format={checkpoint_format!r}: must be one of {{b200, tf}}")
+        if occ_capacity is None:
+            meta = os.path.join(model_dir, "esmm_shapes.json")
+            if not os.path.exists(meta):
+                raise ValueError(f"{meta} does not exist: pass occ_capacity")
+            occ_capacity = int(json.load(open(meta))["occ_capacity"])
+        model = ESMM(field_size, feature_size, embedding_size, max_batch, occ_capacity, deep_layers=deep_layers,
+                     update_mode="lazy", device=device, batch_norm=batch_norm, batch_norm_decay=batch_norm_decay)
+        if checkpoint_format == "tf":
+            from . import tf_checkpoint
+            tf_checkpoint.restore(model, model_dir, variables_only=True)
+        else:
+            path = _ckpt_path(model_dir)
+            if not os.path.exists(path):
+                raise FileNotFoundError(f"{path} does not exist")
+            model.load_variables(torch.load(path, map_location="cpu")["variables"])
+        return cls(model)
+
+    def _alloc_batch(self, cap: int) -> dict:
+        """the emit's buffers for slices of up to cap bag occurrences; committed by the caller"""
+        m = self.model
+        B, F, dev = m.B, m.Fp, m.device
+        i32 = dict(dtype=torch.int32, device=dev)
+        return {"slot_off": torch.empty(B, dtype=torch.int64, device=dev), "slot_len": torch.empty(B, **i32),
+                "labels": torch.empty(2, B, dtype=torch.float32, device=dev),   # absorbs the emit's y and z
+                "batch": {"feat_ids": torch.empty(B, F, **i32), "a_ids": torch.empty(3, B, **i32),
+                          "bag_ids": torch.empty(cap, **i32), "bag_wgt": torch.empty(cap, dtype=torch.float32, device=dev),
+                          "bag_off": torch.empty(5 * B + 1, **i32)}}
+
+    def _commit_batch(self, bufs: dict):
+        self._slot_off, self._slot_len, self._labels, self._batch = (bufs["slot_off"], bufs["slot_len"], bufs["labels"],
+                                                                     bufs["batch"])
+
+    def _grow(self, cap: int):
+        """model and emit buffers for cap occurrences, or neither: the emit buffers are allocated first, and ESMM.grow
+        allocates nothing"""
+        bufs = self._alloc_batch(max(cap, self.model.cap))
+        self.model.grow(cap)
+        self._commit_batch(bufs)
+
+    def _run(self, data, off, lo: int, hi: int, err, total, out):
+        m, bt = self.model, self._batch
+        # the emit writes up to m.cap occurrences (the scan empties a slice's bags past it): never past these tensors
+        if bt["bag_ids"].numel() != m.cap or bt["bag_wgt"].numel() != m.cap:
+            raise RuntimeError(f"ESMMServable: occurrence buffers of {bt['bag_ids'].numel()} do not match the model's "
+                               f"occ_capacity={m.cap}")
+        ops.esmm_serve_scan(data, off[lo:hi + 1], lo, m.Fp, m.B, m.cap, self._slot_off, self._slot_len,
+                            bt["bag_off"], total, err)
+        ops.tfrecord_emit_esmm(data, self._slot_off, self._slot_len, m.B, m.Fp, bt["bag_off"], bt["feat_ids"],
+                               bt["a_ids"], bt["bag_ids"], bt["bag_wgt"], self._labels[0], self._labels[1])
+        for o, p in zip(out, m.predict(bt)):
+            o[lo:hi].copy_(p[:hi - lo])
+
+    def predict(self, examples) -> Dict[str, np.ndarray]:
+        """examples: the serialized tf.Examples of the request (a sequence of bytes) -> {"pctr", "pcvr", "pctcvr"},
+        each float32 [n].  Raises ValueError naming the first rejected Example (its index in the whole request) and
+        the check."""
+        n = len(examples)
+        if n == 0:
+            return {k: np.zeros(0, dtype=np.float32) for k in ESMM_OUTPUTS}
+        m = self.model
+        slices = [(lo, min(lo + m.B, n)) for lo in range(0, n, m.B)]
+        S = len(slices)
+        # extra: the model's out-of-range id counter int32 [2], then each slice's occurrence total int64 [S]
+        out, err, extra, off, data = self._requests.send(examples, 8 + 8 * S, outputs=len(ESMM_OUTPUTS))
+        out = out.view(len(ESMM_OUTPUTS), n)
+        oob, totals = extra[:8].view(torch.int32), extra[8:].view(torch.int64)
+        todo = list(range(S))
+        while True:
+            cap = m.cap
+            for s in todo:
+                self._run(data, off, *slices[s], err, totals[s:s + 1], out)
+            oob.copy_(m.oob)
+            p, error, h_extra = self._requests.receive()
+            n_oob = int(h_extra[:4].view(np.int32)[0])
+            if error is not None or n_oob:
+                m.oob.zero_()
+                ex = error[0] if error is not None else n
+                msg = din_id_range_error(examples, ex, m.N)       # DIN's schema: the same keys, ids and checks
+                if msg is None and error is not None:
+                    msg = din_error_message(*error, m.Fp)
+                raise ValueError(msg or f"an id outside [0, feature_size={m.N})")
+            tot = h_extra[8:].view(np.int64)
+            todo = [s for s in todo if tot[s] > cap]
+            if not todo:
+                p = p.reshape(len(ESMM_OUTPUTS), n)
+                return {k: p[i].copy() for i, k in enumerate(ESMM_OUTPUTS)}
+            need = int(tot[todo].max())
+            if need >= 1 << 31:
+                s = todo[int(np.argmax(tot[todo]))]
+                raise ValueError(f"examples {slices[s][0]}..{slices[s][1] - 1}: {need} bag occurrences in one slice of "
+                                 f"max_batch={m.B} Examples, more than 2^31 - 1")
+            self._grow(need)
 
 
 class Servable:
