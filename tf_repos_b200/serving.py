@@ -127,7 +127,9 @@ _WD_CHECKS = {1: "malformed tf.Example protobuf", 2: "required key {key!r} is mi
 class WideDeepServable:
     """serving_default of an exported wide_n_deep: serialized tf.Examples in, the binary head's classification out.
     Per request: one pinned host->device copy (error word, offsets and bytes), the parse + feature-column kernel and
-    the MLP per slice of at most max_batch Examples, one device->host copy (probabilities and error word)."""
+    the MLP per slice of at most max_batch Examples, one device->host copy (probabilities and error word).  It keeps
+    its own loop: the columns map every id into range and its buffers never grow, so it has none of the out-of-range
+    counter, per-slice records and growth that _DINSchemaServable's loop is built around."""
 
     def __init__(self, model):
         self.model = model
@@ -180,39 +182,86 @@ _DIN_ID_KEYS = (("feat_ids", None), ("a_catids", 1), ("a_shopids", 1), ("a_brand
     tuple(("u_%sids" % u, None) for u in _DIN_U)
 
 
-def din_error_message(index: int, check: int, arg: int, F: int) -> str:
-    """ValueError text of the DIN serving check `check` (ctr_din_serve_scan's numbering) on Example `index`"""
-    key = _DIN_KEYS[arg]
-    kind = "float_list" if key.endswith("vals") else "int64_list"
-    return f"example {index}: " + _DIN_CHECKS[check].format(key=key, F=F, u=_DIN_U[arg % 4], kind=kind)
+class _DINSchemaServable:
+    """The request loop of DINServable and ESMMServable, whose requests are serialized tf.Examples with DIN's training
+    schema (ESMM's adds the label z, and serving reads neither label), so the checks and their messages are the same
+    (DESIGN.md §2.10).  Per request: one pinned host->device copy (error word, extra, offsets, bytes); per slice of at
+    most max_batch Examples `parse` and the model's predict; one device->host copy (outputs, error word, extra) after
+    the only synchronisation.  extra is the model's out-of-range id counter int32 [2], then one 8-byte record per slice
+    from the scan.  A slice whose record (`_need`) exceeds the model's `_capacity()` is run again after `_grow`, a
+    second round trip.  Growth is permanent; a failed growth (out of memory) raises and leaves the servable as it was.
 
+    A subclass supplies OUTPUTS, `_capacity`, `_alloc`, `parse`, `_predict`, `_need` (host records uint8 [S, 8] -> each
+    slice's sizes [S, len(_capacity())]) and `_result` (host outputs float32 [OUTPUTS * n] -> predict's value)."""
 
-def din_id_range_error(examples, upto: int, N: int):
-    """the message for the first of examples[:upto] (all passing the parse checks) whose read ids reach feature_size N,
-    or None"""
-    from .tfrecord import parse_example
-    for i in range(upto):
-        ex = parse_example(examples[i])
-        for key, first in _DIN_ID_KEYS:
-            v = np.asarray(ex.get(key, []), dtype=np.int64)[:first]
-            if len(v) and int(v.max()) >= N:
-                return f"example {i}: key {key!r} holds an id outside [0, feature_size={N})"
-    return None
-
-
-class DINServable:
-    """serving_default of an exported DIN (DIN.py:385-397, DESIGN.md §2.10): serialized tf.Examples with the training
-    schema of DIN.py:60-77 (labels not read) in, prob out.  Per request: one pinned host->device copy (error word,
-    maxima, offsets and bytes); per slice of at most max_batch Examples ctr_din_serve_scan, ctr_tfrecord_emit_din and
-    DIN.predict; one device->host copy (probabilities, error word, out-of-range id counter, maxima) after the only
-    synchronisation.  A slice whose behaviour lists or a_int bags outgrow the model's buffers is run again after
-    DIN.grow, which costs a second round trip.  Growth is permanent: later requests run the forward at the larger P.
-    A failed growth (out of memory) raises and leaves the servable as it was."""
+    OUTPUTS = 1                 # float32 outputs per Example
 
     def __init__(self, model):
         self.model = model
         self._requests = _Requests(model.device)
-        self._commit_batch(self._alloc_batch(model.P, model.max_a_int))
+        self._scratch, self._batch = self._alloc(*self._capacity())
+
+    def _grow(self, need):
+        """model and emit buffers for the sizes `need`, or neither: the emit buffers are allocated first, and the
+        model's grow changes nothing until all of its own allocations succeeded"""
+        bufs = self._alloc(*map(max, need, self._capacity()))
+        self.model.grow(*need)
+        self._scratch, self._batch = bufs
+
+    def _rejection(self, examples, error) -> str:
+        """error: the device's first error word as (example, check, arg), or None when only the model's out-of-range
+        counter is set -> the ValueError text.  An id >= feature_size is found by the host parser among the Examples
+        before the device's first error, so the text names the first rejected Example of the whole request."""
+        from .tfrecord import parse_example
+        m = self.model
+        for i in range(len(examples) if error is None else error[0]):
+            ex = parse_example(examples[i])
+            for key, first in _DIN_ID_KEYS:
+                v = np.asarray(ex.get(key, []), dtype=np.int64)[:first]
+                if len(v) and int(v.max()) >= m.N:
+                    return f"example {i}: key {key!r} holds an id outside [0, feature_size={m.N})"
+        if error is None:
+            return f"an id outside [0, feature_size={m.N})"
+        index, check, arg = error
+        key = _DIN_KEYS[arg]
+        kind = "float_list" if key.endswith("vals") else "int64_list"
+        return f"example {index}: " + _DIN_CHECKS[check].format(key=key, F=m.Fp, u=_DIN_U[arg % 4], kind=kind)
+
+    def predict(self, examples):
+        """examples: the serialized tf.Examples of the request (a sequence of bytes) -> DIN: prob float32 [n]; ESMM:
+        {"pctr", "pcvr", "pctcvr"}, each float32 [n].  Raises ValueError naming the first rejected Example (its index
+        in the whole request) and the check."""
+        n, m, k = len(examples), self.model, self.OUTPUTS
+        if n == 0:
+            return self._result(np.zeros(0, dtype=np.float32))
+        slices = [(lo, min(lo + m.B, n)) for lo in range(0, n, m.B)]
+        S = len(slices)
+        out, err, extra, off, data = self._requests.send(examples, 8 + 8 * S, outputs=k)
+        oob, rec = extra[:8].view(torch.int32), extra[8:].view(S, 8)
+        todo = range(S)
+        while True:
+            for s in todo:
+                lo, hi = slices[s]
+                for i, y in enumerate(self._predict(self.parse(data, off[lo:hi + 1], lo, err, rec[s]))):
+                    out[i * n + lo:i * n + hi].copy_(y[:hi - lo])
+            oob.copy_(m.oob)
+            p, error, h_extra = self._requests.receive()
+            if error is not None or int(h_extra[:4].view(np.int32)[0]):
+                m.oob.zero_()
+                raise ValueError(self._rejection(examples, error))
+            need, cap = self._need(h_extra[8:].reshape(S, 8), slices).tolist(), self._capacity()
+            todo = [s for s in todo if any(a > c for a, c in zip(need[s], cap))]
+            if not todo:
+                return self._result(p)
+            self._grow([max(sizes) for sizes in zip(*(need[s] for s in todo))])
+
+
+class DINServable(_DINSchemaServable):
+    """serving_default of an exported DIN (DIN.py:385-397, DESIGN.md §2.10): serialized tf.Examples with the training
+    schema of DIN.py:60-77 (labels not read) in, prob out, through ctr_din_serve_scan, ctr_tfrecord_emit_din and
+    DIN.predict per slice.  A slice's record is int32 (longest behaviour list, longest a_int bag); a slice whose lists
+    or bags outgrow the model's P / max_a_int is run again after DIN.grow.  Later requests run the forward at the
+    larger P."""
 
     @classmethod
     def load(cls, export_dir: str, max_batch: int = 4096, device="cuda", max_len: int = 64,
@@ -230,90 +279,55 @@ class DINServable:
         model.load_variables(torch.load(os.path.join(export_dir, "variables.pt"), map_location="cpu"))
         return cls(model)
 
-    def _alloc_batch(self, P: int, A: int) -> dict:
-        """the emit's buffers for behaviour lists up to P and a_int bags up to A; committed by the caller"""
+    def _capacity(self):
+        return self.model.P, self.model.max_a_int
+
+    def _alloc(self, P: int, A: int):
+        """(scan scratch, batch): the buffers for behaviour lists up to P and a_int bags up to A"""
         m = self.model
         B, F, dev = m.B, m.Fp, m.device
         i32 = dict(dtype=torch.int32, device=dev)
-        return {"slot_off": torch.empty(B, dtype=torch.int64, device=dev), "slot_len": torch.empty(B, **i32),
-                "y": torch.empty(B, dtype=torch.float32, device=dev),          # absorbs the emit's label
-                "batch": {"feat_ids": torch.empty(B, F, **i32), "a_ids": torch.empty(3, B, **i32),
-                          "a_int_ids": torch.empty(B * A, **i32), "a_int_off": torch.empty(B + 1, **i32),
-                          "u_ids": torch.empty(4, B, P, **i32),
-                          "u_wgt": torch.empty(4, B, P, dtype=torch.float32, device=dev)}}
+        return ({"slot_off": torch.empty(B, dtype=torch.int64, device=dev), "slot_len": torch.empty(B, **i32),
+                 "y": torch.empty(B, dtype=torch.float32, device=dev)},         # absorbs the emit's label
+                {"feat_ids": torch.empty(B, F, **i32), "a_ids": torch.empty(3, B, **i32),
+                 "a_int_ids": torch.empty(B * A, **i32), "a_int_off": torch.empty(B + 1, **i32),
+                 "u_ids": torch.empty(4, B, P, **i32), "u_wgt": torch.empty(4, B, P, dtype=torch.float32, device=dev)})
 
-    def _commit_batch(self, bufs: dict):
-        self._slot_off, self._slot_len, self._y, self._batch = bufs["slot_off"], bufs["slot_len"], bufs["y"], bufs["batch"]
-
-    def _grow(self, P: int, A: int):
-        """model and emit buffers for (P, A), or neither: the emit buffers are allocated first, and DIN.grow only
-        changes the model once all of its own allocations succeeded"""
-        bufs = self._alloc_batch(max(P, self.model.P), max(A, self.model.max_a_int))
-        self.model.grow(P, A)
-        self._commit_batch(bufs)
-
-    def _run(self, data, off, lo: int, hi: int, err, maxima, pred):
-        m, bt = self.model, self._batch
+    def parse(self, data, off, lo: int, err, rec) -> Dict[str, torch.Tensor]:
+        """One slice: the serialized Examples data[off[b], off[b+1]) (uint8, off int64 [n+1], n <= max_batch),
+        Example lo + b of the request -> DIN.predict's batch, in the servable's buffers.  err int64 [1] (~0 = none)
+        and rec uint8 [8] (int32 longest behaviour list, longest a_int bag; zeroed by the caller) are folded into."""
+        m, sc, bt = self.model, self._scratch, self._batch
         # the emit writes u_ids / u_wgt at stride P and up to B * max_a_int a_int ids: never past these tensors
         if bt["u_ids"].shape[2] != m.P or bt["a_int_ids"].numel() != m.B * m.max_a_int:
             raise RuntimeError(f"DINServable: batch buffers {tuple(bt['u_ids'].shape)} / {bt['a_int_ids'].numel()} do "
                                f"not match the model's P={m.P}, max_a_int={m.max_a_int}")
-        ops.din_serve_scan(data, off[lo:hi + 1], lo, m.Fp, m.B, m.max_a_int, self._slot_off, self._slot_len,
-                           bt["a_int_off"], maxima, err)
-        ops.tfrecord_emit_din(data, self._slot_off, self._slot_len, m.B, m.Fp, m.P, bt["a_int_off"], bt["feat_ids"],
-                              bt["a_ids"], bt["a_int_ids"], bt["u_ids"], bt["u_wgt"], self._y)
-        pred[lo:hi].copy_(m.predict(bt)[:hi - lo])
+        ops.din_serve_scan(data, off, lo, m.Fp, m.B, m.max_a_int, sc["slot_off"], sc["slot_len"], bt["a_int_off"],
+                           rec.view(torch.int32), err)
+        ops.tfrecord_emit_din(data, sc["slot_off"], sc["slot_len"], m.B, m.Fp, m.P, bt["a_int_off"], bt["feat_ids"],
+                              bt["a_ids"], bt["a_int_ids"], bt["u_ids"], bt["u_wgt"], sc["y"])
+        return bt
 
-    def predict(self, examples) -> np.ndarray:
-        """examples: the serialized tf.Examples of the request (a sequence of bytes) -> prob float32 [n].  Raises
-        ValueError naming the first rejected Example (its index in the whole request) and the check."""
-        n = len(examples)
-        if n == 0:
-            return np.zeros(0, dtype=np.float32)
-        m = self.model
-        slices = [(lo, min(lo + m.B, n)) for lo in range(0, n, m.B)]
-        S = len(slices)
-        # extra: the model's out-of-range id counter int32 [2], then maxima int32 [S, 2]
-        pred, err, extra, off, data = self._requests.send(examples, 8 + 8 * S)
-        oob, maxima = extra[:8].view(torch.int32), extra[8:].view(torch.int32).view(S, 2)
-        todo = list(range(S))
-        while True:
-            P, A = m.P, m.max_a_int
-            for s in todo:
-                self._run(data, off, *slices[s], err, maxima[s], pred)
-            oob.copy_(m.oob)
-            p, error, h_extra = self._requests.receive()
-            n_oob = int(h_extra[:4].view(np.int32)[0])
-            if error is not None or n_oob:
-                m.oob.zero_()
-                ex = error[0] if error is not None else n
-                msg = din_id_range_error(examples, ex, m.N)
-                if msg is None and error is not None:
-                    msg = din_error_message(*error, m.Fp)
-                raise ValueError(msg or f"an id outside [0, feature_size={m.N})")
-            mx = h_extra[8:].view(np.int32).reshape(S, 2)
-            todo = [s for s in todo if mx[s, 0] > P or mx[s, 1] > A]
-            if not todo:
-                return p.copy()
-            self._grow(int(mx[todo, 0].max()), int(mx[todo, 1].max()))
+    def _predict(self, batch):
+        return (self.model.predict(batch),)
+
+    def _need(self, rec, slices):
+        return rec.view(np.int32)
+
+    def _result(self, p):
+        return p.copy()
 
 
 ESMM_OUTPUTS = ("pctr", "pcvr", "pctcvr")       # PredictOutput of DeepCvrMTL.py:210-217
 
 
-class ESMMServable:
+class ESMMServable(_DINSchemaServable):
     """serving_default of a trained ESMM (DeepCvrMTL.py:210-217, DESIGN.md §2.14): serialized tf.Examples with the
-    training schema of DeepCvrMTL.py:66-83 (labels not read) in, pctr / pcvr / pctcvr out.  Per request: one pinned
-    host->device copy (error word, occurrence totals, offsets and bytes); per slice of at most max_batch Examples
-    ctr_esmm_serve_scan, ctr_tfrecord_emit_esmm and ESMM.predict; one device->host copy (the three outputs, error word,
-    out-of-range id counter, occurrence totals) after the only synchronisation.  A slice whose bag occurrences outgrow
-    the occurrence buffers is run again after ESMM.grow, which costs a second round trip.  Growth is permanent.  A
-    failed growth (out of memory) raises and leaves the servable as it was."""
+    training schema of DeepCvrMTL.py:66-83 (labels not read) in, pctr / pcvr / pctcvr out, through
+    ctr_esmm_serve_scan, ctr_tfrecord_emit_esmm and ESMM.predict per slice.  A slice's record is its int64 bag
+    occurrence total; a slice past the occurrence capacity is run again after ESMM.grow."""
 
-    def __init__(self, model):
-        self.model = model
-        self._requests = _Requests(model.device)
-        self._commit_batch(self._alloc_batch(model.cap))
+    OUTPUTS = len(ESMM_OUTPUTS)
 
     @classmethod
     def load(cls, model_dir: str, field_size: int, feature_size: int, embedding_size: int,
@@ -345,81 +359,50 @@ class ESMMServable:
             model.load_variables(torch.load(path, map_location="cpu")["variables"])
         return cls(model)
 
-    def _alloc_batch(self, cap: int) -> dict:
-        """the emit's buffers for slices of up to cap bag occurrences; committed by the caller"""
+    def _capacity(self):
+        return (self.model.cap,)
+
+    def _alloc(self, cap: int):
+        """(scan scratch, batch): the buffers for slices of up to cap bag occurrences; ESMM.grow allocates nothing"""
         m = self.model
         B, F, dev = m.B, m.Fp, m.device
         i32 = dict(dtype=torch.int32, device=dev)
-        return {"slot_off": torch.empty(B, dtype=torch.int64, device=dev), "slot_len": torch.empty(B, **i32),
-                "labels": torch.empty(2, B, dtype=torch.float32, device=dev),   # absorbs the emit's y and z
-                "batch": {"feat_ids": torch.empty(B, F, **i32), "a_ids": torch.empty(3, B, **i32),
-                          "bag_ids": torch.empty(cap, **i32), "bag_wgt": torch.empty(cap, dtype=torch.float32, device=dev),
-                          "bag_off": torch.empty(5 * B + 1, **i32)}}
+        return ({"slot_off": torch.empty(B, dtype=torch.int64, device=dev), "slot_len": torch.empty(B, **i32),
+                 "labels": torch.empty(2, B, dtype=torch.float32, device=dev)},    # absorbs the emit's y and z
+                {"feat_ids": torch.empty(B, F, **i32), "a_ids": torch.empty(3, B, **i32),
+                 "bag_ids": torch.empty(cap, **i32), "bag_wgt": torch.empty(cap, dtype=torch.float32, device=dev),
+                 "bag_off": torch.empty(5 * B + 1, **i32)})
 
-    def _commit_batch(self, bufs: dict):
-        self._slot_off, self._slot_len, self._labels, self._batch = (bufs["slot_off"], bufs["slot_len"], bufs["labels"],
-                                                                     bufs["batch"])
-
-    def _grow(self, cap: int):
-        """model and emit buffers for cap occurrences, or neither: the emit buffers are allocated first, and ESMM.grow
-        allocates nothing"""
-        bufs = self._alloc_batch(max(cap, self.model.cap))
-        self.model.grow(cap)
-        self._commit_batch(bufs)
-
-    def _run(self, data, off, lo: int, hi: int, err, total, out):
-        m, bt = self.model, self._batch
+    def parse(self, data, off, lo: int, err, rec) -> Dict[str, torch.Tensor]:
+        """One slice: the serialized Examples data[off[b], off[b+1]) (uint8, off int64 [n+1], n <= max_batch),
+        Example lo + b of the request -> ESMM.predict's batch, in the servable's buffers.  err int64 [1] (~0 = none)
+        is folded into; rec uint8 [8] receives the slice's int64 occurrence total (its bags are empty past the
+        capacity)."""
+        m, sc, bt = self.model, self._scratch, self._batch
         # the emit writes up to m.cap occurrences (the scan empties a slice's bags past it): never past these tensors
         if bt["bag_ids"].numel() != m.cap or bt["bag_wgt"].numel() != m.cap:
             raise RuntimeError(f"ESMMServable: occurrence buffers of {bt['bag_ids'].numel()} do not match the model's "
                                f"occ_capacity={m.cap}")
-        ops.esmm_serve_scan(data, off[lo:hi + 1], lo, m.Fp, m.B, m.cap, self._slot_off, self._slot_len,
-                            bt["bag_off"], total, err)
-        ops.tfrecord_emit_esmm(data, self._slot_off, self._slot_len, m.B, m.Fp, bt["bag_off"], bt["feat_ids"],
-                               bt["a_ids"], bt["bag_ids"], bt["bag_wgt"], self._labels[0], self._labels[1])
-        for o, p in zip(out, m.predict(bt)):
-            o[lo:hi].copy_(p[:hi - lo])
+        ops.esmm_serve_scan(data, off, lo, m.Fp, m.B, m.cap, sc["slot_off"], sc["slot_len"], bt["bag_off"],
+                            rec.view(torch.int64), err)
+        ops.tfrecord_emit_esmm(data, sc["slot_off"], sc["slot_len"], m.B, m.Fp, bt["bag_off"], bt["feat_ids"],
+                               bt["a_ids"], bt["bag_ids"], bt["bag_wgt"], sc["labels"][0], sc["labels"][1])
+        return bt
 
-    def predict(self, examples) -> Dict[str, np.ndarray]:
-        """examples: the serialized tf.Examples of the request (a sequence of bytes) -> {"pctr", "pcvr", "pctcvr"},
-        each float32 [n].  Raises ValueError naming the first rejected Example (its index in the whole request) and
-        the check."""
-        n = len(examples)
-        if n == 0:
-            return {k: np.zeros(0, dtype=np.float32) for k in ESMM_OUTPUTS}
-        m = self.model
-        slices = [(lo, min(lo + m.B, n)) for lo in range(0, n, m.B)]
-        S = len(slices)
-        # extra: the model's out-of-range id counter int32 [2], then each slice's occurrence total int64 [S]
-        out, err, extra, off, data = self._requests.send(examples, 8 + 8 * S, outputs=len(ESMM_OUTPUTS))
-        out = out.view(len(ESMM_OUTPUTS), n)
-        oob, totals = extra[:8].view(torch.int32), extra[8:].view(torch.int64)
-        todo = list(range(S))
-        while True:
-            cap = m.cap
-            for s in todo:
-                self._run(data, off, *slices[s], err, totals[s:s + 1], out)
-            oob.copy_(m.oob)
-            p, error, h_extra = self._requests.receive()
-            n_oob = int(h_extra[:4].view(np.int32)[0])
-            if error is not None or n_oob:
-                m.oob.zero_()
-                ex = error[0] if error is not None else n
-                msg = din_id_range_error(examples, ex, m.N)       # DIN's schema: the same keys, ids and checks
-                if msg is None and error is not None:
-                    msg = din_error_message(*error, m.Fp)
-                raise ValueError(msg or f"an id outside [0, feature_size={m.N})")
-            tot = h_extra[8:].view(np.int64)
-            todo = [s for s in todo if tot[s] > cap]
-            if not todo:
-                p = p.reshape(len(ESMM_OUTPUTS), n)
-                return {k: p[i].copy() for i, k in enumerate(ESMM_OUTPUTS)}
-            need = int(tot[todo].max())
-            if need >= 1 << 31:
-                s = todo[int(np.argmax(tot[todo]))]
-                raise ValueError(f"examples {slices[s][0]}..{slices[s][1] - 1}: {need} bag occurrences in one slice of "
-                                 f"max_batch={m.B} Examples, more than 2^31 - 1")
-            self._grow(need)
+    def _predict(self, batch):
+        return self.model.predict(batch)
+
+    def _need(self, rec, slices):
+        tot = rec.view(np.int64)
+        s = int(np.argmax(tot))
+        if tot[s, 0] > max(self.model.cap, (1 << 31) - 1):        # outgrown, and past the int32 CSR offsets
+            raise ValueError(f"examples {slices[s][0]}..{slices[s][1] - 1}: {int(tot[s, 0])} bag occurrences in one "
+                             f"slice of max_batch={self.model.B} Examples, more than 2^31 - 1")
+        return tot
+
+    def _result(self, p):
+        p = p.reshape(len(ESMM_OUTPUTS), -1)
+        return {k: p[i].copy() for i, k in enumerate(ESMM_OUTPUTS)}
 
 
 class Servable:

@@ -8,9 +8,9 @@ of U{1..8} ids.  The servable's buffers start at P = 100 and max_a_int = 8, so n
 
   latency     wall clock around predict (host -> device copy, kernels, device -> host copy, the one synchronise) per
               request after a warm-up of every size: median and p99 for n in --sizes
-  device      parse = ctr_din_serve_scan + ctr_tfrecord_emit_din, model = DIN.predict on the emitted batch: device time
-              from torch.profiler (CUDA activity only, in a phase of its own) per slice.  DIN.predict always runs the
-              full max_batch rows, so the model time does not shrink with n
+  device      parse = DINServable.parse (the scan and emit kernels), model = DIN.predict on the emitted batch: device
+              time from torch.profiler (CUDA activity only, in a phase of its own) per slice.  DIN.predict always runs
+              the full max_batch rows, so the model time does not shrink with n
   throughput  Examples/s of predict at each n (n / median latency)
 """
 from __future__ import annotations
@@ -64,7 +64,6 @@ def main():
     ap.add_argument("--out", default="din_serving.json")
     a = ap.parse_args()
     assert torch.cuda.is_available(), "bench_din_serving measures on a GPU"
-    from tf_repos_b200 import ops
     from tf_repos_b200.din import DIN
     from tf_repos_b200.serving import DINServable
 
@@ -102,15 +101,11 @@ def main():
         off = torch.tensor(np.concatenate([[0], np.cumsum(lens)]), dtype=torch.int64, device="cuda:0")
         data = torch.tensor(np.frombuffer(b"".join(ex), dtype=np.uint8), device="cuda:0")
         err = torch.full((1,), -1, dtype=torch.int64, device="cuda:0")
-        maxima = torch.zeros(2, dtype=torch.int32, device="cuda:0")
-        bt = s._batch
-
-        def parse():
-            ops.din_serve_scan(data, off, 0, F, B, A, s._slot_off, s._slot_len, bt["a_int_off"], maxima, err)
-            ops.tfrecord_emit_din(data, s._slot_off, s._slot_len, B, F, P, bt["a_int_off"], bt["feat_ids"],
-                                  bt["a_ids"], bt["a_int_ids"], bt["u_ids"], bt["u_wgt"], s._y)
+        rec = torch.zeros(8, dtype=torch.uint8, device="cuda:0")        # the slice's maxima int32 [2]
+        bt = s.parse(data, off, 0, err, rec)
         reps = 50
-        d = {"parse": _kernel_ms(parse, reps), "model": _kernel_ms(lambda: m.predict(bt), reps),
+        d = {"parse": _kernel_ms(lambda: s.parse(data, off, 0, err, rec), reps),
+             "model": _kernel_ms(lambda: m.predict(bt), reps),
              "request_bytes": int(lens.sum())}
         assert int(err.item()) == -1
         d["parse_over_model"] = d["parse"] / d["model"]

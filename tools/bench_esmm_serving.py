@@ -9,9 +9,9 @@ max_batch x the longest possible Example (654 occurrences), so no request grows 
 
   latency     wall clock around predict (host -> device copy, kernels, device -> host copy, the one synchronise) per
               request after a warm-up of every size: median and p99 for n in --sizes
-  device      parse = ctr_esmm_serve_scan (scan, one-CTA offset scan, capacity clamp) + ctr_tfrecord_emit_esmm, model =
-              ESMM.predict on the emitted batch: device time from torch.profiler (CUDA activity only, in a phase of its
-              own) per slice.  ESMM.predict always runs the full max_batch rows, so the model time does not shrink with
+  device      parse = ESMMServable.parse (scan, one-CTA offset scan, capacity clamp, emit), model = ESMM.predict on
+              the emitted batch: device time from torch.profiler (CUDA activity only, in a phase of its own) per
+              slice.  ESMM.predict always runs the full max_batch rows, so the model time does not shrink with
               n; its bag sums do, with the padding slots repeating Example 0
   throughput  Examples/s of predict at each n (n / median latency)
 """
@@ -68,7 +68,6 @@ def main():
     ap.add_argument("--out", default="esmm_serving.json")
     a = ap.parse_args()
     assert torch.cuda.is_available(), "bench_esmm_serving measures on a GPU"
-    from tf_repos_b200 import ops
     from tf_repos_b200.esmm import ESMM
     from tf_repos_b200.serving import ESMMServable
 
@@ -108,16 +107,12 @@ def main():
         off = torch.tensor(np.concatenate([[0], np.cumsum(lens)]), dtype=torch.int64, device="cuda:0")
         data = torch.tensor(np.frombuffer(b"".join(ex), dtype=np.uint8), device="cuda:0")
         err = torch.full((1,), -1, dtype=torch.int64, device="cuda:0")
-        total = torch.zeros(1, dtype=torch.int64, device="cuda:0")
-        bt = s._batch
-
-        def parse():
-            ops.esmm_serve_scan(data, off, 0, F, B, cap, s._slot_off, s._slot_len, bt["bag_off"], total, err)
-            ops.tfrecord_emit_esmm(data, s._slot_off, s._slot_len, B, F, bt["bag_off"], bt["feat_ids"], bt["a_ids"],
-                                   bt["bag_ids"], bt["bag_wgt"], s._labels[0], s._labels[1])
+        rec = torch.zeros(8, dtype=torch.uint8, device="cuda:0")
+        total = rec.view(torch.int64)                                  # the slice's occurrence total
+        bt = s.parse(data, off, 0, err, rec)
         reps = 50
-        d = {"parse": _kernel_ms(parse, reps), "model": _kernel_ms(lambda: m.predict(bt), reps),
-             "request_bytes": int(lens.sum())}
+        d = {"parse": _kernel_ms(lambda: s.parse(data, off, 0, err, rec), reps),
+             "model": _kernel_ms(lambda: m.predict(bt), reps), "request_bytes": int(lens.sum())}
         assert int(err.item()) == -1 and int(total.item()) <= cap
         d["occurrences"] = int(total.item())
         d["parse_over_model"] = d["parse"] / d["model"]
